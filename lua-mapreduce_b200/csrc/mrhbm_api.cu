@@ -7,6 +7,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <initializer_list>
 #include <map>
 #include <mutex>
 #include <string>
@@ -25,7 +26,7 @@ enum { R_OPEN = 0, R_COMMITTED = 1, R_DEAD = 2 };
 constexpr uint32_t kErrfLongKeys = 0x80000000u;  // rides on the error-flag all-gather of a multi-GPU shuffle: this rank holds long keys
 constexpr size_t kMaxLongKey = 1u << 20;  // bytes; longer keys are refused (MRHBM_E_KEY)
 struct LongPair {
-  std::string esc;  // the key as a record slot would hold it: 0x00 / 0x01 escaped (order preserving, see mrhbm_emit_str)
+  std::string esc;  // the key as a record slot would hold it: 0x00 / 0x01 escaped (order preserving, see escape)
   uint64_t value;
 };
 struct LongGroup {
@@ -85,9 +86,6 @@ struct mrhbm_ctx {
   uint64_t l1all_cap = 0;
   uint32_t *d_ipc = nullptr, *h_ipc = nullptr;  // 16 words per rank: the IPC handles
   uint32_t *d_sample = nullptr, *h_sample = nullptr;  // 256 buckets of the key sample
-  uint32_t tune = 0;                          // MRHBM_TUNE, read once at init, measurement hooks only: bit 0 = no fast path,
-                                              // bit 6 = print when the CTAs of level 1 and of the combiner start / end (with bit 24:
-                                              // of the u64 sort), bits 8-15 = the combiner's L2 prefetch distance in trips
   std::recursive_mutex mu;                    // entry points serialise per ctx
   uint32_t *d_small = nullptr, *h_small = nullptr;  // 64 words each
   bool no_optimistic = false;  // sticky: a fixed-capacity bin overflowed once (skewed keys)
@@ -261,6 +259,13 @@ int stage_slot(mrhbm_map* m, unsigned char** slot) {
   return 0;
 }
 
+// room for n records of the map's output straight in the pool, behind what it has staged (emission order): *off is
+// the first of them.  The caller fills them and then adds the range.
+int pool_take(mrhbm_map* m, uint64_t n, uint64_t* off) {
+  int rc = stage_flush(m);
+  return rc ? rc : pool_reserve(m->ctx, n, off);
+}
+
 void map_release(mrhbm_map* m) {
   for (int i = 0; i < 2; i++) {
     if (m->stage_busy[i]) cudaEventSynchronize(m->stage_ev[i]);
@@ -277,54 +282,52 @@ void invalidate(mrhbm_ctx* c) {
   c->long_group_count = 0;
 }
 
+struct DevBuf {
+  void** p;
+  size_t elem;  // bytes per element
+};
+// Grows device buffers that share one capacity to at least `need` elements each; their contents are not kept.  When
+// they hold fewer, they are freed and `alloc` >= need elements (the caller's headroom) are allocated: *cap = alloc.
+int grow(mrhbm_ctx* c, uint64_t* cap, uint64_t need, uint64_t alloc, std::initializer_list<DevBuf> bufs) {
+  if (need <= *cap) return 0;
+  *cap = 0;
+  for (const DevBuf& b : bufs) {
+    if (*b.p) CU(c, cudaFree(*b.p));
+    *b.p = nullptr;
+  }
+  for (const DevBuf& b : bufs) CU(c, cudaMalloc(b.p, alloc * b.elem));
+  *cap = alloc;
+  return 0;
+}
+
+// at least `need` records, and at least one
+int ensure_records(mrhbm_ctx* c, void** buf, uint64_t* cap, uint64_t need) {
+  need = std::max<uint64_t>(need, 1);
+  return grow(c, cap, need, need, {{buf, (size_t)c->rb}});
+}
+
+// the sorted output: keys and sums of at least `need` rows, and at least one
+int ensure_out(mrhbm_ctx* c, uint64_t need) {
+  need = std::max<uint64_t>(need, 1);
+  return grow(c, &c->out_cap, need, need, {{&c->sb.out_keys, (size_t)c->kb}, {(void**)&c->sb.out_sums, sizeof(uint64_t)}});
+}
+
 // per-bin arrays (offsets, group counts, spread-out atomic counters) for B bins
 int ensure_small_arrays(mrhbm_ctx* c, uint64_t B) {
-  if (B + 1 > c->B_cap) {
-    uint64_t nb = B + 1 + (B >> 2);
-    uint32_t** ptrs[] = {&c->sb.bin_off, &c->sb.ucount, &c->sb.uoff, &c->sb.big_list};
-    for (auto p : ptrs) {
-      if (*p) CU(c, cudaFree(*p));
-      *p = nullptr;
-      CU(c, cudaMalloc((void**)p, nb * sizeof(uint32_t)));
-    }
-    c->B_cap = nb;
-  }
-  if ((B << c->ctr_shift) > c->ctr_cap) {  // spread-out atomic counters
-    uint64_t nc = (B + (B >> 2) + 1) << c->ctr_shift;
-    uint32_t** ptrs[] = {&c->sb.hist, &c->sb.cursor};
-    for (auto p : ptrs) {
-      if (*p) CU(c, cudaFree(*p));
-      *p = nullptr;
-      CU(c, cudaMalloc((void**)p, nc * sizeof(uint32_t)));
-    }
-    c->ctr_cap = nc;
-  }
+  int rc = grow(c, &c->B_cap, B + 1, B + 1 + (B >> 2),
+                {{(void**)&c->sb.bin_off, 4}, {(void**)&c->sb.ucount, 4}, {(void**)&c->sb.uoff, 4}, {(void**)&c->sb.big_list, 4}});
+  if (rc) return rc;
+  rc = grow(c, &c->ctr_cap, B << c->ctr_shift, (B + (B >> 2) + 1) << c->ctr_shift,  // spread-out atomic counters
+            {{(void**)&c->sb.hist, 4}, {(void**)&c->sb.cursor, 4}});
+  if (rc) return rc;
   if (!c->sb.counters) CU(c, cudaMalloc((void**)&c->sb.counters, 8 * sizeof(uint32_t)));
   return 0;
 }
 
 int ensure_buffers(mrhbm_ctx* c, uint64_t B, uint64_t N) {
   int rc = ensure_small_arrays(c, B);
-  if (rc) return rc;
-  uint64_t need = std::max<uint64_t>(N, 1);
-  if (need > c->mid_cap) {
-    if (c->sb.mid) CU(c, cudaFree(c->sb.mid));
-    c->sb.mid = nullptr;
-    c->mid_cap = 0;
-    CU(c, cudaMalloc(&c->sb.mid, need * c->rb));
-    c->mid_cap = need;
-  }
-  if (need > c->out_cap) {
-    if (c->sb.out_keys) CU(c, cudaFree(c->sb.out_keys));
-    if (c->sb.out_sums) CU(c, cudaFree(c->sb.out_sums));
-    c->sb.out_keys = nullptr;
-    c->sb.out_sums = nullptr;
-    c->out_cap = 0;
-    CU(c, cudaMalloc(&c->sb.out_keys, need * c->kb));
-    CU(c, cudaMalloc((void**)&c->sb.out_sums, need * sizeof(uint64_t)));
-    c->out_cap = need;
-  }
-  return 0;
+  if (!rc) rc = ensure_records(c, &c->sb.mid, &c->mid_cap, N);
+  return rc ? rc : ensure_out(c, N);
 }
 
 // committed ranges, adjacent ones merged
@@ -343,17 +346,9 @@ std::vector<std::pair<uint64_t, uint64_t>> live_ranges(const mrhbm_ctx* c) {
 int ensure_compact(mrhbm_ctx* c) {
   if (!c->shuffled) return fail(c, MRHBM_E_INVAL, "no shuffle result (call mrhbm_shuffle first)");
   if (c->compacted) return 0;
-  uint64_t need = std::max<uint64_t>(c->groups, 1);
-  if (need > c->c_cap) {
-    if (c->ckeys) CU(c, cudaFree(c->ckeys));
-    if (c->csums) CU(c, cudaFree(c->csums));
-    c->ckeys = nullptr;
-    c->csums = nullptr;
-    c->c_cap = 0;
-    CU(c, cudaMalloc(&c->ckeys, need * c->kb));
-    CU(c, cudaMalloc((void**)&c->csums, need * sizeof(uint64_t)));
-    c->c_cap = need;
-  }
+  const uint64_t need = std::max<uint64_t>(c->groups, 1);
+  int rc = grow(c, &c->c_cap, need, need, {{&c->ckeys, (size_t)c->kb}, {(void**)&c->csums, sizeof(uint64_t)}});
+  if (rc) return rc;
   launch_compact(c->rb, c->rv, c->B, c->ckeys, c->csums, c->stream);
   CU(c, cudaGetLastError());
   CU(c, cudaStreamSynchronize(c->stream));
@@ -368,6 +363,35 @@ float ev_ms(mrhbm_ctx* c, int a, int b) {
     return 0;
   }
   return ms;
+}
+
+// Key slots are zero padded, so a key byte 0x00 cannot be stored as such.  Bytes 0x00 and 0x01 travel escaped --
+// 0x00 -> 01 01, 0x01 -> 01 02 -- which keeps the bytewise order of the keys ("a" < "a\0" < "a\1" < "ab", SURVEY A.3)
+// and is the identity for text.  Record slots and the host-side store of long keys hold keys in this form; the
+// device partitioner hashes the unescaped bytes, the iterator unescapes.
+// escape: the escaped form of key[0..n) to dst (room for n + the number of bytes <= 1), returns its length
+size_t escape(const unsigned char* key, size_t n, unsigned char* dst) {
+  size_t o = 0;
+  for (size_t i = 0; i < n; i++) {
+    if (key[i] <= 1) {
+      dst[o++] = 1;
+      dst[o++] = (unsigned char)(key[i] + 1);
+    } else {
+      dst[o++] = key[i];
+    }
+  }
+  return o;
+}
+// unescape: out = the original bytes of the escaped key esc[0..n)
+void unescape(const void* esc, size_t n, std::vector<unsigned char>& out) {
+  const unsigned char* e = (const unsigned char*)esc;
+  out.clear();
+  for (size_t i = 0; i < n; i++) {
+    if (e[i] == 1 && i + 1 < n)
+      out.push_back((unsigned char)(e[++i] - 1));
+    else
+      out.push_back(e[i]);
+  }
 }
 
 }  // namespace
@@ -432,8 +456,6 @@ int mrhbm_init(const mrhbm_config* cfg, mrhbm_ctx** out) {
   c->cap = (cfg->flags & MRHBM_F_SMALL_BINS) ? 96 : cap_records(c->rb);
   CU(c, cudaMalloc((void**)&c->d_sample, 256 * sizeof(uint32_t)));
   CU(c, cudaHostAlloc((void**)&c->h_sample, 256 * sizeof(uint32_t), cudaHostAllocDefault));
-  if (const char* e = getenv("MRHBM_TUNE")) c->tune = (uint32_t)strtoul(e, nullptr, 0);  // measurement hooks, read once
-  kernels_set_tune(c->tune);
   if (cfg->reserve_pairs) {
     uint64_t off;
     int rc = pool_reserve(c, cfg->reserve_pairs, &off);
@@ -514,24 +536,15 @@ int mrhbm_emit_str(mrhbm_map* m, const void* key, size_t klen, uint32_t value) {
   mrhbm_ctx* c = m->ctx;
   Entry g(c);
   if (c->cfg.key_kind != MRHBM_KEY_STR) return fail(c, MRHBM_E_INVAL, "ctx holds u64 keys");
-  // Key slots are zero padded, so a key byte 0x00 cannot be stored as such.  Bytes 0x00 and 0x01 travel escaped --
-  // 0x00 -> 01 01, 0x01 -> 01 02 -- which keeps the bytewise order of the keys ("a" < "a\0" < "a\1" < "ab", SURVEY A.3)
-  // and is the identity for text.  The device partitioner hashes the unescaped bytes, the iterator unescapes.
+  // (keys are stored escaped, see escape)
   const unsigned char* k = (const unsigned char*)key;
-  size_t extra = 0;
-  for (size_t i = 0; i < klen; i++) extra += k[i] <= 1;
-  if (klen + extra >= (size_t)c->kb) {  // longer than a record slot: kept on the host (escaped like a slot would hold it)
+  size_t elen = klen;
+  for (size_t i = 0; i < klen; i++) elen += k[i] <= 1;
+  if (elen >= (size_t)c->kb) {  // longer than a record slot: kept on the host (escaped like a slot would hold it)
     if (klen > kMaxLongKey) return fail(c, MRHBM_E_KEY, "key of %zu bytes (limit %zu)", klen, (size_t)kMaxLongKey);
     LongPair lp;
-    lp.esc.reserve(klen + extra);
-    for (size_t i = 0; i < klen; i++) {
-      if (k[i] <= 1) {
-        lp.esc.push_back((char)1);
-        lp.esc.push_back((char)(k[i] + 1));
-      } else {
-        lp.esc.push_back((char)k[i]);
-      }
-    }
+    lp.esc.resize(elen);
+    escape(k, klen, (unsigned char*)&lp.esc[0]);
     lp.value = value;
     m->long_pairs.push_back(std::move(lp));
     return MRHBM_OK;
@@ -539,20 +552,8 @@ int mrhbm_emit_str(mrhbm_map* m, const void* key, size_t klen, uint32_t value) {
   unsigned char* slot;
   int rc = stage_slot(m, &slot);
   if (rc) return rc;
-  if (!extra) {
-    memcpy(slot, key, klen);
-  } else {
-    size_t o = 0;
-    for (size_t i = 0; i < klen; i++) {
-      if (k[i] <= 1) {
-        slot[o++] = 1;
-        slot[o++] = (unsigned char)(k[i] + 1);
-      } else {
-        slot[o++] = k[i];
-      }
-    }
-  }
-  memset(slot + klen + extra, 0, c->kb - (klen + extra));
+  escape(k, klen, slot);
+  memset(slot + elen, 0, c->kb - elen);
   memcpy(slot + c->kb, &value, 4);
   return MRHBM_OK;
 }
@@ -575,10 +576,8 @@ int mrhbm_emit_batch(mrhbm_map* m, const void* recs, size_t n) {
   mrhbm_ctx* c = m->ctx;
   Entry g(c);
   if (!n) return MRHBM_OK;
-  int rc = stage_flush(m);  // keep emission order
-  if (rc) return rc;
   uint64_t off;
-  rc = pool_reserve(c, n, &off);
+  int rc = pool_take(m, n, &off);
   if (rc) return rc;
   cudaPointerAttributes at{};
   bool pinned = cudaPointerGetAttributes(&at, recs) == cudaSuccess && at.type == cudaMemoryTypeHost;
@@ -594,10 +593,8 @@ int mrhbm_emit_device(mrhbm_map* m, const void* drecs, size_t n) {
   mrhbm_ctx* c = m->ctx;
   Entry g(c);
   if (!n) return MRHBM_OK;
-  int rc = stage_flush(m);
-  if (rc) return rc;
   uint64_t off;
-  rc = pool_reserve(c, n, &off);
+  int rc = pool_take(m, n, &off);
   if (rc) return rc;
   CU(c, cudaMemcpyAsync((char*)c->pool + off * c->rb, drecs, n * c->rb, cudaMemcpyDeviceToDevice, c->stream));
   add_range(m, off, n);
@@ -609,10 +606,8 @@ int mrhbm_map_gen_u64(mrhbm_map* m, uint64_t seed, uint64_t start, uint64_t n) {
   mrhbm_ctx* c = m->ctx;
   Entry g(c);
   if (c->rb != 16) return fail(c, MRHBM_E_INVAL, "gen_u64 needs a u64-key ctx");
-  int rc = stage_flush(m);
-  if (rc) return rc;
   uint64_t off;
-  rc = pool_reserve(c, n, &off);
+  int rc = pool_take(m, n, &off);
   if (rc) return rc;
   launch_gen_u64((char*)c->pool + off * c->rb, seed, start, n, c->stream);
   CU(c, cudaGetLastError());
@@ -636,10 +631,8 @@ int mrhbm_map_gen_zipf(mrhbm_map* m, uint64_t seed, uint64_t start, uint64_t n, 
     c->d_table_first = table[0];
     c->d_table_last = table[V - 1];
   }
-  int rc = stage_flush(m);
-  if (rc) return rc;
   uint64_t off;
-  rc = pool_reserve(c, n, &off);
+  int rc = pool_take(m, n, &off);
   if (rc) return rc;
   launch_gen_zipf32((char*)c->pool + off * c->rb, seed, start, n, c->d_table, V, c->stream);
   CU(c, cudaGetLastError());
@@ -922,7 +915,6 @@ void set_range_hint(ShuffleBuffers& b, uint32_t S, uint32_t ordered) {
 
 BinParams make_bp(const mrhbm_ctx* c, uint32_t S, uint32_t ordered) {
   BinParams bp{};
-  bp.rep_shift = 0;
   bp.P = c->cfg.num_partitions;
   bp.S = S;
   bp.partitioner = c->cfg.partitioner;
@@ -934,22 +926,6 @@ BinParams make_bp(const mrhbm_ctx* c, uint32_t S, uint32_t ordered) {
     if ((1u << k) == bp.world) bp.wshift = k;
   for (int r = 0; r <= 8; r++) bp.pbase[r] = c->pbase[r];
   return bp;
-}
-
-// all ranks: one u32 from every rank (host value in, host values out); synchronises the stream
-int gather_u32(mrhbm_ctx* c, uint32_t mine, uint32_t* all) {
-  if (c->world == 1) {
-    all[0] = mine;
-    return 0;
-  }
-  c->h_small[0] = mine;
-  CU(c, cudaMemcpyAsync(c->d_small, c->h_small, 4, cudaMemcpyHostToDevice, c->stream));
-  int rc = comm_allgather_u32(c->comm, c->d_small, c->d_small + 16, 1, c->stream, &c->err);
-  if (rc) return rc;
-  CU(c, cudaMemcpyAsync(c->h_small + 16, c->d_small + 16, 4 * c->world, cudaMemcpyDeviceToHost, c->stream));
-  CU(c, cudaStreamSynchronize(c->stream));
-  for (int r = 0; r < c->world; r++) all[r] = c->h_small[16 + r];
-  return 0;
 }
 
 // all ranks: k <= 2 words from every rank (host values in, all[rank * k + i] out); synchronises the stream
@@ -967,8 +943,6 @@ int gather_words(mrhbm_ctx* c, const uint32_t* mine, int k, uint32_t* all) {
   for (int i = 0; i < k * c->world; i++) all[i] = c->h_small[16 + i];
   return 0;
 }
-
-int ensure_records(mrhbm_ctx* c, void** buf, uint64_t* cap, uint64_t need);
 
 // The region buffer of the two-level split.  One GPU: a plain allocation.  Several GPUs: COLLECTIVE -- every
 // rank calls it with the same `need`; all buffers grow together and their IPC handles are re-exchanged, so that
@@ -990,14 +964,11 @@ int ensure_regions(mrhbm_ctx* c, uint64_t need, bool* shared_ok) {
     c->peer_regions[r] = nullptr;
   }
   cudaGetLastError();
-  uint32_t flags[8];
-  int rc = gather_u32(c, 0, flags);  // every rank has unmapped its peers before anybody frees
+  uint32_t flag = 0, flags[8];
+  int rc = gather_words(c, &flag, 1, flags);  // every rank has unmapped its peers before anybody frees
   if (rc) return rc;
-  need += need / 8 + 1024;
-  if (c->regions) CU(c, cudaFree(c->regions));
-  c->regions = nullptr;
-  c->regions_cap = 0;
-  CU(c, cudaMalloc(&c->regions, need * c->rb));
+  rc = grow(c, &c->regions_cap, need, need + need / 8 + 1024, {{&c->regions, (size_t)c->rb}});
+  if (rc) return rc;
   bool ok = true;
   cudaIpcMemHandle_t h;
   memset(&h, 0, sizeof h);
@@ -1011,7 +982,8 @@ int ensure_regions(mrhbm_ctx* c, uint64_t need, bool* shared_ok) {
   if (rc) return rc;
   CU(c, cudaMemcpyAsync(c->h_ipc + 16, c->d_ipc + 16, 64 * (size_t)G, cudaMemcpyDeviceToHost, c->stream));
   CU(c, cudaStreamSynchronize(c->stream));
-  rc = gather_u32(c, ok ? 0u : 1u, flags);  // a rank that could not export: nobody opens anything
+  flag = ok ? 0u : 1u;
+  rc = gather_words(c, &flag, 1, flags);  // a rank that could not export: nobody opens anything
   if (rc) return rc;
   for (int r = 0; r < G; r++) ok = ok && flags[r] == 0;
   if (ok) {
@@ -1028,7 +1000,8 @@ int ensure_regions(mrhbm_ctx* c, uint64_t need, bool* shared_ok) {
         ok = false;
       }
     }
-    rc = gather_u32(c, ok ? 0u : 1u, flags);
+    flag = ok ? 0u : 1u;
+    rc = gather_words(c, &flag, 1, flags);
     if (rc) return rc;
     for (int r = 0; r < G; r++) ok = ok && flags[r] == 0;
   }
@@ -1040,64 +1013,16 @@ int ensure_regions(mrhbm_ctx* c, uint64_t need, bool* shared_ok) {
     cudaGetLastError();
     c->ipc_failed = true;
     *shared_ok = false;
-    return 0;
   }
-  c->regions_cap = need;
   return 0;
 }
 
 int ensure_multi_buffers(mrhbm_ctx* c, uint64_t B, uint64_t Bl) {
-  const int G = c->world;
-  if (B > c->hd_cap) {
-    uint64_t nb = B + (B >> 2) + 1;
-    for (uint32_t** p : {&c->d_hd, &c->d_hall}) {
-      if (*p) CU(c, cudaFree(*p));
-      *p = nullptr;
-    }
-    CU(c, cudaMalloc((void**)&c->d_hd, nb * 4));
-    CU(c, cudaMalloc((void**)&c->d_hall, nb * 4 * G));
-    c->hd_cap = nb;
-  }
-  if (Bl + 1 > c->bl_cap) {
-    uint64_t nb = Bl + (Bl >> 2) + 2;
-    for (uint32_t** p : {&c->d_tot, &c->d_outoff, &c->d_segoff}) {
-      if (*p) CU(c, cudaFree(*p));
-      *p = nullptr;
-    }
-    CU(c, cudaMalloc((void**)&c->d_tot, nb * 4));
-    CU(c, cudaMalloc((void**)&c->d_outoff, nb * 4));
-    CU(c, cudaMalloc((void**)&c->d_segoff, nb * 4 * G));
-    c->bl_cap = nb;
-  }
-  return 0;
-}
-
-int ensure_records(mrhbm_ctx* c, void** buf, uint64_t* cap, uint64_t need);
-int gather_u32(mrhbm_ctx* c, uint32_t mine, uint32_t* all);
-
-int ensure_records(mrhbm_ctx* c, void** buf, uint64_t* cap, uint64_t need) {
-  need = std::max<uint64_t>(need, 1);
-  if (need <= *cap) return 0;
-  if (*buf) CU(c, cudaFree(*buf));
-  *buf = nullptr;
-  *cap = 0;
-  CU(c, cudaMalloc(buf, need * c->rb));
-  *cap = need;
-  return 0;
-}
-
-int ensure_out(mrhbm_ctx* c, uint64_t need) {
-  need = std::max<uint64_t>(need, 1);
-  if (need <= c->out_cap) return 0;
-  if (c->sb.out_keys) CU(c, cudaFree(c->sb.out_keys));
-  if (c->sb.out_sums) CU(c, cudaFree(c->sb.out_sums));
-  c->sb.out_keys = nullptr;
-  c->sb.out_sums = nullptr;
-  c->out_cap = 0;
-  CU(c, cudaMalloc(&c->sb.out_keys, need * c->kb));
-  CU(c, cudaMalloc((void**)&c->sb.out_sums, need * sizeof(uint64_t)));
-  c->out_cap = need;
-  return 0;
+  const size_t G = (size_t)c->world;
+  int rc = grow(c, &c->hd_cap, B, B + (B >> 2) + 1, {{(void**)&c->d_hd, 4}, {(void**)&c->d_hall, 4 * G}});
+  if (rc) return rc;
+  return grow(c, &c->bl_cap, Bl + 1, Bl + (Bl >> 2) + 2,
+              {{(void**)&c->d_tot, 4}, {(void**)&c->d_outoff, 4}, {(void**)&c->d_segoff, 4 * G}});
 }
 
 struct Src {
@@ -1106,6 +1031,10 @@ struct Src {
 };
 constexpr uint32_t kGtabLog = 21;       // global combiner table: 2^21 16-byte entries = 32 MB, resident in the 50 MB L2
 constexpr uint32_t kGtabMaxExtra = 5;   // ... grown up to 32x (1 GB) when the keys do not fit
+
+int overflow_error(mrhbm_ctx* c) {
+  return fail(c, MRHBM_E_OVERFLOW, "u32 partial sum overflow while combining a hot key");
+}
 
 // The pairs the shuffle partitions: the committed pool ranges, or -- with a combiner declared
 // (job.lua:92-96,198-202) and enough pairs to pay for it -- one record per distinct key of this rank's pairs
@@ -1132,23 +1061,14 @@ int collect_sources(mrhbm_ctx* c, std::vector<Src>& srcs, uint64_t* N, mrhbm_sta
     if (rc) return rc;
     CU(c, cudaMemsetAsync(c->gtab, 0, tab_bytes, s));
     CU(c, cudaMemsetAsync(c->d_small, 0, 3 * sizeof(uint32_t), s));  // [0] flags, [1] records out, [2] largest value
-    if (c->tune & 64u) {  // measurement hook: k_combine's first CTA start, last CTA end, first CTA end at words 8..13
-      CU(c, cudaMemsetAsync(c->d_small + 8, 0xff, 8, s));
-      CU(c, cudaMemsetAsync(c->d_small + 10, 0, 8, s));
-      CU(c, cudaMemsetAsync(c->d_small + 12, 0xff, 8, s));
-    }
     for (auto& sr : srcs)
       st.launches += launch_combine(c->rb, sr.p, sr.n, (uint32_t*)c->gtab, glog, c->d_small, checked, c->sm_count, s);
     st.launches += launch_gtab_compact(c->rb, (const uint32_t*)c->gtab, glog, c->comb, c->d_small + 1, s);
     CU(c, cudaGetLastError());
-    CU(c, cudaMemcpyAsync(c->h_small, c->d_small, 14 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+    CU(c, cudaMemcpyAsync(c->h_small, c->d_small, 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
     CU(c, cudaStreamSynchronize(s));
-    if (c->tune & 64u) {
-      const uint64_t* t = (const uint64_t*)(c->h_small + 8);
-      fprintf(stderr, "[mrhbm] k_combine: first CTA ends after %.3f ms, last after %.3f ms\n", (t[2] - t[0]) * 1e-6, (t[1] - t[0]) * 1e-6);
-    }
     const uint32_t ef = c->h_small[0];
-    if (ef & ERRF_OVERFLOW) return fail(c, MRHBM_E_OVERFLOW, "u32 partial sum overflow while combining a hot key");
+    if (ef & ERRF_OVERFLOW) return overflow_error(c);
     if (ef & ERRF_SKEW) {  // the table filled up: more distinct keys than it takes
       if (c->gtab_extra < kGtabMaxExtra) {
         c->gtab_extra++;
@@ -1179,17 +1099,110 @@ uint32_t pick_sub_bins(const mrhbm_ctx* c, uint64_t n_total, uint32_t copies = 1
   return (uint32_t)std::max<uint64_t>(1, (n_total + P * target - 1) / (P * target));
 }
 
-void finish_stats(mrhbm_ctx* c, mrhbm_stats& st) {
+// The error flags of an attempt, OR-ed over all ranks: every rank must take the same branch.  The all-gather also
+// tells every rank whether any rank holds long keys (c->any_long).  One GPU: *ef stays as it is.  A u32 sum that
+// wrapped on any rank is an error no retry fixes.
+int agree_flags(mrhbm_ctx* c, uint32_t* ef) {
+  if (c->world > 1) {
+    const uint32_t mine = *ef | (c->long_jobs.empty() ? 0u : kErrfLongKeys);
+    uint32_t all[8];
+    int rc = gather_words(c, &mine, 1, all);
+    if (rc) return rc;
+    for (int r = 0; r < c->world; r++) *ef |= all[r];
+    c->any_long = (*ef & kErrfLongKeys) != 0;
+    *ef &= ~kErrfLongKeys;
+  }
+  return (*ef & ERRF_OVERFLOW) ? overflow_error(c) : 0;
+}
+
+// Exact layout (bin offsets in sb.bin_off after k_hist + k_exscan): the records of `live` go to their B bins in sb.mid
+// (on several GPUs: the destination-major send buffer), through the two-level coalesced split when there are enough
+// bins (claims relative to bin_off), else the direct scatter.
+int exact_split(mrhbm_ctx* c, const std::vector<Src>& live, const BinParams& bp, uint64_t B, uint64_t N, mrhbm_stats& st) {
+  cudaStream_t s = c->stream;
+  uint32_t F = 1;
+  while ((uint64_t)F * F < B) F <<= 1;
+  const uint32_t C1 = (uint32_t)((B + F - 1) / F);
+  if (B >= 2048 && F <= 1024 && C1 <= 1024) {
+    int rc = ensure_records(c, &c->l1buf, &c->l1_cap, N);
+    if (rc) return rc;
+    // relative fill levels: coarse levels live in hist (dead after the scan), fine levels in cursor
+    CU(c, cudaMemsetAsync(c->sb.hist, 0, ((uint64_t)C1 << c->ctr_shift) * sizeof(uint32_t), s));
+    CU(c, cudaMemsetAsync(c->sb.cursor, 0, (B << c->ctr_shift) * sizeof(uint32_t), s));
+    SplitPlan pl{};
+    pl.B = (uint32_t)B;
+    pl.F = F;
+    pl.C1 = pl.C1_local = C1;
+    pl.cap = c->cap;
+    pl.cursor1 = c->sb.hist;
+    pl.cursor = c->sb.cursor;
+    pl.l1 = c->l1buf;
+    pl.mid = c->sb.mid;
+    pl.err_flags = c->sb.counters + CNT_ERR;
+    pl.base_off = c->sb.bin_off;
+    pl.ndest = 1;
+    for (auto& r : live) st.launches += launch_split_l1(c->rb, r.p, r.n, bp, pl, s);
+    st.launches += launch_split_l2(c->rb, bp, pl, s);
+  } else {
+    for (auto& r : live) st.launches += launch_scatter(c->rb, r.p, r.n, bp, c->sb.cursor, c->sb.mid, s);
+  }
+  return 0;
+}
+
+// Exact layout, after the sort of the nb bins of view v (nbig of them oversized): k_big_bins, the group offsets, and
+// the bin offsets (v.bin_off), group offsets and counters read back.  EV_BIG, EV_END; synchronises the stream.
+int exact_tail(mrhbm_ctx* c, const ShuffleBuffers& v, uint64_t nb, uint32_t nbig, mrhbm_stats& st) {
+  cudaStream_t s = c->stream;
+  st.launches += launch_big_bins(c->rb, v, nbig, c->cap, s);
+  CU(c, cudaEventRecord(c->ev[EV_BIG], s));
+  c->h_big.clear();
+  if (c->sb.no_reduce && nbig) {  // group-only mode: the iterator merges the runs of an oversized bin
+    c->h_big.resize(nbig);
+    CU(c, cudaMemcpyAsync(c->h_big.data(), c->sb.big_list, nbig * 4, cudaMemcpyDeviceToHost, s));
+  }
+  st.launches += launch_exscan(c->sb.ucount, (uint32_t)nb, c->sb.uoff, nullptr, nullptr, 0xffffffffu, nullptr, nullptr,
+                               c->sb.counters + CNT_TOTAL, 0, s, c->d_small + 64);
+  c->h_bin_off.resize(nb + 1);
+  c->h_uoff.resize(nb + 1);
+  CU(c, cudaMemcpyAsync(c->h_bin_off.data(), v.bin_off, (nb + 1) * 4, cudaMemcpyDeviceToHost, s));
+  CU(c, cudaMemcpyAsync(c->h_uoff.data(), c->sb.uoff, (nb + 1) * 4, cudaMemcpyDeviceToHost, s));
+  CU(c, cudaMemcpyAsync(c->h_counters, c->sb.counters, 8 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+  CU(c, cudaEventRecord(c->ev[EV_END], s));
+  CU(c, cudaGetLastError());
+  CU(c, cudaStreamSynchronize(s));
+  return 0;
+}
+
+// View v over Bl local bins (the first is global bin bin_base) becomes the result the accessors read, and the stats
+// are filled in.  Which events bound the exchange and the scatter depends on the path: the caller times them.
+int publish(mrhbm_ctx* c, const ShuffleBuffers& v, uint64_t Bl, uint32_t S, uint32_t ordered, uint64_t N_in,
+            uint64_t N_recv, uint32_t bin_base, uint32_t nbig, mrhbm_stats& st, float ms_exchange, float ms_scatter) {
+  c->rv = v;
+  c->B = (uint32_t)Bl;
+  c->S = S;
+  c->ordered = ordered;
+  c->N = N_in;
+  c->N_recv = N_recv;
+  c->bin_base = bin_base;
+  c->groups = c->h_uoff[Bl];
+  c->shuffled = true;
+  c->compacted = false;
+  st.bins = (uint32_t)Bl;
+  st.sub_bins = S;
+  st.big_bins = nbig;
+  st.groups = c->groups;
   st.ms_total = ev_ms(c, EV_START, EV_END);
   st.ms_combine = ev_ms(c, EV_START, EV_CSTART);
   st.ms_hist = ev_ms(c, EV_COMBINE, EV_HIST);
   st.ms_plan = ev_ms(c, EV_HIST, EV_PLAN);
-  st.ms_scatter = ev_ms(c, EV_PLAN, EV_SCATTER);
+  st.ms_exchange = ms_exchange;
+  st.ms_scatter = ms_scatter;
   st.ms_sort_reduce = ev_ms(c, EV_EXCH, EV_SORT);
   st.ms_bigbins = ev_ms(c, EV_SORT, EV_BIG);
   st.ms_setup = ev_ms(c, EV_CSTART, EV_COMBINE);
   st.ms_finish = ev_ms(c, EV_BIG, EV_END);
   c->stats = st;
+  return MRHBM_OK;
 }
 
 // ---- the default path: optimistic fixed-capacity layout, no histogram pass, any number of GPUs --------
@@ -1240,190 +1253,144 @@ int shuffle_fast(mrhbm_ctx* c, std::vector<Src>& live, uint64_t N, uint64_t N_in
   }
   if (Nglobal == 0) return 0;  // nothing to do here: the exact path handles the empty shuffle
   const uint32_t S = pick_sub_bins(c, Nglobal, c->cfg.combiner && G > 1 ? (uint32_t)G : 1u);
+  const uint64_t B = (uint64_t)P * S;
+  if (B >= (1ull << 31)) return 0;
+  const uint32_t ordered = (want_ordered && !nonuniform) || S == 1;
+  uint64_t Bl_of[8];
+  for (int r = 0; r < G; r++) Bl_of[r] = (uint64_t)(c->pbase[r + 1] - c->pbase[r]) * S;
+  const uint64_t Bl = Bl_of[me];
+  const uint32_t bin_stride = c->cap;  // slots per fine bin: what one CTA sorts in shared memory
+  // ---- levels.  One GPU, few bins: level 1 goes straight into the fine bins.
+  SplitPlan pl{};
+  const bool single_level = G == 1 && B <= kSplitMaxBinsHost;
+  uint32_t F = 1;
+  if (!single_level) {
+    while ((uint64_t)F * F < B) F <<= 1;  // power of two >= sqrt(B): both levels see about the same fan-out
+    for (;; F <<= 1) {
+      uint64_t c1 = 0;
+      for (int r = 0; r < G; r++) c1 += (Bl_of[r] + F - 1) / F;
+      if (c1 <= kSplitMaxBinsHost) break;
+    }
+    if (F > kSplitMaxBinsHost) return 0;  // more bins than two levels reach: exact path
+  }
+  pl.rbase[0] = 0;
+  for (int r = 0; r < 8; r++) {
+    const uint64_t bl = r < G ? Bl_of[r] : 0;
+    pl.rbase[r + 1] = pl.rbase[r] + (uint32_t)((bl + F - 1) / F);
+    pl.fbase[r] = c->pbase[r] * S;
+  }
+  pl.fbase[8] = c->pbase[8] * S;
+  pl.B = (uint32_t)B;
+  pl.F = F;
+  pl.C1 = pl.rbase[G];
+  pl.C1_local = pl.rbase[me + 1] - pl.rbase[me];
+  pl.cap = bin_stride;
+  pl.ndest = (uint32_t)G;
+  pl.me = (uint32_t)me;
   {
-    const uint64_t B = (uint64_t)P * S;
-    if (B >= (1ull << 31)) return 0;
-    const uint32_t ordered = (want_ordered && !nonuniform) || S == 1;
-    uint64_t Bl_of[8], Bl_max = 0;
-    for (int r = 0; r < G; r++) {
-      Bl_of[r] = (uint64_t)(c->pbase[r + 1] - c->pbase[r]) * S;
-      Bl_max = std::max(Bl_max, Bl_of[r]);
-    }
-    const uint64_t Bl = Bl_of[me];
-    const uint32_t bin_stride = c->cap;  // slots per fine bin: what one CTA sorts in shared memory
-    // ---- levels.  One GPU, few bins: level 1 goes straight into the fine bins.
-    SplitPlan pl{};
-    const bool single_level = G == 1 && B <= kSplitMaxBinsHost;
-    uint32_t F = 1;
-    if (!single_level) {
-      while ((uint64_t)F * F < B) F <<= 1;  // power of two >= sqrt(B): both levels see about the same fan-out
-      for (;; F <<= 1) {
-        uint64_t c1 = 0;
-        for (int r = 0; r < G; r++) c1 += (Bl_of[r] + F - 1) / F;
-        if (c1 <= kSplitMaxBinsHost) break;
-      }
-      if (F > kSplitMaxBinsHost) return 0;  // more bins than two levels reach: exact path
-    }
-    pl.rbase[0] = 0;
-    for (int r = 0; r < 8; r++) {
-      const uint64_t bl = r < G ? Bl_of[r] : 0;
-      pl.rbase[r + 1] = pl.rbase[r] + (uint32_t)((bl + F - 1) / F);
-      pl.fbase[r] = c->pbase[r] * S;
-    }
-    pl.fbase[8] = c->pbase[8] * S;
-    pl.B = (uint32_t)B;
-    pl.F = F;
-    pl.C1 = pl.rbase[G];
-    pl.C1_local = pl.rbase[me + 1] - pl.rbase[me];
-    pl.cap = bin_stride;
-    pl.ndest = (uint32_t)G;
-    pl.me = (uint32_t)me;
-    {
-      // one rank's contribution to one region: F of the B bins, hash balanced
-      const double mean = (double)Nmax * (double)F / (double)B;
-      const double ss = single_level ? (double)bin_stride : mean + 8.0 * std::sqrt(mean) + 64.0;
-      if (ss >= 4.0e9) return 0;
-      pl.sub_stride = ((uint64_t)ss + 7u) & ~7ull;
-    }
-    // ---- buffers
-    rc = ensure_small_arrays(c, std::max<uint64_t>(Bl, pl.C1));
+    // one rank's contribution to one region: F of the B bins, hash balanced
+    const double mean = (double)Nmax * (double)F / (double)B;
+    const double ss = single_level ? (double)bin_stride : mean + 8.0 * std::sqrt(mean) + 64.0;
+    if (ss >= 4.0e9) return 0;
+    pl.sub_stride = ((uint64_t)ss + 7u) & ~7ull;
+  }
+  // ---- buffers
+  rc = ensure_small_arrays(c, std::max<uint64_t>(Bl, pl.C1));
+  if (rc) return rc;
+  // k_split_tma addresses destination slots with 32 bits, and lets the records of a run that does not fit (the
+  // attempt is abandoned then) land at the start of the run's region: one tile of slack behind the last region
+  const uint64_t tile_slack = kSplitTileBytes / c->rb;
+  if (Bl * bin_stride + tile_slack >= (1ull << 32) || (uint64_t)pl.C1 * pl.sub_stride + tile_slack >= (1ull << 32)) return 0;
+  rc = ensure_records(c, &c->sb.mid, &c->mid_cap, Bl * bin_stride + tile_slack);
+  if (rc) return rc;
+  rc = ensure_out(c, Bl * (uint64_t)c->cap);
+  if (rc) return rc;
+  if (!single_level) {
+    bool shared_ok = true;
+    rc = ensure_regions(c, (uint64_t)pl.C1 * pl.sub_stride + tile_slack, &shared_ok);
     if (rc) return rc;
-    // k_split_tma addresses destination slots with 32 bits, and lets the records of a run that does not fit (the
-    // attempt is abandoned then) land at the start of the run's region: one tile of slack behind the last region
-    const uint64_t tile_slack = kSplitTileBytes / c->rb;
-    if (Bl * bin_stride + tile_slack >= (1ull << 32) || (uint64_t)pl.C1 * pl.sub_stride + tile_slack >= (1ull << 32)) return 0;
-    rc = ensure_records(c, &c->sb.mid, &c->mid_cap, Bl * bin_stride + tile_slack);
-    if (rc) return rc;
-    rc = ensure_out(c, Bl * (uint64_t)c->cap);
-    if (rc) return rc;
-    if (!single_level) {
-      bool shared_ok = true;
-      rc = ensure_regions(c, (uint64_t)pl.C1 * pl.sub_stride + tile_slack, &shared_ok);
-      if (rc) return rc;
-      if (!shared_ok) {  // peer mapping unavailable (decided by all ranks together): NCCL exchange instead
-        c->no_optimistic = true;
-        return 0;
-      }
-      if (G > 1) {
-        const uint64_t words = ((uint64_t)pl.C1 << c->ctr_shift) * G;
-        if (words > c->l1all_cap) {
-          if (c->d_l1all) CU(c, cudaFree(c->d_l1all));
-          c->d_l1all = nullptr;
-          c->l1all_cap = 0;
-          CU(c, cudaMalloc((void**)&c->d_l1all, (words + words / 4) * sizeof(uint32_t)));
-          c->l1all_cap = words + words / 4;
-        }
-      }
-    }
-    pl.cursor1 = c->sb.hist;
-    pl.cursor = c->sb.cursor;
-    pl.l1 = single_level ? c->sb.mid : c->regions;
-    pl.mid = c->sb.mid;
-    pl.err_flags = c->sb.counters + CNT_ERR;
-    pl.ticket = c->sb.counters + 5;  // (words 5 and 6 of the 8 counters cleared below)
-    pl.base_off = nullptr;
-    for (int r = 0; r < 8; r++) pl.peer[r] = (unsigned long long)(uintptr_t)(G == 1 ? (r == 0 ? c->regions : nullptr) : c->peer_regions[r]);
-    pl.l1_counts = G == 1 ? c->sb.hist : c->d_l1all;
-    pl.l1_zstride = G == 1 ? 0 : ((uint64_t)pl.C1 << c->ctr_shift);
-    const BinParams bp = make_bp(c, S, ordered);
-    st.attempts++;
-    CU(c, cudaMemsetAsync(c->sb.hist, 0, (((uint64_t)pl.C1) << c->ctr_shift) * sizeof(uint32_t), s));
-    if (!single_level) CU(c, cudaMemsetAsync(c->sb.cursor, 0, (std::max<uint64_t>(Bl, 1) << c->ctr_shift) * sizeof(uint32_t), s));
-    CU(c, cudaMemsetAsync(c->sb.counters, 0, 8 * sizeof(uint32_t), s));
-    if (c->tune & 64u) {  // measurement hook: when do the CTAs of level 1 (bit 24 set: of the u64 sort) start and end (%globaltimer)?
-      if (!(c->tune & (1u << 24))) pl.span = (unsigned long long*)(c->d_acc + 4);
-      CU(c, cudaMemsetAsync(c->d_acc + 4, 0xff, 8, s));
-      CU(c, cudaMemsetAsync(c->d_acc + 5, 0, 16, s));
-      CU(c, cudaMemsetAsync(c->d_acc + 7, 0xff, 8, s));
-    }
-    CU(c, cudaEventRecord(c->ev[EV_COMBINE], s));
-    CU(c, cudaEventRecord(c->ev[EV_HIST], s));
-    for (auto& r : live) st.launches += launch_split_l1(c->rb, r.p, r.n, bp, pl, s);
-    CU(c, cudaEventRecord(c->ev[EV_PLAN], s));
-    if (G > 1) {
-      rc = comm_allgather_u32(c->comm, c->sb.hist, c->d_l1all, (size_t)pl.C1 << c->ctr_shift, s, &c->err);
-      if (rc) return rc;
-    }
-    CU(c, cudaEventRecord(c->ev[EV_GATH], s));
-    if (!single_level) st.launches += launch_split_l2(c->rb, bp, pl, s);
-    CU(c, cudaEventRecord(c->ev[EV_SCATTER], s));
-    CU(c, cudaEventRecord(c->ev[EV_EXCH], s));
-    c->sb.src = c->sb.mid;
-    c->sb.nseg = 1;
-    c->sb.stride = bin_stride;
-    c->sb.out_stride = c->cap;
-    c->sb.rep_shift = 0;
-    c->sb.ctr_shift = c->ctr_shift;
-    // single level: the level-1 cursors ARE the fine fill levels
-    uint32_t* fine_cursor = single_level ? c->sb.hist : c->sb.cursor;
-    ShuffleBuffers v = c->sb;
-    v.cursor = fine_cursor;
-    set_range_hint(v, S, ordered);
-    if ((c->tune & 64u) && (c->tune & (1u << 24))) v.span = (unsigned long long*)(c->d_acc + 4);
-    if (Bl) st.launches += launch_sort_reduce(c->rb, v, (uint32_t)Bl, c->cap, c->sm_count, s);
-    v.span = nullptr;
-    CU(c, cudaEventRecord(c->ev[EV_SORT], s));
-    CU(c, cudaEventRecord(c->ev[EV_BIG], s));
-    c->h_uoff.assign(Bl + 1, 0);
-    if (Bl) {
-      st.launches += launch_exscan(c->sb.ucount, (uint32_t)Bl, c->sb.uoff, nullptr, nullptr, 0xffffffffu, nullptr, nullptr,
-                                   c->sb.counters + CNT_TOTAL, 0, s, c->d_small + 64);
-      CU(c, cudaMemcpyAsync(c->h_uoff.data(), c->sb.uoff, (Bl + 1) * 4, cudaMemcpyDeviceToHost, s));
-    }
-    // pairs this rank reduced (and how many of them came from peers)
-    st.launches += launch_region_totals(pl.l1_counts, pl.l1_zstride, (uint32_t)G, (uint32_t)me, pl.rbase[me], pl.C1_local,
-                                        c->ctr_shift, (uint32_t)std::min<uint64_t>(single_level ? bin_stride : pl.sub_stride, 0xffffffffull),
-                                        c->d_acc, s);
-    CU(c, cudaMemcpyAsync(c->h_acc, c->d_acc, 8 * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
-    CU(c, cudaMemcpyAsync(c->h_counters, c->sb.counters, 8 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
-    CU(c, cudaEventRecord(c->ev[EV_END], s));
-    CU(c, cudaGetLastError());
-    CU(c, cudaStreamSynchronize(s));
-    if (c->tune & 64u)
-      fprintf(stderr, (c->tune & (1u << 24)) ? "[mrhbm] u64 sort: CTAs start over %.3f ms, first ends after %.3f ms, last after %.3f ms (level 1 events: %.3f ms)\n" : "[mrhbm] level 1: CTAs start over %.3f ms, first ends after %.3f ms, last after %.3f ms (events: %.3f ms)\n",
-              (c->h_acc[6] - c->h_acc[4]) * 1e-6, (c->h_acc[7] - c->h_acc[4]) * 1e-6, (c->h_acc[5] - c->h_acc[4]) * 1e-6,
-              ev_ms(c, EV_HIST, EV_PLAN));
-    uint32_t ef = c->h_counters[CNT_ERR];
-    if (G > 1) {  // every rank must take the same branch; also: nobody leaves while a peer still reads its regions
-      uint32_t efs[8];
-      rc = gather_u32(c, ef | (c->long_jobs.empty() ? 0u : kErrfLongKeys), efs);
-      if (rc) return rc;
-      for (int r = 0; r < G; r++) ef |= efs[r];
-      c->any_long = (ef & kErrfLongKeys) != 0;
-      ef &= ~kErrfLongKeys;
-    }
-    if (ef & ERRF_OVERFLOW) return fail(c, MRHBM_E_OVERFLOW, "u32 partial sum overflow while combining a hot key");
-    if (ef & ERRF_CAPACITY) {  // skewed keys: the exact layout from now on
-      c->sb.stride = 0;
+    if (!shared_ok) {  // peer mapping unavailable (decided by all ranks together): NCCL exchange instead
       c->no_optimistic = true;
-      if ((ordered && S > 1) || nonuniform) c->no_ordered = true;  // key-ordered sub-bins overflowed, or would
       return 0;
     }
-    c->h_big.clear();
-    c->rv = v;
-    c->sb.stride = 0;
-    c->B = (uint32_t)Bl;
-    c->S = S;
-    c->ordered = ordered;
-    c->N = N_in;
-    c->N_recv = c->h_acc[0];
-    c->bin_base = c->pbase[me] * S;
-    c->groups = c->h_uoff[Bl];
-    c->shuffled = true;
-    c->compacted = false;
-    st.bins = (uint32_t)Bl;
-    st.sub_bins = S;
-    st.big_bins = 0;
-    st.groups = c->groups;
-    st.bytes_exchanged = (c->h_acc[0] - c->h_acc[1]) * (uint64_t)c->rb;
-    finish_stats(c, st);
-    // plan = level 1, exchange = the fill-level all-gather (waits for the slowest rank's level 1), scatter = level 2
-    // (on several GPUs: including the NVLink pulls)
-    c->stats.ms_exchange = ev_ms(c, EV_PLAN, EV_GATH);
-    c->stats.ms_scatter = ev_ms(c, EV_GATH, EV_SCATTER);
-    *done = true;
-    return MRHBM_OK;
+    if (G > 1) {
+      const uint64_t words = ((uint64_t)pl.C1 << c->ctr_shift) * G;
+      rc = grow(c, &c->l1all_cap, words, words + words / 4, {{(void**)&c->d_l1all, sizeof(uint32_t)}});
+      if (rc) return rc;
+    }
   }
+  pl.cursor1 = c->sb.hist;
+  pl.cursor = c->sb.cursor;
+  pl.l1 = single_level ? c->sb.mid : c->regions;
+  pl.mid = c->sb.mid;
+  pl.err_flags = c->sb.counters + CNT_ERR;
+  pl.ticket = c->sb.counters + 5;  // (words 5 and 6 of the 8 counters cleared below)
+  pl.base_off = nullptr;
+  for (int r = 0; r < 8; r++) pl.peer[r] = (unsigned long long)(uintptr_t)(G == 1 ? (r == 0 ? c->regions : nullptr) : c->peer_regions[r]);
+  pl.l1_counts = G == 1 ? c->sb.hist : c->d_l1all;
+  pl.l1_zstride = G == 1 ? 0 : ((uint64_t)pl.C1 << c->ctr_shift);
+  const BinParams bp = make_bp(c, S, ordered);
+  st.attempts++;
+  CU(c, cudaMemsetAsync(c->sb.hist, 0, (((uint64_t)pl.C1) << c->ctr_shift) * sizeof(uint32_t), s));
+  if (!single_level) CU(c, cudaMemsetAsync(c->sb.cursor, 0, (std::max<uint64_t>(Bl, 1) << c->ctr_shift) * sizeof(uint32_t), s));
+  CU(c, cudaMemsetAsync(c->sb.counters, 0, 8 * sizeof(uint32_t), s));
+  CU(c, cudaEventRecord(c->ev[EV_COMBINE], s));
+  CU(c, cudaEventRecord(c->ev[EV_HIST], s));
+  for (auto& r : live) st.launches += launch_split_l1(c->rb, r.p, r.n, bp, pl, s);
+  CU(c, cudaEventRecord(c->ev[EV_PLAN], s));
+  if (G > 1) {
+    rc = comm_allgather_u32(c->comm, c->sb.hist, c->d_l1all, (size_t)pl.C1 << c->ctr_shift, s, &c->err);
+    if (rc) return rc;
+  }
+  CU(c, cudaEventRecord(c->ev[EV_GATH], s));
+  if (!single_level) st.launches += launch_split_l2(c->rb, bp, pl, s);
+  CU(c, cudaEventRecord(c->ev[EV_SCATTER], s));
+  CU(c, cudaEventRecord(c->ev[EV_EXCH], s));
+  c->sb.src = c->sb.mid;
+  c->sb.nseg = 1;
+  c->sb.stride = bin_stride;
+  c->sb.out_stride = c->cap;
+  c->sb.ctr_shift = c->ctr_shift;
+  // single level: the level-1 cursors ARE the fine fill levels
+  uint32_t* fine_cursor = single_level ? c->sb.hist : c->sb.cursor;
+  ShuffleBuffers v = c->sb;
+  v.cursor = fine_cursor;
+  set_range_hint(v, S, ordered);
+  if (Bl) st.launches += launch_sort_reduce(c->rb, v, (uint32_t)Bl, c->cap, c->sm_count, s);
+  CU(c, cudaEventRecord(c->ev[EV_SORT], s));
+  CU(c, cudaEventRecord(c->ev[EV_BIG], s));
+  c->h_uoff.assign(Bl + 1, 0);
+  if (Bl) {
+    st.launches += launch_exscan(c->sb.ucount, (uint32_t)Bl, c->sb.uoff, nullptr, nullptr, 0xffffffffu, nullptr, nullptr,
+                                 c->sb.counters + CNT_TOTAL, 0, s, c->d_small + 64);
+    CU(c, cudaMemcpyAsync(c->h_uoff.data(), c->sb.uoff, (Bl + 1) * 4, cudaMemcpyDeviceToHost, s));
+  }
+  // pairs this rank reduced (and how many of them came from peers)
+  st.launches += launch_region_totals(pl.l1_counts, pl.l1_zstride, (uint32_t)G, (uint32_t)me, pl.rbase[me], pl.C1_local,
+                                      c->ctr_shift, (uint32_t)std::min<uint64_t>(single_level ? bin_stride : pl.sub_stride, 0xffffffffull),
+                                      c->d_acc, s);
+  CU(c, cudaMemcpyAsync(c->h_acc, c->d_acc, 8 * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
+  CU(c, cudaMemcpyAsync(c->h_counters, c->sb.counters, 8 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+  CU(c, cudaEventRecord(c->ev[EV_END], s));
+  CU(c, cudaGetLastError());
+  CU(c, cudaStreamSynchronize(s));
+  uint32_t ef = c->h_counters[CNT_ERR];
+  rc = agree_flags(c, &ef);  // (several GPUs: also, nobody leaves while a peer still reads its regions)
+  if (rc) return rc;
+  if (ef & ERRF_CAPACITY) {  // skewed keys: the exact layout from now on
+    c->sb.stride = 0;
+    c->no_optimistic = true;
+    if ((ordered && S > 1) || nonuniform) c->no_ordered = true;  // key-ordered sub-bins overflowed, or would
+    return 0;
+  }
+  c->h_big.clear();
+  c->sb.stride = 0;
+  st.bytes_exchanged = (c->h_acc[0] - c->h_acc[1]) * (uint64_t)c->rb;
+  *done = true;
+  // plan = level 1, exchange = the fill-level all-gather (waits for the slowest rank's level 1), scatter = level 2
+  // (on several GPUs: including the NVLink pulls)
+  return publish(c, v, Bl, S, ordered, N_in, c->h_acc[0], c->pbase[me] * S, 0, st, ev_ms(c, EV_PLAN, EV_GATH),
+                 ev_ms(c, EV_GATH, EV_SCATTER));
 }
 
 // ---- one GPU, exact layout: hist -> scan -> scatter -> sort+reduce (skewed keys, oversized bins) ---------
@@ -1440,61 +1407,31 @@ int shuffle_single_exact(mrhbm_ctx* c, std::vector<Src>& live, uint64_t N, uint6
   for (int widen = 0;; widen++) {
     B = (uint64_t)P * S;
     if (B >= (1ull << 31)) return fail(c, MRHBM_E_INVAL, "too many bins");
-    const uint64_t Bv = B;
-    rc = ensure_buffers(c, Bv, N);
+    rc = ensure_buffers(c, B, N);
     if (rc) return rc;
     ordered = ((c->cfg.key_kind == MRHBM_KEY_U64 && !(c->cfg.flags & MRHBM_F_FORCE_RUNS) && widen == 0 && !skip_ordered) || S == 1);
     c->sb.stride = 0;
-    for (int attempt = 0;; attempt++) {
+    for (;;) {
       st.attempts++;
       BinParams bp = make_bp(c, S, ordered);
-      CU(c, cudaMemsetAsync(c->sb.hist, 0, (Bv << c->ctr_shift) * sizeof(uint32_t), s));
+      CU(c, cudaMemsetAsync(c->sb.hist, 0, (B << c->ctr_shift) * sizeof(uint32_t), s));
       CU(c, cudaMemsetAsync(c->sb.counters, 0, 8 * sizeof(uint32_t), s));
       CU(c, cudaEventRecord(c->ev[EV_COMBINE], s));
       for (auto& r : live) st.launches += launch_hist(c->rb, r.p, r.n, bp, c->sb.hist, s);
       CU(c, cudaEventRecord(c->ev[EV_HIST], s));
-      st.launches += launch_exscan(c->sb.hist, (uint32_t)Bv, c->sb.bin_off, c->sb.cursor, nullptr, c->cap, c->sb.big_list,
+      st.launches += launch_exscan(c->sb.hist, (uint32_t)B, c->sb.bin_off, c->sb.cursor, nullptr, c->cap, c->sb.big_list,
                                    c->sb.counters + CNT_NBIG, c->sb.counters + CNT_TOTAL, c->ctr_shift, s, c->d_small + 64);
       CU(c, cudaMemcpyAsync(c->h_counters, c->sb.counters, 8 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
       CU(c, cudaEventRecord(c->ev[EV_PROBE], s));
       CU(c, cudaEventRecord(c->ev[EV_PLAN], s));
-      {
-        // exact layout through the two-level coalesced split when there are enough bins (claims relative
-        // to bin_off); else the direct scatter
-        uint32_t F = 1;
-        while ((uint64_t)F * F < B) F <<= 1;
-        uint32_t C1 = (uint32_t)((B + F - 1) / F);
-        if (B >= 2048 && F <= 1024 && C1 <= 1024) {
-          rc = ensure_records(c, &c->l1buf, &c->l1_cap, N);
-          if (rc) return rc;
-          // relative fill levels: coarse levels live in hist (dead after the scan), fine levels in cursor
-          CU(c, cudaMemsetAsync(c->sb.hist, 0, ((uint64_t)C1 << c->ctr_shift) * sizeof(uint32_t), s));
-          CU(c, cudaMemsetAsync(c->sb.cursor, 0, (B << c->ctr_shift) * sizeof(uint32_t), s));
-          SplitPlan pl{};
-          pl.B = (uint32_t)B;
-          pl.F = F;
-          pl.C1 = pl.C1_local = C1;
-          pl.cap = c->cap;
-          pl.cursor1 = c->sb.hist;
-          pl.cursor = c->sb.cursor;
-          pl.l1 = c->l1buf;
-          pl.mid = c->sb.mid;
-          pl.err_flags = c->sb.counters + CNT_ERR;
-          pl.base_off = c->sb.bin_off;
-          pl.ndest = 1;
-          for (auto& r : live) st.launches += launch_split_l1(c->rb, r.p, r.n, bp, pl, s);
-          st.launches += launch_split_l2(c->rb, bp, pl, s);
-        } else {
-          for (auto& r : live) st.launches += launch_scatter(c->rb, r.p, r.n, bp, c->sb.cursor, c->sb.mid, s);
-        }
-      }
+      rc = exact_split(c, live, bp, B, N, st);
+      if (rc) return rc;
       CU(c, cudaEventRecord(c->ev[EV_SCATTER], s));
       CU(c, cudaEventRecord(c->ev[EV_EXCH], s));
       c->sb.src = c->sb.mid;
       c->sb.nseg = 1;
       c->sb.seg_off[0] = c->sb.bin_off;
       c->sb.seg_base[0] = 0;
-      c->sb.rep_shift = 0;
       set_range_hint(c->sb, S, ordered);
       st.launches += launch_sort_reduce(c->rb, c->sb, (uint32_t)B, c->cap, c->sm_count, s);
       CU(c, cudaEventRecord(c->ev[EV_SORT], s));
@@ -1509,25 +1446,11 @@ int shuffle_single_exact(mrhbm_ctx* c, std::vector<Src>& live, uint64_t N, uint6
       }
       break;
     }
-    st.launches += launch_big_bins(c->rb, c->sb, nbig, c->cap, s);
-    CU(c, cudaEventRecord(c->ev[EV_BIG], s));
-    c->h_big.clear();
-    if (c->sb.no_reduce && nbig) {
-      c->h_big.resize(nbig);
-      CU(c, cudaMemcpyAsync(c->h_big.data(), c->sb.big_list, nbig * 4, cudaMemcpyDeviceToHost, s));
-    }
-    st.launches += launch_exscan(c->sb.ucount, (uint32_t)B, c->sb.uoff, nullptr, nullptr, 0xffffffffu, nullptr, nullptr,
-                                 c->sb.counters + CNT_TOTAL, 0, s, c->d_small + 64);
-    c->h_bin_off.resize(B + 1);
-    c->h_uoff.resize(B + 1);
-    CU(c, cudaMemcpyAsync(c->h_bin_off.data(), c->sb.bin_off, (B + 1) * 4, cudaMemcpyDeviceToHost, s));
-    CU(c, cudaMemcpyAsync(c->h_uoff.data(), c->sb.uoff, (B + 1) * 4, cudaMemcpyDeviceToHost, s));
-    CU(c, cudaMemcpyAsync(c->h_counters, c->sb.counters, 8 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
-    CU(c, cudaEventRecord(c->ev[EV_END], s));
-    CU(c, cudaGetLastError());
-    CU(c, cudaStreamSynchronize(s));
+    rc = exact_tail(c, c->sb, B, nbig, st);
+    if (rc) return rc;
     uint32_t ef = c->h_counters[CNT_ERR];
-    if (ef & ERRF_OVERFLOW) return fail(c, MRHBM_E_OVERFLOW, "u32 partial sum overflow while combining a hot key");
+    rc = agree_flags(c, &ef);
+    if (rc) return rc;
     if (ef & ERRF_SKEW) {
       if (widen < 4 && (uint64_t)P * S * 2 < (1ull << 31)) {
         S *= 2;
@@ -1537,23 +1460,7 @@ int shuffle_single_exact(mrhbm_ctx* c, std::vector<Src>& live, uint64_t N, uint6
     }
     break;
   }
-  c->rv = c->sb;
-  c->B = (uint32_t)B;
-  c->S = S;
-  c->ordered = ordered;
-  c->N = N_in;
-  c->N_recv = N;
-  c->bin_base = 0;
-  c->groups = c->h_uoff[B];
-  c->shuffled = true;
-  c->compacted = false;
-  st.bins = (uint32_t)B;
-  st.sub_bins = S;
-  st.big_bins = nbig;
-  st.groups = c->groups;
-  st.ms_exchange = 0;
-  finish_stats(c, st);
-  return MRHBM_OK;
+  return publish(c, c->sb, B, S, ordered, N_in, N, 0, nbig, st, 0.f, ev_ms(c, EV_PLAN, EV_SCATTER));
 }
 
 // ---- several GPUs, exact layout: hist -> all-gather counts -> scatter (destination-major) -> NCCL all-to-all
@@ -1561,8 +1468,9 @@ int shuffle_single_exact(mrhbm_ctx* c, std::vector<Src>& live, uint64_t N, uint6
 int shuffle_multi_exact(mrhbm_ctx* c, std::vector<Src>& live, uint64_t N, uint64_t N_in, mrhbm_stats& st) {
   const int G = c->world, me = c->rank;
   const uint32_t P = c->cfg.num_partitions;
+  const uint32_t n32 = (uint32_t)N;
   uint32_t all[8];
-  int rc = gather_u32(c, (uint32_t)N, all);
+  int rc = gather_words(c, &n32, 1, all);
   if (rc) return rc;
   uint64_t Nglobal = 0;
   for (int r = 0; r < G; r++) Nglobal += all[r];
@@ -1583,7 +1491,7 @@ int shuffle_multi_exact(mrhbm_ctx* c, std::vector<Src>& live, uint64_t N, uint64
     if (rc) return rc;
     ordered = ((c->cfg.key_kind == MRHBM_KEY_U64 && !(c->cfg.flags & MRHBM_F_FORCE_RUNS) && widen == 0 && !c->no_ordered) || S == 1);
     c->sb.stride = 0;
-    for (int attempt = 0;; attempt++) {
+    for (;;) {
       st.attempts++;
       BinParams bp = make_bp(c, S, ordered);
       CU(c, cudaMemsetAsync(c->sb.hist, 0, (B << c->ctr_shift) * sizeof(uint32_t), s));
@@ -1607,34 +1515,8 @@ int shuffle_multi_exact(mrhbm_ctx* c, std::vector<Src>& live, uint64_t N, uint64
       CU(c, cudaMemcpyAsync(c->h_small + 32, c->d_small + 32, 4 * G, cudaMemcpyDeviceToHost, s));
       CU(c, cudaMemcpyAsync(c->h_counters, c->sb.counters, 8 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
       CU(c, cudaEventRecord(c->ev[EV_PLAN], s));
-      {
-        // send buffer (destination-major exact layout) through the two-level coalesced split
-        uint32_t F = 1;
-        while ((uint64_t)F * F < B) F <<= 1;
-        uint32_t C1 = (uint32_t)((B + F - 1) / F);
-        if (B >= 2048 && F <= 1024 && C1 <= 1024) {
-          rc = ensure_records(c, &c->l1buf, &c->l1_cap, N);
-          if (rc) return rc;
-          CU(c, cudaMemsetAsync(c->sb.hist, 0, ((uint64_t)C1 << c->ctr_shift) * sizeof(uint32_t), s));
-          CU(c, cudaMemsetAsync(c->sb.cursor, 0, (B << c->ctr_shift) * sizeof(uint32_t), s));
-          SplitPlan pl{};
-          pl.B = (uint32_t)B;
-          pl.F = F;
-          pl.C1 = pl.C1_local = C1;
-          pl.cap = c->cap;
-          pl.cursor1 = c->sb.hist;
-          pl.cursor = c->sb.cursor;
-          pl.l1 = c->l1buf;
-          pl.mid = c->sb.mid;
-          pl.err_flags = c->sb.counters + CNT_ERR;
-          pl.base_off = c->sb.bin_off;
-          pl.ndest = 1;
-          for (auto& r : live) st.launches += launch_split_l1(c->rb, r.p, r.n, bp, pl, s);
-          st.launches += launch_split_l2(c->rb, bp, pl, s);
-        } else {
-          for (auto& r : live) st.launches += launch_scatter(c->rb, r.p, r.n, bp, c->sb.cursor, c->sb.mid, s);
-        }
-      }
+      rc = exact_split(c, live, bp, B, N, st);  // into the send buffer
+      if (rc) return rc;
       CU(c, cudaEventRecord(c->ev[EV_SCATTER], s));
       CU(c, cudaGetLastError());
       CU(c, cudaStreamSynchronize(s));
@@ -1679,7 +1561,6 @@ int shuffle_multi_exact(mrhbm_ctx* c, std::vector<Src>& live, uint64_t N, uint64
     CU(c, cudaEventRecord(c->ev[EV_EXCH], s));
     v = c->sb;
     v.stride = 0;
-    v.rep_shift = 0;
     v.bin_off = c->d_outoff;
     v.src = c->recvbuf;
     v.mid = nbig ? c->bigbuf : c->recvbuf;
@@ -1698,32 +1579,12 @@ int shuffle_multi_exact(mrhbm_ctx* c, std::vector<Src>& live, uint64_t N, uint64
     }
     st.launches += launch_sort_reduce(c->rb, v, (uint32_t)Bl, c->cap, c->sm_count, s);
     CU(c, cudaEventRecord(c->ev[EV_SORT], s));
-    st.launches += launch_big_bins(c->rb, v, nbig, c->cap, s);
-    CU(c, cudaEventRecord(c->ev[EV_BIG], s));
-    c->h_big.clear();
-    if (c->sb.no_reduce && nbig) {  // group-only mode: the iterator merges the runs of an oversized bin
-      c->h_big.resize(nbig);
-      CU(c, cudaMemcpyAsync(c->h_big.data(), c->sb.big_list, nbig * 4, cudaMemcpyDeviceToHost, s));
-    }
-    st.launches += launch_exscan(c->sb.ucount, (uint32_t)Bl, c->sb.uoff, nullptr, nullptr, 0xffffffffu, nullptr, nullptr,
-                                 c->sb.counters + CNT_TOTAL, 0, s, c->d_small + 64);
-    c->h_bin_off.resize(Bl + 1);
-    c->h_uoff.resize(Bl + 1);
-    CU(c, cudaMemcpyAsync(c->h_bin_off.data(), c->d_outoff, (Bl + 1) * 4, cudaMemcpyDeviceToHost, s));
-    CU(c, cudaMemcpyAsync(c->h_uoff.data(), c->sb.uoff, (Bl + 1) * 4, cudaMemcpyDeviceToHost, s));
-    CU(c, cudaMemcpyAsync(c->h_counters, c->sb.counters, 8 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
-    CU(c, cudaEventRecord(c->ev[EV_END], s));
-    CU(c, cudaGetLastError());
-    CU(c, cudaStreamSynchronize(s));
-    uint32_t ef = c->h_counters[CNT_ERR];
-    rc = gather_u32(c, ef | (c->long_jobs.empty() ? 0u : kErrfLongKeys), all);  // every rank must take the same branch
+    rc = exact_tail(c, v, Bl, nbig, st);
     if (rc) return rc;
-    uint32_t ef_any = 0;
-    for (int r = 0; r < G; r++) ef_any |= all[r];
-    c->any_long = (ef_any & kErrfLongKeys) != 0;
-    ef_any &= ~kErrfLongKeys;
-    if (ef_any & ERRF_OVERFLOW) return fail(c, MRHBM_E_OVERFLOW, "u32 partial sum overflow while combining a hot key");
-    if (ef_any & ERRF_SKEW) {
+    uint32_t ef = c->h_counters[CNT_ERR];
+    rc = agree_flags(c, &ef);
+    if (rc) return rc;
+    if (ef & ERRF_SKEW) {
       if (widen < 4 && (uint64_t)P * S * 2 < (1ull << 31)) {
         S *= 2;
         continue;
@@ -1732,24 +1593,8 @@ int shuffle_multi_exact(mrhbm_ctx* c, std::vector<Src>& live, uint64_t N, uint64
     }
     break;
   }
-  c->rv = v;
-  c->B = (uint32_t)Bl;
-  c->S = S;
-  c->ordered = ordered;
-  c->N = N_in;
-  c->N_recv = total_recv;
-  c->bin_base = c->pbase[me] * S;
-  c->groups = c->h_uoff[Bl];
-  c->shuffled = true;
-  c->compacted = false;
-  st.bins = (uint32_t)Bl;
-  st.sub_bins = S;
-  st.big_bins = nbig;
-  st.groups = c->groups;
-  st.ms_exchange = ev_ms(c, EV_SCATTER, EV_EXCH);
-  finish_stats(c, st);
-  c->stats.ms_exchange = st.ms_exchange;
-  return MRHBM_OK;
+  return publish(c, v, Bl, S, ordered, N_in, total_recv, c->pbase[me] * S, nbig, st, ev_ms(c, EV_SCATTER, EV_EXCH),
+                 ev_ms(c, EV_PLAN, EV_SCATTER));
 }
 
 // partition p -> local slot on this rank, or -1 when another rank owns it
@@ -1761,24 +1606,15 @@ inline int64_t slot_of(const mrhbm_ctx* c, uint32_t p) {
 
 namespace {
 // ---- keys longer than a record slot: partitioned, exchanged and grouped on the host --------------------------
-std::string unescape_key(const std::string& esc) {
-  std::string raw;
-  raw.reserve(esc.size());
-  for (size_t i = 0; i < esc.size(); i++) {
-    if (esc[i] == 1 && i + 1 < esc.size())
-      raw.push_back((char)(esc[++i] - 1));
-    else
-      raw.push_back(esc[i]);
-  }
-  return raw;
-}
 // the partition bin_of (mrhbm_dev.cuh) would give the key if it fitted a slot: FNV-in-doubles over the ORIGINAL bytes
 // (examples/WordCount/partitionfn.lua:8-16), or the word hash over the little-endian words of the STORED bytes
 uint32_t host_partition(const mrhbm_ctx* c, const std::string& esc) {
   const uint32_t P = c->cfg.num_partitions;
   if (c->cfg.partitioner == MRHBM_PART_FNV_LUA) {
+    std::vector<unsigned char> raw;
+    unescape(esc.data(), esc.size(), raw);
     uint32_t h = 2166136261u;
-    for (unsigned char b : unescape_key(esc)) h = fnv_lua_step(h, b);
+    for (unsigned char b : raw) h = fnv_lua_step(h, b);
     return h % P;
   }
   uint64_t h = 0x9E3779B97F4A7C15ull;
@@ -1817,7 +1653,8 @@ int build_long_groups(mrhbm_ctx* c) {
             // then the blobs padded to the largest
     if (!c->any_long) return MRHBM_OK;
     if (blob.size() >= (1u << 28)) return fail(c, MRHBM_E_NOMEM, "more than 1 GB of long keys on one rank");
-    int rc = gather_u32(c, (uint32_t)blob.size(), sizes.data());
+    const uint32_t words = (uint32_t)blob.size();
+    int rc = gather_words(c, &words, 1, sizes.data());
     if (rc) return rc;
     uint32_t mx = 0;
     for (int r = 0; r < G; r++) mx = std::max(mx, sizes[r]);
@@ -1895,7 +1732,7 @@ int mrhbm_shuffle(mrhbm_ctx* c) {
   int rc = collect_sources(c, live, &N, st);
   if (rc) return rc;
   CU(c, cudaEventRecord(c->ev[EV_CSTART], c->stream));
-  if (!c->no_optimistic && !(c->cfg.flags & MRHBM_F_NO_OPTIMISTIC) && !(c->tune & 1u)) {
+  if (!c->no_optimistic && !(c->cfg.flags & MRHBM_F_NO_OPTIMISTIC)) {
     bool done = false;
     rc = shuffle_fast(c, live, N, N_in, st, &done);
     if (rc) return rc;
@@ -2098,8 +1935,7 @@ int mrhbm_groups_next(mrhbm_iter* it, const void** key, size_t* klen, const uint
     }
     if (take) {
       it->long_pos++;
-      const std::string raw = unescape_key(lg.esc);
-      it->unesc.assign(raw.begin(), raw.end());
+      unescape(lg.esc.data(), lg.esc.size(), it->unesc);
       *key = it->unesc.data();
       *klen = it->unesc.size();
       *values = lg.values.data();
@@ -2136,14 +1972,8 @@ int mrhbm_groups_next(mrhbm_iter* it, const void** key, size_t* klen, const uint
     *klen = 8;
   } else {
     size_t len = strnlen((const char*)k, c->kb);
-    if (memchr(k, 1, len)) {  // escaped 0x00 / 0x01 bytes (see mrhbm_emit_str)
-      it->unesc.clear();
-      for (size_t i = 0; i < len; i++) {
-        if (k[i] == 1 && i + 1 < len)
-          it->unesc.push_back((unsigned char)(k[++i] - 1));
-        else
-          it->unesc.push_back(k[i]);
-      }
+    if (memchr(k, 1, len)) {  // escaped 0x00 / 0x01 bytes
+      unescape(k, len, it->unesc);
       k = it->unesc.data();
       len = it->unesc.size();
     }

@@ -19,7 +19,6 @@
 namespace mrhbm {
 
 static int g_sm_count = 132;
-static uint32_t g_tune = 0;  // MRHBM_TUNE measurement hooks (set once by kernels_set_tune)
 
 // ============================================================================
 // synthetic device-side mapfn
@@ -184,7 +183,7 @@ __global__ void __launch_bounds__(256) k_hist(const uint4* __restrict__ recs, ui
     for (int k = 0; k < U; k++) {
       if (base + k * stride < n) {
         uint32_t bin = bin_of<RB>(w[k], bp, nullptr);
-        atomicAdd(hist + (((((size_t)bin) << bp.rep_shift) | (blockIdx.x & ((1u << bp.rep_shift) - 1u))) << bp.ctr_shift), 1u);  // RED
+        atomicAdd(hist + ((size_t)bin << bp.ctr_shift), 1u);  // RED
       }
     }
   }
@@ -205,7 +204,7 @@ __global__ void __launch_bounds__(256) k_scatter(const uint4* __restrict__ recs,
     for (int k = 0; k < U; k++) {
       if (base + k * stride < n) {
         uint32_t bin = bin_of<RB>(w[k], bp, nullptr);
-        pos[k] = atomicAdd(cursor + (((((size_t)bin) << bp.rep_shift) | (blockIdx.x & ((1u << bp.rep_shift) - 1u))) << bp.ctr_shift), 1u);
+        pos[k] = atomicAdd(cursor + ((size_t)bin << bp.ctr_shift), 1u);
       }
     }
 #pragma unroll
@@ -276,16 +275,13 @@ struct SplitArgs {
   uint32_t level;         // 1 or 2
   uint32_t ctr_shift;
   uint32_t* err_flags;
-  // exact layout (after k_hist + k_exscan): bin f starts at base_off[f << rep_shift]; nullptr = the
-  // optimistic fixed-stride layout
+  // exact layout (after k_hist + k_exscan): bin f starts at base_off[f]; nullptr = the optimistic fixed-stride layout
   const uint32_t* base_off;
-  uint32_t rep_shift;
   uint32_t B;
   // optimistic layout: rank d owns the coarse regions [rbase[d], rbase[d+1]) = its fine bins
   // [fbase[d], fbase[d+1]) in blocks of F (one GPU: rbase = {0, C1}, fbase = {0, B})
   uint32_t rbase[9], fbase[9];
   uint32_t ndest, me;
-  unsigned long long* span;  // measurement hook or nullptr (SplitPlan::span)
   uint32_t* ticket;          // level 1, optimistic layout: {next tile - gridDim.x, CTAs that have left}, both 0 at launch
 };
 
@@ -355,12 +351,6 @@ __global__ void __launch_bounds__(THREADS_, MINB) k_split_tma(SplitArgs a, BinPa
   const uint32_t level = SPEC ? (uint32_t)(SPEC & 3) : a.level;
   const bool exact = SPEC ? false : a.base_off != nullptr;
   const bool multi = SPEC ? (SPEC & 4) != 0 : a.ndest > 1;
-  if (a.span && tid == 0 && level == 1) {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    atomicMin(a.span + 0, t);  // first CTA start
-    atomicMax(a.span + 2, t);  // last CTA start
-  }
 #pragma unroll
   for (int i = 0; i < 9; i++)
     if (tid == (uint32_t)i) {
@@ -374,7 +364,7 @@ __global__ void __launch_bounds__(THREADS_, MINB) k_split_tma(SplitArgs a, BinPa
     coarse = blockIdx.y;
     if (exact) {  // the coarse region is the union of its fine bins
       uint32_t f0 = coarse * a.F, f1 = f0 + a.F < a.B ? f0 + a.F : a.B;
-      uint32_t o0 = a.base_off[(size_t)f0 << a.rep_shift], o1 = a.base_off[(size_t)f1 << a.rep_shift];
+      uint32_t o0 = a.base_off[f0], o1 = a.base_off[f1];
       src += (size_t)o0 * R::kVec;
       n = o1 - o0;
     }
@@ -529,7 +519,7 @@ __global__ void __launch_bounds__(THREADS_, MINB) k_split_tma(SplitArgs a, BinPa
         uint32_t gg = g[i], first;
         if (exact) {  // absolute start of the destination region, always large enough
           const uint32_t f = level == 1 ? b * a.F : dbin;
-          first = a.base_off[(size_t)f << a.rep_shift];
+          first = a.base_off[f];
         } else {
           first = dbin * (uint32_t)a.dst_stride;
           if (gg + v[i] > a.capacity) {
@@ -612,12 +602,6 @@ __global__ void __launch_bounds__(THREADS_, MINB) k_split_tma(SplitArgs a, BinPa
       a.ticket[0] = 0;
       a.ticket[1] = 0;
     }
-  }
-  if (a.span && tid == 0 && level == 1) {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    atomicMax(a.span + 1, t);  // last CTA end
-    atomicMin(a.span + 3, t);  // first CTA end
   }
 }
 
@@ -980,15 +964,10 @@ __device__ __forceinline__ void gtab_add_long(bool active, uint32_t* __restrict_
 template <int RB, bool CHECKED>
 __global__ void __launch_bounds__(kCombineThreads, 1)
     k_combine(const uint4* __restrict__ recs, uint64_t n, uint32_t pf_trips, uint32_t vcap, uint32_t* __restrict__ gtab,
-              uint32_t glog, uint32_t* __restrict__ flags, uint32_t tune) {
+              uint32_t glog, uint32_t* __restrict__ flags) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   using R = Rec<RB>;
   constexpr int W = R::kWords, KW = R::kKeyWords;
-  if ((tune & 64u) && threadIdx.x == 0) {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    atomicMin((unsigned long long*)(flags + 8), t);
-  }
   constexpr int KC = KW < 3 ? KW : 3;  // key words of a shared-table entry: only keys of up to 12 bytes live there
   // Shared table, ARRAY PER FIELD (32 lanes probing 32 random entries hit 32 random banks, not the four a record
   // stride allows): tag[e] = 0 empty / 1 being written / the key's 32-bit hash with bit 1 set; val[e] = u32 partial
@@ -1109,11 +1088,11 @@ __global__ void __launch_bounds__(kCombineThreads, 1)
   // the pair of the NEXT trip is requested before this one is processed.  Index arithmetic of the loop: running
   // 64-bit pointers and 32-bit trip bounds (the kernel is issue bound; the per-trip 64-bit index, bounds checks and
   // prefetch address were a visible share of its instructions)
-  const uint32_t span = (uint32_t)(slice_hi - slice_lo);                                    // pairs of this CTA (< 2^32)
-  const uint32_t my_trips = tid < span ? (span - tid + blockDim.x - 1) / blockDim.x : 0u;   // trips in which this thread has a pair
+  const uint32_t npairs = (uint32_t)(slice_hi - slice_lo);                                  // pairs of this CTA (< 2^32)
+  const uint32_t my_trips = tid < npairs ? (npairs - tid + blockDim.x - 1) / blockDim.x : 0u;  // trips in which this thread has a pair
   // the warp's 32 pairs of trip t + pf_trips lie inside the slice for t < pf_ok
   const uint32_t wbase = (tid & ~31u) + 32u;
-  const uint32_t pf_full = span >= wbase ? (span - wbase) / blockDim.x + 1u : 0u;          // trips whose 32 pairs are all there
+  const uint32_t pf_full = npairs >= wbase ? (npairs - wbase) / blockDim.x + 1u : 0u;      // trips whose 32 pairs are all there
   const uint32_t pf_ok = pf_full > pf_trips ? pf_full - pf_trips : 0u;
   const uint4* p_next = recs + (slice_lo + tid) * R::kVec;                                  // this thread's pair of the next trip
   const uint4* p_pf = recs + (slice_lo + (tid & ~31u) + (uint64_t)pf_trips * blockDim.x) * R::kVec;  // the warp's prefetch target
@@ -1210,12 +1189,6 @@ __global__ void __launch_bounds__(kCombineThreads, 1)
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) vmax = max(vmax, __shfl_xor_sync(0xffffffffu, vmax, o));
   if (lane == 0 && vmax) atomicMax(flags + 2, vmax);
-  if ((tune & 64u) && threadIdx.x == 0) {  // measurement hook: when does the first CTA end, when the last?
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    atomicMax((unsigned long long*)(flags + 8) + 1, t);
-    atomicMin((unsigned long long*)(flags + 8) + 2, t);
-  }
 }
 
 // one record per non-empty entry of the global table (short entries first, then the long ones), appended to out
@@ -1430,8 +1403,6 @@ static inline int stream_grid(uint64_t n, int threads, int ctas_per_sm) {
   return (int)(need < cap ? (need ? need : 1) : cap);
 }
 
-void kernels_set_tune(uint32_t bits) { g_tune = bits; }
-
 cudaError_t kernels_configure() {
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
@@ -1531,14 +1502,13 @@ uint64_t gtab_bytes_host(int rb, uint32_t glog) { return gtab_bytes(rb, glog); }
 int launch_combine(int rb, const void* recs, uint64_t n, uint32_t* gtab, uint32_t glog, uint32_t* flags, bool checked,
                    int sm_count, cudaStream_t s) {
   if (!n) return 0;
-  const uint32_t pf_trips = (g_tune >> 8) & 0xffu ? (g_tune >> 8) & 0xffu : (uint32_t)kPrefetchTrips;  // (MRHBM_TUNE bits 8-15: override)
   // the shared table only takes values whose per-CTA sum cannot wrap 32 bits
   const uint64_t per_cta = (n + sm_count - 1) / sm_count + kCombineThreads;
   const uint32_t vcap = (uint32_t)std::min<uint64_t>(0xffffull, 0xffffffefull / per_cta);
   if (checked) {
-    DISPATCH_RB(rb, (k_combine<RB, true><<<sm_count, kCombineThreads, kCombineSmem, s>>>((const uint4*)recs, n, pf_trips, vcap, gtab, glog, flags, g_tune)));
+    DISPATCH_RB(rb, (k_combine<RB, true><<<sm_count, kCombineThreads, kCombineSmem, s>>>((const uint4*)recs, n, (uint32_t)kPrefetchTrips, vcap, gtab, glog, flags)));
   } else {
-    DISPATCH_RB(rb, (k_combine<RB, false><<<sm_count, kCombineThreads, kCombineSmem, s>>>((const uint4*)recs, n, pf_trips, vcap, gtab, glog, flags, g_tune)));
+    DISPATCH_RB(rb, (k_combine<RB, false><<<sm_count, kCombineThreads, kCombineSmem, s>>>((const uint4*)recs, n, (uint32_t)kPrefetchTrips, vcap, gtab, glog, flags)));
   }
   return 1;
 }
@@ -1580,14 +1550,12 @@ int launch_scatter(int rb, const void* recs, uint64_t n, const BinParams& bp, ui
 static SplitArgs split_args(const BinParams& bp, const SplitPlan& pl) {
   SplitArgs a{};
   a.base_off = pl.base_off;
-  a.rep_shift = bp.rep_shift;
   a.B = pl.B;
   a.F = pl.F;
   a.logF = 0;
   while ((1u << a.logF) < pl.F) a.logF++;
   a.ctr_shift = bp.ctr_shift;
   a.err_flags = pl.err_flags;
-  a.span = pl.span;
   a.ticket = pl.ticket;
   a.ndest = pl.base_off ? 1u : pl.ndest;
   a.me = pl.base_off ? 0u : pl.me;

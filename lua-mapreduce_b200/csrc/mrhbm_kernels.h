@@ -24,8 +24,6 @@ struct BinParams {
   uint32_t world;        // 1 = single GPU (slot == p)
   uint32_t wshift;       // log2(world) when world is a power of two, else 0xffffffff
   uint32_t pbase[9];
-  uint32_t rep_shift;    // few, heavily hit bins: 2^rep_shift counter copies per bin (copy = CTA id),
-                         // i.e. bin b owns the consecutive virtual bins [b << rep_shift, (b+1) << rep_shift)
 };
 
 MRHBM_HD inline uint32_t partition_slot(const BinParams& bp, uint32_t pid) {
@@ -66,22 +64,20 @@ struct ShuffleBuffers {
   // min/max pass.  hint_S = 0: unknown.
   uint32_t hint_S;
   uint64_t hint_q;     // floor(2^64 / S)
-  uint32_t rep_shift;  // bin_off / seg_off are indexed by virtual bin = bin << rep_shift
   uint32_t no_reduce;  // MRHBM_RED_NONE: every pair is its own output row (sorted, grouped on the host)
-  unsigned long long* span;  // measurement hook or nullptr: k_sort_reduce_u64's first CTA start, last CTA end, -, first CTA end
 };
 MRHBM_HD inline uint64_t bin_start(const ShuffleBuffers& b, uint32_t bin) {
-  return b.stride ? (uint64_t)bin * b.stride : (uint64_t)b.bin_off[(size_t)bin << b.rep_shift];
+  return b.stride ? (uint64_t)bin * b.stride : (uint64_t)b.bin_off[bin];
 }
 MRHBM_HD inline uint64_t out_start(const ShuffleBuffers& b, uint32_t bin) {
-  return b.stride ? (uint64_t)bin * b.out_stride : (uint64_t)b.bin_off[(size_t)bin << b.rep_shift];
+  return b.stride ? (uint64_t)bin * b.out_stride : (uint64_t)b.bin_off[bin];
 }
 MRHBM_HD inline uint32_t bin_count(const ShuffleBuffers& b, uint32_t bin) {
   if (b.stride) {
     uint32_t c = b.cursor[(size_t)bin << b.ctr_shift];
     return c < b.stride ? c : b.stride;
   }
-  return b.bin_off[(size_t)(bin + 1) << b.rep_shift] - b.bin_off[(size_t)bin << b.rep_shift];
+  return b.bin_off[bin + 1] - b.bin_off[bin];
 }
 enum { CNT_NBIG = 0, CNT_TICKET = 1, CNT_ERR = 2, CNT_TOTAL = 3, CNT_GBIG = 4 };
 enum { ERRF_SKEW = 1, ERRF_OVERFLOW = 2, ERRF_CAPACITY = 4, ERRF_KEYLEN = 8 };
@@ -152,7 +148,6 @@ struct SplitPlan {
   const uint32_t* l1_counts;  // level 2: fill of region r on rank z at l1_counts[z * l1_zstride + (r << ctr_shift)]
   uint64_t l1_zstride;
   uint32_t* ticket;           // two zeroed words: level 1 hands out its tiles from a counter (the kernel zeroes them again)
-  unsigned long long* span;   // measurement hook (MRHBM_TUNE bit 6) or nullptr: level 1's first CTA start, last CTA end, last CTA start, first CTA end (%globaltimer ns)
 };
 int launch_split_l1(int rb, const void* recs, uint64_t n, const BinParams& bp, const SplitPlan& pl, cudaStream_t s);
 int launch_split_l2(int rb, const BinParams& bp, const SplitPlan& pl, cudaStream_t s);
@@ -164,7 +159,6 @@ int launch_compact(int rb, const ShuffleBuffers& b, uint32_t B, void* dst_keys, 
 int launch_checksum_in(int rb, const void* recs, uint64_t n, uint64_t* acc4, cudaStream_t s);
 int launch_checksum_out(int rb, const ShuffleBuffers& b, uint32_t B, const BinParams& bp, uint32_t bin_base,
                         uint64_t* acc6, cudaStream_t s);
-void kernels_set_tune(uint32_t bits);  // measurement hooks (MRHBM_TUNE), read once at mrhbm_init
 cudaError_t kernels_configure();  // opt-in shared memory sizes; call once per device
 
 }  // namespace mrhbm

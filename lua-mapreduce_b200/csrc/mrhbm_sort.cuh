@@ -447,7 +447,7 @@ __global__ void __launch_bounds__(kSortThreads, 2) k_sort_reduce(ShuffleBuffers 
       load_bin(sm.rec, src, cnt * Rec<RB>::kVec);
     } else {
       for (uint32_t sgm = 0; sgm < b.nseg; sgm++) {
-        uint32_t so = b.seg_off[sgm][(size_t)bin << b.rep_shift], sc = b.seg_off[sgm][(size_t)(bin + 1) << b.rep_shift] - so;
+        uint32_t so = b.seg_off[sgm][bin], sc = b.seg_off[sgm][bin + 1] - so;
         const uint4* src = (const uint4*)b.src + (b.seg_base[sgm] + so) * Rec<RB>::kVec;
         load_bin(sm.rec + filled * Rec<RB>::kVec, src, sc * Rec<RB>::kVec);
         filled += sc;
@@ -586,8 +586,8 @@ __global__ void __launch_bounds__(kSortThreads, 2) k_sort_reduce_u64(ShuffleBuff
   auto desc_load = [&](uint32_t bn, uint32_t& so, uint32_t& sn) {
     so = sn = 0;
     if (MULTI && warp == 0 && lane < nseg && bn < B) {
-      so = b.seg_off[lane][(size_t)bn << b.rep_shift];
-      sn = b.seg_off[lane][(size_t)(bn + 1) << b.rep_shift];
+      so = b.seg_off[lane][bn];
+      sn = b.seg_off[lane][bn + 1];
     }
   };
   auto rec_addr = [&](uint32_t i, uint64_t off1) -> const uint4* {
@@ -597,11 +597,6 @@ __global__ void __launch_bounds__(kSortThreads, 2) k_sort_reduce_u64(ShuffleBuff
     return src + s_addr[sg] + i;
   };
 
-  if (b.span && tid == 0) {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    atomicMin(b.span, t);
-  }
   uint32_t bin = blockIdx.x;
   uint64_t off = 0;
   uint32_t cnt = 0;
@@ -839,12 +834,6 @@ __global__ void __launch_bounds__(kSortThreads, 2) k_sort_reduce_u64(ShuffleBuff
     ticket[0] = 0;
     ticket[1] = 0;
   }
-  if (b.span && tid == 0) {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    atomicMax(b.span + 1, t);
-    atomicMin(b.span + 3, t);
-  }
 }
 
 // One CTA per oversized bin (hot keys): chunk-wise in-place reduce until the bin fits.
@@ -858,7 +847,7 @@ __global__ void __launch_bounds__(kSortThreads, 2) k_big_bins(ShuffleBuffers b, 
   if (b.src != b.mid) {  // after an exchange: make the bin contiguous inside the (free) send buffer
     uint64_t filled = 0;
     for (uint32_t sgm = 0; sgm < b.nseg; sgm++) {
-      uint32_t so = b.seg_off[sgm][(size_t)bin << b.rep_shift], sc = b.seg_off[sgm][(size_t)(bin + 1) << b.rep_shift] - so;
+      uint32_t so = b.seg_off[sgm][bin], sc = b.seg_off[sgm][bin + 1] - so;
       const uint4* src = (const uint4*)b.src + (b.seg_base[sgm] + so) * Rec<RB>::kVec;
       for (uint64_t v = threadIdx.x; v < (uint64_t)sc * Rec<RB>::kVec; v += blockDim.x)
         base[filled * Rec<RB>::kVec + v] = src[v];
