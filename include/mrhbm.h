@@ -35,7 +35,7 @@ enum { /* error codes */
   MRHBM_E_NOMEM = -3,     /* host or device allocation failed */
   MRHBM_E_KEY = -4,       /* key does not fit: a fixed-width record or result slot, a word of the device tokeniser, > 1 MB */
   MRHBM_E_SKEW = -5,      /* a bin holds more distinct keys than one SM can sort (see DESIGN.md) */
-  MRHBM_E_OVERFLOW = -6,  /* u32 partial sum overflow while combining string-keyed records */
+  MRHBM_E_OVERFLOW = -6,  /* reserved, no longer returned: sums are u64 on every path, exact up to 2^53 */
   MRHBM_E_NCCL = -7,      /* NCCL missing or failed */
   MRHBM_E_NODEVICE = -8   /* no usable sm_90 GPU: there is no CPU path */
 };

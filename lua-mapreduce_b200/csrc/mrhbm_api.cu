@@ -1032,14 +1032,12 @@ struct Src {
 constexpr uint32_t kGtabLog = 21;       // global combiner table: 2^21 16-byte entries = 32 MB, resident in the 50 MB L2
 constexpr uint32_t kGtabMaxExtra = 5;   // ... grown up to 32x (1 GB) when the keys do not fit
 
-int overflow_error(mrhbm_ctx* c) {
-  return fail(c, MRHBM_E_OVERFLOW, "u32 partial sum overflow while combining a hot key");
-}
-
 // The pairs the shuffle partitions: the committed pool ranges, or -- with a combiner declared
 // (job.lua:92-96,198-202) and enough pairs to pay for it -- one record per distinct key of this rank's pairs
 // with their sum (shared-memory table per SM + one L2-resident global table, see k_combine).  A rank-local
-// decision: the stages that follow only see "the pairs this rank contributes".  EV_START .. EV_CSTART.
+// decision: the stages that follow only see "the pairs this rank contributes".  The combiner never fails a
+// shuffle: when a string key's sum does not fit the u32 value of a combined record (or one value is too large
+// for the table's state word), this shuffle hands on the raw pairs instead.  EV_START .. EV_CSTART.
 int collect_sources(mrhbm_ctx* c, std::vector<Src>& srcs, uint64_t* N, mrhbm_stats& st) {
   srcs.clear();
   uint64_t n = 0;
@@ -1068,7 +1066,7 @@ int collect_sources(mrhbm_ctx* c, std::vector<Src>& srcs, uint64_t* N, mrhbm_sta
     CU(c, cudaMemcpyAsync(c->h_small, c->d_small, 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
     CU(c, cudaStreamSynchronize(s));
     const uint32_t ef = c->h_small[0];
-    if (ef & ERRF_OVERFLOW) return overflow_error(c);
+    if (ef & ERRF_OVERFLOW) return 0;  // not sticky: the next shuffle's sums may fit again
     if (ef & ERRF_SKEW) {  // the table filled up: more distinct keys than it takes
       if (c->gtab_extra < kGtabMaxExtra) {
         c->gtab_extra++;
@@ -1100,8 +1098,7 @@ uint32_t pick_sub_bins(const mrhbm_ctx* c, uint64_t n_total, uint32_t copies = 1
 }
 
 // The error flags of an attempt, OR-ed over all ranks: every rank must take the same branch.  The all-gather also
-// tells every rank whether any rank holds long keys (c->any_long).  One GPU: *ef stays as it is.  A u32 sum that
-// wrapped on any rank is an error no retry fixes.
+// tells every rank whether any rank holds long keys (c->any_long).  One GPU: *ef stays as it is.
 int agree_flags(mrhbm_ctx* c, uint32_t* ef) {
   if (c->world > 1) {
     const uint32_t mine = *ef | (c->long_jobs.empty() ? 0u : kErrfLongKeys);
@@ -1112,7 +1109,7 @@ int agree_flags(mrhbm_ctx* c, uint32_t* ef) {
     c->any_long = (*ef & kErrfLongKeys) != 0;
     *ef &= ~kErrfLongKeys;
   }
-  return (*ef & ERRF_OVERFLOW) ? overflow_error(c) : 0;
+  return 0;
 }
 
 // Exact layout (bin offsets in sb.bin_off after k_hist + k_exscan): the records of `live` go to their B bins in sb.mid

@@ -741,7 +741,8 @@ __global__ void __launch_bounds__(1024) k_exscan_rows(const uint32_t* __restrict
 // The global table does not have to be perfect: two entries for one key only mean that the sort+reduce stage
 // adds them up, so reads of a slot another thread is publishing need no stronger ordering than "state first".
 // A full table raises ERRF_SKEW and the host retries with a larger one (not L2 resident any more) or without
-// the combiner; a u32 sum about to wrap raises ERRF_OVERFLOW (string records carry u32 values).
+// the combiner; a u32 sum about to wrap raises ERRF_OVERFLOW (string records carry u32 values), and the host then
+// hands the raw pairs on, whose sums the sort / reduce stages keep in u64.
 constexpr uint32_t kCombineLock = 0xffffffffu;
 constexpr int kCombineThreads = 1024;
 constexpr int kCombineSmem = 188 * 1024;  // (+ 38 KB of per-warp miss queues = 226 of the 227 KB)
@@ -1416,7 +1417,7 @@ cudaError_t kernels_configure() {
                            (int)sort_smem_bytes(RB));                                             \
   if (e != cudaSuccess) return e;                                                                 \
   e = cudaFuncSetAttribute(k_big_bins<RB>, cudaFuncAttributeMaxDynamicSharedMemorySize,          \
-                           (int)sort_smem_bytes(RB));                                             \
+                           (int)big_smem_bytes(RB));                                              \
   if (e != cudaSuccess) return e;                                                                 \
 
   CFG(16) CFG(32) CFG(64) CFG(128)
@@ -1650,7 +1651,7 @@ int launch_sort_reduce(int rb, const ShuffleBuffers& b, uint32_t B, uint32_t cap
 }
 int launch_big_bins(int rb, const ShuffleBuffers& b, uint32_t nbig, uint32_t cap, cudaStream_t s) {
   if (!nbig) return 0;
-  DISPATCH_RB(rb, (k_big_bins<RB><<<nbig, kSortThreads, sort_smem_bytes(RB), s>>>(b, cap)));
+  DISPATCH_RB(rb, (k_big_bins<RB><<<nbig, kSortThreads, big_smem_bytes(RB), s>>>(b, cap)));
   return 1;
 }
 int launch_compact(int rb, const ShuffleBuffers& b, uint32_t B, void* dst_keys, uint64_t* dst_sums,

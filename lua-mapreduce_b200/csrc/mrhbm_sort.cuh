@@ -32,6 +32,10 @@ __host__ __device__ inline size_t sort_smem_bytes(int rb) {
   size_t cap = kCapBytes / rb;
   return (size_t)kCapBytes * 2 + cap * 8 + 80 * 8 + cap * 2;
 }
+// k_big_bins: string keys carry the u64 values of the loaded chunk behind the carve (process_chunk_wide)
+__host__ __device__ inline size_t big_smem_bytes(int rb) {
+  return sort_smem_bytes(rb) + (rb == 16 ? 0 : (size_t)(kCapBytes / rb) * 8);
+}
 __device__ __forceinline__ SortSmem carve(unsigned char* base, int rb) {
   size_t cap = kCapBytes / rb;
   SortSmem s;
@@ -126,11 +130,22 @@ __device__ __forceinline__ void load_bin(uint4* dst, const uint4* __restrict__ s
 enum { MODE_FINAL = 0, MODE_PARTIAL = 1 };
 struct ChunkOut {
   void* keys;      // FINAL: key slots; PARTIAL: AoS records
-  uint64_t* sums;  // FINAL only
+  uint64_t* sums;  // FINAL; PARTIAL with string keys: the u64 partial sums beside the records
   uint64_t base;   // element offset into the destination
   uint32_t* err_flags;
   uint32_t no_reduce = 0;  // group-only mode: equal keys stay separate rows
+  const uint64_t* wide = nullptr;  // WIDE: the loaded chunk's values, indexed by each record's value word
 };
+
+// The value of a loaded record.  WIDE (k_big_bins, string keys): a merge round's partial sums pass 2^32, so the
+// record's u32 value word holds the index of its u64 value in out.wide instead.
+template <int RB, bool WIDE>
+__device__ __forceinline__ uint64_t chunk_value(const uint32_t* r, const ChunkOut& out) {
+  if constexpr (WIDE)
+    return out.wide[r[Rec<RB>::kKeyWords]];
+  else
+    return rec_value<RB>(r);
+}
 
 template <int RB, int MODE>
 __device__ __forceinline__ void write_group(const ChunkOut& out, uint64_t o, const uint32_t* r, uint64_t s) {
@@ -152,8 +167,7 @@ __device__ __forceinline__ void write_group(const ChunkOut& out, uint64_t o, con
       d[2] = (uint32_t)s;
       d[3] = (uint32_t)(s >> 32);
     } else {
-      if (s > 0xffffffffull) atomicOr(out.err_flags, (uint32_t)ERRF_OVERFLOW);
-      d[R::kKeyWords] = (uint32_t)s;
+      out.sums[o] = s;  // (the record's value word is rewritten when the next round loads it)
     }
   }
 }
@@ -162,7 +176,7 @@ __device__ __forceinline__ void write_group(const ChunkOut& out, uint64_t o, con
 // one u16 per position: on entry (HAVE_FLAGS) 1 for the first record of every key, else it is
 // computed here.  An in-place scan turns the flags into group numbers (a position is a head iff
 // the next number differs); each head sums its run and writes the group.
-template <int RB, int MODE, bool HAVE_FLAGS, typename At>
+template <int RB, int MODE, bool HAVE_FLAGS, bool WIDE, typename At>
 __device__ __forceinline__ uint32_t reduce_sorted(At at, uint32_t cnt, uint16_t* hs, const ChunkOut& out) {
   constexpr int CAP = kCapBytes / RB;
   constexpr int PER = (CAP + kSortThreads - 1) / kSortThreads;
@@ -180,11 +194,11 @@ __device__ __forceinline__ uint32_t reduce_sorted(At at, uint32_t cnt, uint16_t*
     uint32_t g = hs[j], gn = j + 1 < cnt ? hs[j + 1] : groups;
     if (gn == g) continue;  // not a head
     const uint32_t* r = at(j);
-    uint64_t s = rec_value<RB>(r);
+    uint64_t s = chunk_value<RB, WIDE>(r, out);
     for (uint32_t k = j + 1; k < cnt; k++) {  // the run: positions that do not start a group
       uint32_t a = hs[k], an = k + 1 < cnt ? hs[k + 1] : groups;
       if (an != a) break;
-      s += rec_value<RB>(at(k));
+      s += chunk_value<RB, WIDE>(at(k), out);
     }
     write_group<RB, MODE>(out, out.base + g, r, s);
   }
@@ -195,7 +209,7 @@ __device__ __forceinline__ uint32_t reduce_sorted(At at, uint32_t cnt, uint16_t*
 constexpr uint32_t kFixMax = 8;  // largest bucket the rank-among-mates step accepts
 constexpr uint32_t kNoFastPath = 0xffffffffu;
 
-template <int RB, int MODE>
+template <int RB, int MODE, bool WIDE>
 __device__ uint32_t counting_path(const SortSmem& sm, uint32_t cnt, uint64_t pmin, uint64_t pmax,
                                   const ChunkOut& out) {
   using R = Rec<RB>;
@@ -263,7 +277,7 @@ __device__ uint32_t counting_path(const SortSmem& sm, uint32_t cnt, uint64_t pmi
       uint32_t b = bucket_of(r);
       uint32_t s = bcnt[b], e = (b + 1 < NB) ? bcnt[b + 1] : cnt;
       uint32_t rank = 0, head = 1;
-      uint64_t sum = rec_value<RB>(r);
+      uint64_t sum = chunk_value<RB, WIDE>(r, out);
       if (e - s > 1) {  // most buckets hold one record
         for (uint32_t m = s; m < e; m++) {
           if (m == j) continue;
@@ -276,7 +290,7 @@ __device__ uint32_t counting_path(const SortSmem& sm, uint32_t cnt, uint64_t pmi
               rank++;
               if (!out.no_reduce) head = 0;  // an equal key sits earlier: not the first of its group
             } else if (!out.no_reduce) {
-              sum += rec_value<RB>(q);
+              sum += chunk_value<RB, WIDE>(q, out);
             }
           }
         }
@@ -301,7 +315,7 @@ __device__ uint32_t counting_path(const SortSmem& sm, uint32_t cnt, uint64_t pmi
 
 // Sorts cnt (<= cap) records of one bin by key, sums the values of equal keys and writes
 // the groups in ascending key order.  Returns the number of groups.
-template <int RB, int MODE>
+template <int RB, int MODE, bool WIDE = false>
 __device__ uint32_t process_loaded(const SortSmem& sm, uint32_t cnt, const ChunkOut& out, bool have_range = false,
                                    uint64_t lo = 0, uint64_t hi = 0);
 
@@ -315,8 +329,28 @@ __device__ uint32_t process_chunk(const SortSmem& sm, const uint4* __restrict__ 
   return process_loaded<RB, MODE>(sm, cnt, out);
 }
 
-// the bin's cnt records are in sm.rec (all threads have passed a barrier after the load)
+// k_big_bins, string keys: process_chunk with u64 values.  The chunk's values go to wide[] -- the records' own u32
+// values (side == nullptr: the bin's first round) or the partial sums an earlier round left in side[0, cnt) -- and
+// each record's value word becomes the index of its value there.  Every read of side[] happens before the barrier,
+// so the chunk may write its groups over the range it was loaded from.
 template <int RB, int MODE>
+__device__ uint32_t process_chunk_wide(const SortSmem& sm, uint64_t* wide, const uint4* __restrict__ src,
+                                       const uint64_t* side, uint32_t cnt, const ChunkOut& out) {
+  using R = Rec<RB>;
+  for (uint32_t v = threadIdx.x; v < cnt * R::kVec; v += blockDim.x) sm.rec[v] = src[v];
+  __syncthreads();
+  uint32_t* recw = (uint32_t*)sm.rec;
+  for (uint32_t i = threadIdx.x; i < cnt; i += blockDim.x) {
+    uint32_t* r = recw + i * R::kWords;
+    wide[i] = side ? side[i] : (uint64_t)r[R::kKeyWords];
+    r[R::kKeyWords] = i;
+  }
+  __syncthreads();
+  return process_loaded<RB, MODE, true>(sm, cnt, out);
+}
+
+// the bin's cnt records are in sm.rec (all threads have passed a barrier after the load)
+template <int RB, int MODE, bool WIDE>
 __device__ uint32_t process_loaded(const SortSmem& sm, uint32_t cnt, const ChunkOut& out, bool have_range,
                                    uint64_t lo, uint64_t hi) {
   using R = Rec<RB>;
@@ -324,7 +358,7 @@ __device__ uint32_t process_loaded(const SortSmem& sm, uint32_t cnt, const Chunk
   const uint32_t tid = threadIdx.x, T = blockDim.x;
   const uint32_t* recw = (const uint32_t*)sm.rec;
   if (have_range) {  // key-ordered sub-bin: the prefix range is known from the bin id
-    uint32_t g = counting_path<RB, MODE>(sm, cnt, lo, hi, out);
+    uint32_t g = counting_path<RB, MODE, WIDE>(sm, cnt, lo, hi, out);
     if (g != kNoFastPath) return g;
   }
   // range of the 64-bit key prefix
@@ -364,7 +398,7 @@ __device__ uint32_t process_loaded(const SortSmem& sm, uint32_t cnt, const Chunk
   pmax = sm.red[65];
   __syncthreads();
   {
-    uint32_t g = counting_path<RB, MODE>(sm, cnt, pmin, pmax, out);
+    uint32_t g = counting_path<RB, MODE, WIDE>(sm, cnt, pmin, pmax, out);
     if (g != kNoFastPath) return g;
   }
   // general path: bitonic sort of (prefix digit | index) words, whole-key passes on ties
@@ -418,7 +452,7 @@ __device__ uint32_t process_loaded(const SortSmem& sm, uint32_t cnt, const Chunk
   }
   const uint16_t* pp = perm;
   auto at = [&](uint32_t j) -> const uint32_t* { return recw + (uint32_t)pp[j] * R::kWords; };
-  return reduce_sorted<RB, MODE, false>(at, cnt, other, out);
+  return reduce_sorted<RB, MODE, false, WIDE>(at, cnt, other, out);
 }
 
 template <int RB>
@@ -836,7 +870,9 @@ __global__ void __launch_bounds__(kSortThreads, 2) k_sort_reduce_u64(ShuffleBuff
   }
 }
 
-// One CTA per oversized bin (hot keys): chunk-wise in-place reduce until the bin fits.
+// One CTA per oversized bin (hot keys): chunk-wise in-place reduce until the bin fits.  Sums are u64 on every round:
+// u64 keys keep them in the record, string keys (a u32 value word) in the bin's own range of out_sums,
+// [off, off + n), which no other bin writes and which the final round overwrites with the groups.
 template <int RB>
 __global__ void __launch_bounds__(kSortThreads, 2) k_big_bins(ShuffleBuffers b, uint32_t cap) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -867,13 +903,21 @@ __global__ void __launch_bounds__(kSortThreads, 2) k_big_bins(ShuffleBuffers b, 
     if (threadIdx.x == 0) b.ucount[bin] = n;
     return;
   }
+  uint64_t* side = b.out_sums + off;  // string keys: the partial sums of the records at base[0, n)
+  uint64_t* wide = (uint64_t*)(smem_raw + sort_smem_bytes(RB));
+  bool carried = false;               // ... once a merge round has written them
   while (n > cap) {
     uint32_t w = 0;
     for (uint32_t c = 0; c < n; c += cap) {
       uint32_t m = n - c < cap ? n - c : cap;
-      ChunkOut out{base, nullptr, w, b.counters + CNT_ERR};
+      ChunkOut out{base, side, w, b.counters + CNT_ERR};
+      out.wide = wide;
       // groups of a chunk never outnumber the records consumed so far: w + g <= c + m
-      w += process_chunk<RB, MODE_PARTIAL, false>(sm, base + (uint64_t)c * Rec<RB>::kVec, m, out);
+      if constexpr (Rec<RB>::kU64)
+        w += process_chunk<RB, MODE_PARTIAL, false>(sm, base + (uint64_t)c * Rec<RB>::kVec, m, out);
+      else
+        w += process_chunk_wide<RB, MODE_PARTIAL>(sm, wide, base + (uint64_t)c * Rec<RB>::kVec,
+                                                  carried ? side + c : nullptr, m, out);
       __threadfence_block();
     }
     if (w == n) {  // nothing merged: more distinct keys than one CTA can sort
@@ -884,9 +928,15 @@ __global__ void __launch_bounds__(kSortThreads, 2) k_big_bins(ShuffleBuffers b, 
       return;
     }
     n = w;
+    carried = true;
   }
   ChunkOut out{b.out_keys, b.out_sums, off, b.counters + CNT_ERR, b.no_reduce};
-  uint32_t g = process_chunk<RB, MODE_FINAL, false>(sm, base, n, out);
+  out.wide = wide;
+  uint32_t g;
+  if constexpr (Rec<RB>::kU64)
+    g = process_chunk<RB, MODE_FINAL, false>(sm, base, n, out);
+  else
+    g = process_chunk_wide<RB, MODE_FINAL>(sm, wide, base, carried ? side : nullptr, n, out);
   if (threadIdx.x == 0) b.ucount[bin] = g;
 }
 

@@ -176,3 +176,31 @@ def test_job_size_oracles_agree_with_the_flat_ones():
     wk1, ws1, wpo1 = O.wordcount_from_counts(counts, O.PART_FNV_LUA, 15, world=2, rank=1)
     sel = np.concatenate([np.arange(int(fpo[p]), int(fpo[p + 1])) for p in range(15) if p % 2 == 1])
     assert (wk1 == fk[sel]).all() and (ws1 == fs[sel]).all()
+
+
+@pytest.mark.parametrize("rb", [32, 64, 128])
+def test_groupby_rec_sums_past_32_bits(rb):
+    """the GPU suite checks string-key sums past 2^32 against O.groupby_rec: pin it against a plain dict sum with
+    values near 2^32 and sums up to about 2^45, keys up to the record class's full slot"""
+    rng = np.random.default_rng(rb)
+    kb = rb - 4
+    vocab = [b"k%d" % i + b"x" * int(rng.integers(0, kb - 6)) for i in range(300)] + [b"z" * kb, b"z" * (kb - 1)]
+    idx = np.concatenate([rng.integers(0, len(vocab), 20_000), np.full(8192, len(vocab) - 2)])  # one key: 2^13 pairs
+    vals = rng.integers(0xF0000000, 1 << 32, idx.size, dtype=np.uint64).astype(np.uint32)
+    recs = np.zeros(idx.size, dtype=[("key", "S%d" % kb), ("val", "<u4")])
+    recs["key"] = np.array(vocab, dtype="S%d" % kb)[idx]
+    recs["val"] = vals
+    P = 7
+    okeys, osum, po = O.groupby_rec(recs.view(np.uint8).reshape(idx.size, rb), O.PART_FNV_LUA, P)
+    want = {}
+    for k, v in zip(idx.tolist(), vals.tolist()):
+        want[vocab[k]] = want.get(vocab[k], 0) + v
+    assert max(want.values()) > 1 << 44
+    got = {}
+    for p in range(P):
+        ks = [bytes(k).rstrip(b"\0") for k in okeys[int(po[p]):int(po[p + 1])]]
+        assert ks == sorted(ks)
+        for k, s in zip(ks, osum[int(po[p]):int(po[p + 1])].tolist()):
+            assert O.part_fnv_lua(k, P) == p and k not in got
+            got[k] = s
+    assert got == want
