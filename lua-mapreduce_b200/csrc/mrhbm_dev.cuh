@@ -242,7 +242,7 @@ __device__ __forceinline__ void key_mix2(const uint32_t* r, uint64_t& f1, uint64
   f2 = mix64(b);
 }
 
-// ---- shared-memory hash tables of whole records (k_combine, k_agg_bins) --------------------
+// ---- shared-memory hash tables of whole records (k_combine) --------------------------------
 // 128-bit volatile shared loads: one or two per probe instead of a word-by-word compare (a
 // record-strided word access hits only 4 bank groups)
 __device__ __forceinline__ uint4 lds128_volatile(const uint4* p) {
@@ -287,6 +287,37 @@ __device__ __forceinline__ void stg_stream(uint4* p, const uint4& v) {
   asm volatile("st.global.L1::no_allocate.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(v.x),
                "r"(v.y), "r"(v.z), "r"(v.w)
                : "memory");
+}
+
+// ---- CTA-wide exclusive scan --------------------------------------------------
+// inclusive prefix sum of v over the first WIDTH lanes of the warp (a power of two <= 32)
+template <int WIDTH = 32>
+__device__ __forceinline__ uint32_t warp_inscan(uint32_t v) {
+  const uint32_t lane = threadIdx.x & 31;
+#pragma unroll
+  for (int d = 1; d < WIDTH; d <<= 1) {
+    const uint32_t t = __shfl_up_sync(0xffffffffu, v, d);
+    if (lane >= (uint32_t)d) v += t;
+  }
+  return v;
+}
+struct CtaScan {
+  uint32_t excl;   // sum of `mine` over the threads before this one
+  uint32_t total;  // sum of `mine` over the CTA
+};
+// One value per thread, THREADS == blockDim.x threads, one barrier: every warp scans the warp totals itself.
+// The warp totals live in static scratch that every call in the kernel shares: it may be written again only
+// after a barrier that follows every read of it (a barrier after the call, before the next call).
+template <int THREADS>
+__device__ __forceinline__ CtaScan cta_exscan(uint32_t mine) {
+  constexpr int kWarps = THREADS / 32;
+  __shared__ uint32_t s_warp[kWarps];
+  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const uint32_t incl = warp_inscan(mine);
+  if (lane == 31) s_warp[warp] = incl;
+  __syncthreads();
+  const uint32_t w = lane < (uint32_t)kWarps ? s_warp[lane] : 0u, wi = warp_inscan<kWarps>(w);
+  return {__shfl_sync(0xffffffffu, wi - w, warp) + incl - mine, __shfl_sync(0xffffffffu, wi, kWarps - 1)};
 }
 
 }  // namespace mrhbm

@@ -341,13 +341,12 @@ __global__ void __launch_bounds__(THREADS_, MINB) k_split_tma(SplitArgs a, BinPa
   __shared__ uint32_t scnt[kSplitMaxBins], soff[kSplitMaxBins];
   // this tile: the slot (record index in a.dst, 32-bit wrap-around arithmetic) output position 0 would have in the bin's run
   __shared__ uint32_t sbase[kSplitMaxBins];
-  __shared__ uint32_t wsum[THREADS / 32];
   __shared__ uint32_t s_rbase[9], s_fbase[9];  // (kernel-parameter arrays indexed by a register would be copied to local memory)
   __shared__ unsigned long long s_src[8];      // byte address and length (records) of the tile streams of this CTA
   __shared__ uint32_t s_n[8];
   __shared__ __align__(8) uint64_t mbar[2];
   __shared__ uint32_t s_next_len[2];
-  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const uint32_t tid = threadIdx.x;
   const uint32_t level = SPEC ? (uint32_t)(SPEC & 3) : a.level;
   const bool exact = SPEC ? false : a.base_off != nullptr;
   const bool multi = SPEC ? (SPEC & 4) != 0 : a.ndest > 1;
@@ -481,22 +480,8 @@ __global__ void __launch_bounds__(THREADS_, MINB) k_split_tma(SplitArgs a, BinPa
         g[i] = atomicAdd(a.cursor + ((size_t)dbin << a.ctr_shift), v[i]);  // result needed only after the placement
       }
     }
-    uint32_t incl = s;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      uint32_t t = __shfl_up_sync(0xffffffffu, incl, d);
-      if (lane >= (uint32_t)d) incl += t;
-    }
-    if (lane == 31) wsum[warp] = incl;
-    __syncthreads();
     {
-      uint32_t ws = lane < THREADS / 32 ? wsum[lane] : 0u, wi = ws;
-#pragma unroll
-      for (int d = 1; d < THREADS / 32; d <<= 1) {
-        uint32_t t = __shfl_up_sync(0xffffffffu, wi, d);
-        if (lane >= (uint32_t)d) wi += t;
-      }
-      uint32_t e = __shfl_sync(0xffffffffu, wi - ws, warp) + incl - s;
+      uint32_t e = cta_exscan<THREADS>(s).excl;
 #pragma unroll
       for (int i = 0; i < IPT; i++) {
         ex[i] = e;
@@ -605,38 +590,19 @@ __global__ void __launch_bounds__(THREADS_, MINB) k_split_tma(SplitArgs a, BinPa
   }
 }
 
-// single-CTA exclusive scan (B <= a few million): out_excl[0..n], optional copy into
+// single-CTA exclusive scan (B <= a few million, 1024 threads): out_excl[0..n], optional copy into
 // out_copy (scatter cursors), optional list of entries larger than cap
 __device__ __forceinline__ void exscan_body(const uint32_t* __restrict__ in, uint32_t n,
                                             uint32_t* __restrict__ out_excl, uint32_t* __restrict__ out_copy,
                                             uint32_t* __restrict__ out_dense, uint32_t cap,
                                             uint32_t* __restrict__ big_list, uint32_t* nbig, uint32_t* total,
                                             uint32_t shift) {
-  __shared__ uint32_t warp_sums[32];
   const uint32_t T = blockDim.x, tid = threadIdx.x;
   uint32_t per = (n + T - 1) / T;
   uint32_t b0 = tid * per, b1 = min(n, b0 + per);
   uint32_t s = 0;
   for (uint32_t i = b0; i < b1; i++) s += in[(size_t)i << shift];
-  uint32_t incl = s;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    uint32_t t = __shfl_up_sync(0xffffffffu, incl, d);
-    if ((tid & 31) >= (uint32_t)d) incl += t;
-  }
-  if ((tid & 31) == 31) warp_sums[tid >> 5] = incl;
-  __syncthreads();
-  if (tid < 32) {
-    uint32_t w = tid < (T >> 5) ? warp_sums[tid] : 0u, wi = w;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      uint32_t t = __shfl_up_sync(0xffffffffu, wi, d);
-      if (tid >= (uint32_t)d) wi += t;
-    }
-    warp_sums[tid] = wi - w;  // exclusive
-  }
-  __syncthreads();
-  uint32_t run = warp_sums[tid >> 5] + incl - s;
+  uint32_t run = cta_exscan<1024>(s).excl;
   for (uint32_t i = b0; i < b1; i++) {
     uint32_t c = in[(size_t)i << shift];
     out_excl[i] = run;
@@ -683,31 +649,19 @@ __global__ void __launch_bounds__(1024) k_exscan_apply(const uint32_t* __restric
                                                        uint32_t* __restrict__ out_dense, uint32_t cap,
                                                        uint32_t* __restrict__ big_list, uint32_t* nbig, uint32_t* total,
                                                        uint32_t shift, const uint32_t* __restrict__ partials) {
-  __shared__ uint32_t warp_sums[32], warp_pre[32];
-  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, i = blockIdx.x * 1024u + tid;
+  __shared__ uint32_t warp_pre[32];
+  const uint32_t tid = threadIdx.x, lane = tid & 31, i = blockIdx.x * 1024u + tid;
   uint32_t pre = 0;  // sum of the preceding blocks
   for (uint32_t b = tid; b < blockIdx.x; b += 1024u) pre += partials[b];
 #pragma unroll
   for (int d = 16; d > 0; d >>= 1) pre += __shfl_xor_sync(0xffffffffu, pre, d);
   const uint32_t c = i < n ? in[(size_t)i << shift] : 0u;
-  uint32_t incl = c;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    uint32_t t = __shfl_up_sync(0xffffffffu, incl, d);
-    if (lane >= (uint32_t)d) incl += t;
-  }
-  if (lane == 31) warp_sums[warp] = incl;
-  if (lane == 0) warp_pre[warp] = pre;
-  __syncthreads();
-  uint32_t w = warp_sums[lane], wi = w, p = warp_pre[lane];
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    uint32_t t = __shfl_up_sync(0xffffffffu, wi, d);
-    if (lane >= (uint32_t)d) wi += t;
-  }
+  if (lane == 0) warp_pre[tid >> 5] = pre;  // read behind the barrier of the scan
+  const uint32_t excl = cta_exscan<1024>(c).excl;
+  uint32_t p = warp_pre[lane];
 #pragma unroll
   for (int d = 16; d > 0; d >>= 1) p += __shfl_xor_sync(0xffffffffu, p, d);
-  const uint32_t run = p + __shfl_sync(0xffffffffu, wi - w, warp) + incl - c;  // exclusive prefix of element i
+  const uint32_t run = p + excl;  // exclusive prefix of element i
   if (i < n) {
     out_excl[i] = run;
     if (out_copy) out_copy[(size_t)i << shift] = run;
@@ -1412,15 +1366,12 @@ cudaError_t kernels_configure() {
   e = cudaGetDeviceProperties(&prop, dev);
   if (e != cudaSuccess) return e;
   g_sm_count = prop.multiProcessorCount;
-#define CFG(RB)                                                                                   \
-  e = cudaFuncSetAttribute(k_sort_reduce<RB>, cudaFuncAttributeMaxDynamicSharedMemorySize,       \
-                           (int)sort_smem_bytes(RB));                                             \
-  if (e != cudaSuccess) return e;                                                                 \
-  e = cudaFuncSetAttribute(k_big_bins<RB>, cudaFuncAttributeMaxDynamicSharedMemorySize,          \
-                           (int)big_smem_bytes(RB));                                              \
-  if (e != cudaSuccess) return e;                                                                 \
-
-  CFG(16) CFG(32) CFG(64) CFG(128)
+#define CFG(KERNEL, RB, BYTES)                                                                           \
+  e = cudaFuncSetAttribute(KERNEL<RB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BYTES(RB));      \
+  if (e != cudaSuccess) return e;
+  CFG(k_sort_reduce, 32, sort_smem_bytes) CFG(k_sort_reduce, 64, sort_smem_bytes) CFG(k_sort_reduce, 128, sort_smem_bytes)
+  CFG(k_big_bins, 16, big_smem_bytes) CFG(k_big_bins, 32, big_smem_bytes) CFG(k_big_bins, 64, big_smem_bytes)
+  CFG(k_big_bins, 128, big_smem_bytes)
 #undef CFG
 #define CFGS(M, X)                                                                                                       \
   e = cudaFuncSetAttribute(k_sort_reduce_u64<M, X>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sort_smem_bytes(16)); \
@@ -1646,7 +1597,11 @@ int launch_sort_reduce(int rb, const ShuffleBuffers& b, uint32_t B, uint32_t cap
     if (multi && minmax) k_sort_reduce_u64<true, true><<<grid, kSortThreads, sort_smem_bytes(16), s>>>(b, B, cap);
     return 1;
   }
-  DISPATCH_RB(rb, (k_sort_reduce<RB><<<grid, kSortThreads, sort_smem_bytes(RB), s>>>(b, B, cap)));
+  switch (rb) {
+    case 32: k_sort_reduce<32><<<grid, kSortThreads, sort_smem_bytes(32), s>>>(b, B, cap); break;
+    case 64: k_sort_reduce<64><<<grid, kSortThreads, sort_smem_bytes(64), s>>>(b, B, cap); break;
+    default: k_sort_reduce<128><<<grid, kSortThreads, sort_smem_bytes(128), s>>>(b, B, cap); break;
+  }
   return 1;
 }
 int launch_big_bins(int rb, const ShuffleBuffers& b, uint32_t nbig, uint32_t cap, cudaStream_t s) {

@@ -26,7 +26,8 @@ struct SortSmem {
   uint4* rec;     // cap records: the loaded bin, later the sorted bin
   uint4* rec2;    // cap records in bucket order (fast path) / permutations + flags (general path)
   uint32_t* cnt;  // 2*cap words: bucket counters -> offsets; general path: cap composite u64
-  uint64_t* red;  // 80 words of reduction / scan scratch
+  uint64_t* red;  // 80 words: process_loaded's min / max of the key prefixes
+  uint16_t* heads;  // cap u16: head flags -> group numbers in sorted order (fast path)
 };
 __host__ __device__ inline size_t sort_smem_bytes(int rb) {
   size_t cap = kCapBytes / rb;
@@ -43,6 +44,7 @@ __device__ __forceinline__ SortSmem carve(unsigned char* base, int rb) {
   s.rec2 = (uint4*)(base + kCapBytes);
   s.cnt = (uint32_t*)(base + 2 * kCapBytes);
   s.red = (uint64_t*)(base + 2 * kCapBytes + cap * 8);
+  s.heads = (uint16_t*)(s.red + 80);
   return s;
 }
 
@@ -67,11 +69,10 @@ __device__ __forceinline__ void bitonic_sort(uint64_t* comp, uint32_t n2) {
 }
 
 // in-place exclusive scan of a[0..n) by the whole CTA (thread t owns a[t*PER .. t*PER+PER)),
-// PER * blockDim.x >= n required; returns the total.  scratch: 33 words.
+// PER * kSortThreads >= n required; returns the total
 template <int PER, typename T_>
-__device__ __forceinline__ uint32_t block_exscan(T_* a, uint32_t n, uint32_t* /*unused*/) {
-  __shared__ uint32_t scratch[40];  // static: keeps the address arithmetic away from the carve
-  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
+__device__ __forceinline__ uint32_t block_exscan(T_* a, uint32_t n) {
+  const uint32_t tid = threadIdx.x;
   uint32_t v[PER];
   uint32_t s = 0;
 #pragma unroll
@@ -80,35 +81,88 @@ __device__ __forceinline__ uint32_t block_exscan(T_* a, uint32_t n, uint32_t* /*
     v[k] = i < n ? (uint32_t)a[i] : 0u;
     s += v[k];
   }
-  uint32_t incl = s;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    uint32_t t = __shfl_up_sync(0xffffffffu, incl, d);
-    if (lane >= (uint32_t)d) incl += t;
-  }
-  if (lane == 31) scratch[warp] = incl;
-  __syncthreads();
-  if (warp == 0) {
-    uint32_t w = lane < nwarps ? scratch[lane] : 0u, wi = w;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      uint32_t t = __shfl_up_sync(0xffffffffu, wi, d);
-      if (lane >= (uint32_t)d) wi += t;
-    }
-    scratch[lane] = wi - w;
-    if (lane == 31) scratch[32] = wi;
-  }
-  __syncthreads();
-  uint32_t run = scratch[warp] + incl - s;
+  const CtaScan sc = cta_exscan<kSortThreads>(s);
+  uint32_t run = sc.excl;
 #pragma unroll
   for (int k = 0; k < PER; k++) {
     uint32_t i = tid * PER + k;
     if (i < n) a[i] = (T_)run;
     run += v[k];
   }
-  uint32_t total = scratch[32];
   __syncthreads();
-  return total;
+  return sc.total;
+}
+// exclusive scan of a[0 .. 8*kSortThreads) in place, 8 consecutive words per thread; returns the total
+__device__ __forceinline__ uint32_t block_exscan_u32x8(uint32_t* a) {
+  const uint32_t tid = threadIdx.x;
+  uint4 x = ((const uint4*)a)[2 * tid], y = ((const uint4*)a)[2 * tid + 1];
+  const CtaScan sc = cta_exscan<kSortThreads>(x.x + x.y + x.z + x.w + y.x + y.y + y.z + y.w);
+  uint32_t run = sc.excl;
+  uint4 ox, oy;
+  ox.x = run; run += x.x;
+  ox.y = run; run += x.y;
+  ox.z = run; run += x.z;
+  ox.w = run; run += x.w;
+  oy.x = run; run += y.x;
+  oy.y = run; run += y.y;
+  oy.z = run; run += y.z;
+  oy.w = run;
+  ((uint4*)a)[2 * tid] = ox;
+  ((uint4*)a)[2 * tid + 1] = oy;
+  __syncthreads();
+  return sc.total;
+}
+// exclusive scan of the u16 flags a[0 .. 4*kSortThreads) in place (entries at index >= n count as 0)
+__device__ __forceinline__ uint32_t block_exscan_u16x4(uint16_t* a, uint32_t n) {
+  const uint32_t tid = threadIdx.x;
+  uint2 x = ((const uint2*)a)[tid];
+  uint32_t v0 = x.x & 0xffffu, v1 = x.x >> 16, v2 = x.y & 0xffffu, v3 = x.y >> 16;
+  const uint32_t i0 = 4 * tid;
+  v0 = i0 < n ? v0 : 0u;
+  v1 = i0 + 1 < n ? v1 : 0u;
+  v2 = i0 + 2 < n ? v2 : 0u;
+  v3 = i0 + 3 < n ? v3 : 0u;
+  const CtaScan sc = cta_exscan<kSortThreads>(v0 + v1 + v2 + v3);
+  const uint32_t e0 = sc.excl, e1 = e0 + v0, e2 = e1 + v1, e3 = e2 + v2;
+  ((uint2*)a)[tid] = make_uint2(e0 | (e1 << 16), e2 | (e3 << 16));
+  __syncthreads();
+  return sc.total;
+}
+
+// min of lo and max of hi over the CTA (kSortThreads threads), one barrier; the same reuse rule as cta_exscan
+__device__ __forceinline__ void cta_minmax_u64(uint64_t& lo, uint64_t& hi) {
+  constexpr uint32_t kWarps = kSortThreads / 32;
+  __shared__ uint64_t s_mm[2][kWarps];  // per-warp min / max
+  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  auto warp_minmax = [&]() {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const uint64_t l2 = __shfl_xor_sync(0xffffffffu, lo, o), h2 = __shfl_xor_sync(0xffffffffu, hi, o);
+      lo = l2 < lo ? l2 : lo;
+      hi = h2 > hi ? h2 : hi;
+    }
+  };
+  warp_minmax();
+  if (lane == 0) {
+    s_mm[0][warp] = lo;
+    s_mm[1][warp] = hi;
+  }
+  __syncthreads();
+  lo = lane < kWarps ? s_mm[0][lane] : ~0ull;
+  hi = lane < kWarps ? s_mm[1][lane] : 0ull;
+  warp_minmax();
+}
+
+// the source segments of `bin` in order (one per source rank after the all-to-all; one on a single GPU):
+// seg(first, src, n) for each, `first` = the records of the bin in the segments before it
+template <int RB, typename Seg>
+__device__ __forceinline__ void for_each_segment(const ShuffleBuffers& b, uint32_t bin, Seg seg) {
+  uint32_t first = 0;
+  for (uint32_t s = 0; s < b.nseg; s++) {
+    const uint32_t so = b.seg_off[s][bin], sc = b.seg_off[s][bin + 1] - so;
+    seg(first, (const uint4*)b.src + (b.seg_base[s] + so) * Rec<RB>::kVec, sc);
+    first += sc;
+  }
 }
 
 // coalesced copy of nvec uint4 from global to shared memory, four independent loads in
@@ -132,7 +186,6 @@ struct ChunkOut {
   void* keys;      // FINAL: key slots; PARTIAL: AoS records
   uint64_t* sums;  // FINAL; PARTIAL with string keys: the u64 partial sums beside the records
   uint64_t base;   // element offset into the destination
-  uint32_t* err_flags;
   uint32_t no_reduce = 0;  // group-only mode: equal keys stay separate rows
   const uint64_t* wide = nullptr;  // WIDE: the loaded chunk's values, indexed by each record's value word
 };
@@ -189,7 +242,7 @@ __device__ __forceinline__ uint32_t reduce_sorted(At at, uint32_t cnt, uint16_t*
     }
     __syncthreads();
   }
-  const uint32_t groups = block_exscan<PER>(hs, cnt, nullptr);
+  const uint32_t groups = block_exscan<PER>(hs, cnt);
   for (uint32_t j = tid; j < cnt; j += T) {
     uint32_t g = hs[j], gn = j + 1 < cnt ? hs[j + 1] : groups;
     if (gn == g) continue;  // not a head
@@ -220,7 +273,7 @@ __device__ uint32_t counting_path(const SortSmem& sm, uint32_t cnt, uint64_t pmi
   const uint32_t* recw = (const uint32_t*)sm.rec;
   const uint32_t* rec2w = (const uint32_t*)sm.rec2;
   uint32_t* bcnt = sm.cnt;
-  uint16_t* heads = (uint16_t*)sm.red + 4 * 80;  // CAP u16 after the scratch words (see sort_smem_bytes)
+  uint16_t* heads = sm.heads;
   uint64_t range = pmax - pmin;
   // monotone map prefix -> [0, NB): drop just enough low bits of (prefix - pmin)
   int bits = range ? 64 - __clzll((long long)range) : 0;
@@ -249,7 +302,7 @@ __device__ uint32_t counting_path(const SortSmem& sm, uint32_t cnt, uint64_t pmi
     }
   }
   if (__syncthreads_or(over)) return kNoFastPath;
-  block_exscan<ZPER>(bcnt, NB, (uint32_t*)sm.red);  // bcnt[b] = first position of bucket b
+  block_exscan<ZPER>(bcnt, NB);  // bcnt[b] = first position of bucket b
   // records into bucket order
 #pragma unroll
   for (int k = 0; k < ITEMS; k++) {
@@ -302,7 +355,7 @@ __device__ uint32_t counting_path(const SortSmem& sm, uint32_t cnt, uint64_t pmi
   }
   __syncthreads();
   constexpr int PER = (CAP + kSortThreads - 1) / kSortThreads;
-  const uint32_t groups = block_exscan<PER>(heads, cnt, nullptr);  // heads[f] = groups before sorted slot f
+  const uint32_t groups = block_exscan<PER>(heads, cnt);  // heads[f] = groups before sorted slot f
 #pragma unroll
   for (int k = 0; k < ITEMS; k++) {
     uint32_t j = tid + k * T;
@@ -316,15 +369,14 @@ __device__ uint32_t counting_path(const SortSmem& sm, uint32_t cnt, uint64_t pmi
 // Sorts cnt (<= cap) records of one bin by key, sums the values of equal keys and writes
 // the groups in ascending key order.  Returns the number of groups.
 template <int RB, int MODE, bool WIDE = false>
-__device__ uint32_t process_loaded(const SortSmem& sm, uint32_t cnt, const ChunkOut& out, bool have_range = false,
-                                   uint64_t lo = 0, uint64_t hi = 0);
+__device__ uint32_t process_loaded(const SortSmem& sm, uint32_t cnt, const ChunkOut& out);
 
-template <int RB, int MODE, bool NC>
+template <int RB, int MODE>
 __device__ uint32_t process_chunk(const SortSmem& sm, const uint4* __restrict__ src, uint32_t cnt,
                                   const ChunkOut& out) {
   using R = Rec<RB>;
   // coalesced load of the bin
-  for (uint32_t v = threadIdx.x; v < cnt * R::kVec; v += blockDim.x) sm.rec[v] = NC ? ldg_stream(src + v) : src[v];
+  for (uint32_t v = threadIdx.x; v < cnt * R::kVec; v += blockDim.x) sm.rec[v] = src[v];
   __syncthreads();
   return process_loaded<RB, MODE>(sm, cnt, out);
 }
@@ -351,16 +403,11 @@ __device__ uint32_t process_chunk_wide(const SortSmem& sm, uint64_t* wide, const
 
 // the bin's cnt records are in sm.rec (all threads have passed a barrier after the load)
 template <int RB, int MODE, bool WIDE>
-__device__ uint32_t process_loaded(const SortSmem& sm, uint32_t cnt, const ChunkOut& out, bool have_range,
-                                   uint64_t lo, uint64_t hi) {
+__device__ uint32_t process_loaded(const SortSmem& sm, uint32_t cnt, const ChunkOut& out) {
   using R = Rec<RB>;
   constexpr uint32_t CAP = kCapBytes / RB;
   const uint32_t tid = threadIdx.x, T = blockDim.x;
   const uint32_t* recw = (const uint32_t*)sm.rec;
-  if (have_range) {  // key-ordered sub-bin: the prefix range is known from the bin id
-    uint32_t g = counting_path<RB, MODE, WIDE>(sm, cnt, lo, hi, out);
-    if (g != kNoFastPath) return g;
-  }
   // range of the 64-bit key prefix
   uint64_t pmin = ~0ull, pmax = 0;
   for (uint32_t i = tid; i < cnt; i += T) {
@@ -368,6 +415,8 @@ __device__ uint32_t process_loaded(const SortSmem& sm, uint32_t cnt, const Chunk
     pmin = p < pmin ? p : pmin;
     pmax = p > pmax ? p : pmax;
   }
+  // (not cta_minmax_u64: inlined into k_sort_reduce_u64, its one-barrier form costs that kernel 32 more bytes of
+  // spills in its hot loop)
 #pragma unroll
   for (int d = 16; d > 0; d >>= 1) {
     uint64_t a = __shfl_xor_sync(0xffffffffu, pmin, d), b = __shfl_xor_sync(0xffffffffu, pmax, d);
@@ -397,10 +446,8 @@ __device__ uint32_t process_loaded(const SortSmem& sm, uint32_t cnt, const Chunk
   pmin = sm.red[64];
   pmax = sm.red[65];
   __syncthreads();
-  {
-    uint32_t g = counting_path<RB, MODE, WIDE>(sm, cnt, pmin, pmax, out);
-    if (g != kNoFastPath) return g;
-  }
+  const uint32_t g = counting_path<RB, MODE, WIDE>(sm, cnt, pmin, pmax, out);
+  if (g != kNoFastPath) return g;
   // general path: bitonic sort of (prefix digit | index) words, whole-key passes on ties
   uint64_t* comp = (uint64_t*)sm.cnt;
   uint16_t* perm = (uint16_t*)sm.rec2;
@@ -455,8 +502,10 @@ __device__ uint32_t process_loaded(const SortSmem& sm, uint32_t cnt, const Chunk
   return reduce_sorted<RB, MODE, false, WIDE>(at, cnt, other, out);
 }
 
+// string keys (u64 keys: k_sort_reduce_u64)
 template <int RB>
 __global__ void __launch_bounds__(kSortThreads, 2) k_sort_reduce(ShuffleBuffers b, uint32_t B, uint32_t cap) {
+  static_assert(!Rec<RB>::kU64, "u64 keys are sorted by k_sort_reduce_u64");
   extern __shared__ __align__(16) unsigned char smem_raw[];
   __shared__ uint32_t s_bin;
   SortSmem sm = carve(smem_raw, RB);
@@ -473,113 +522,29 @@ __global__ void __launch_bounds__(kSortThreads, 2) k_sort_reduce(ShuffleBuffers 
       if (threadIdx.x == 0) b.ucount[bin] = 0;
       continue;
     }
-    ChunkOut out{b.out_keys, b.out_sums, out_start(b, bin), b.counters + CNT_ERR, b.no_reduce};
-    // gather the bin's segments (one per source rank after the all-to-all; one on a single GPU)
-    uint32_t filled = 0;
+    ChunkOut out{b.out_keys, b.out_sums, out_start(b, bin), b.no_reduce};
     if (b.stride) {
-      const uint4* src = (const uint4*)b.src + off * Rec<RB>::kVec;
-      load_bin(sm.rec, src, cnt * Rec<RB>::kVec);
+      load_bin(sm.rec, (const uint4*)b.src + off * Rec<RB>::kVec, cnt * Rec<RB>::kVec);
     } else {
-      for (uint32_t sgm = 0; sgm < b.nseg; sgm++) {
-        uint32_t so = b.seg_off[sgm][bin], sc = b.seg_off[sgm][bin + 1] - so;
-        const uint4* src = (const uint4*)b.src + (b.seg_base[sgm] + so) * Rec<RB>::kVec;
-        load_bin(sm.rec + filled * Rec<RB>::kVec, src, sc * Rec<RB>::kVec);
-        filled += sc;
-      }
+      for_each_segment<RB>(b, bin, [&](uint32_t first, const uint4* src, uint32_t n) {
+        load_bin(sm.rec + first * Rec<RB>::kVec, src, n * Rec<RB>::kVec);
+      });
     }
     __syncthreads();
-    bool have_range = false;
-    uint64_t lo = 0, hi = 0;
-    if (Rec<RB>::kU64 && b.hint_S > 1) {  // sub = mulhi(key, S): keys of sub-bin `sub` lie in [sub*q, (sub+1)*(q+1)]
-      uint32_t sub = bin % b.hint_S;
-      have_range = true;
-      lo = (uint64_t)sub * b.hint_q;
-      hi = sub + 1 == b.hint_S ? ~0ull : (uint64_t)(sub + 1) * (b.hint_q + 1);
-    }
-    uint32_t g = process_loaded<RB, MODE_FINAL>(sm, cnt, out, have_range, lo, hi);
+    uint32_t g = process_loaded<RB, MODE_FINAL>(sm, cnt, out);
     if (threadIdx.x == 0) b.ucount[bin] = g;
   }
 }
 
-// ---- u64 keys, key-ordered sub-bins, one source segment: the software-pipelined variant ----
+// ---- u64 keys: the software-pipelined variant ----
 //
-// Same algorithm as counting_path, restructured around the two things the profile of
-// k_sort_reduce<16> showed (most stall samples wait at barriers, then on the bin load): the records
+// Same algorithm as counting_path, restructured around the two things the profile of the
+// shared-memory path on u64 keys showed (most stall samples wait at barriers, then on the bin load): the records
 // of a bin go from global memory into REGISTERS (4 x 16 B per thread), are counted from there and land
 // directly in bucket order, and the loads of the CTA's next bin are issued right after that, so they
 // fly while the current bin is ranked, scanned and written.
-// Bins are assigned round-robin (no ticket, no descriptor barrier); 7 barriers per bin instead of 14.
-
-// exclusive scan of a[0 .. 8*blockDim.x) in place, 8 consecutive words per thread; returns the total
-__device__ __forceinline__ uint32_t block_exscan_u32x8(uint32_t* a) {
-  __shared__ uint32_t scratch[32];
-  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
-  uint4 x = ((const uint4*)a)[2 * tid], y = ((const uint4*)a)[2 * tid + 1];
-  const uint32_t s = x.x + x.y + x.z + x.w + y.x + y.y + y.z + y.w;
-  uint32_t incl = s;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    uint32_t t = __shfl_up_sync(0xffffffffu, incl, d);
-    if (lane >= (uint32_t)d) incl += t;
-  }
-  if (lane == 31) scratch[warp] = incl;
-  __syncthreads();
-  // every warp scans the (<= 32) warp totals itself: no second barrier
-  uint32_t w = lane < nwarps ? scratch[lane] : 0u, wi = w;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    uint32_t t = __shfl_up_sync(0xffffffffu, wi, d);
-    if (lane >= (uint32_t)d) wi += t;
-  }
-  const uint32_t total = __shfl_sync(0xffffffffu, wi, 31);
-  uint32_t run = __shfl_sync(0xffffffffu, wi - w, warp) + incl - s;
-  uint4 ox, oy;
-  ox.x = run; run += x.x;
-  ox.y = run; run += x.y;
-  ox.z = run; run += x.z;
-  ox.w = run; run += x.w;
-  oy.x = run; run += y.x;
-  oy.y = run; run += y.y;
-  oy.z = run; run += y.z;
-  oy.w = run;
-  ((uint4*)a)[2 * tid] = ox;
-  ((uint4*)a)[2 * tid + 1] = oy;
-  __syncthreads();
-  return total;
-}
-// exclusive scan of the u16 flags a[0 .. 4*blockDim.x) in place (entries at index >= n count as 0)
-__device__ __forceinline__ uint32_t block_exscan_u16x4(uint16_t* a, uint32_t n) {
-  __shared__ uint32_t scratch[32];
-  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
-  uint2 x = ((const uint2*)a)[tid];
-  uint32_t v0 = x.x & 0xffffu, v1 = x.x >> 16, v2 = x.y & 0xffffu, v3 = x.y >> 16;
-  const uint32_t i0 = 4 * tid;
-  v0 = i0 < n ? v0 : 0u;
-  v1 = i0 + 1 < n ? v1 : 0u;
-  v2 = i0 + 2 < n ? v2 : 0u;
-  v3 = i0 + 3 < n ? v3 : 0u;
-  const uint32_t s = v0 + v1 + v2 + v3;
-  uint32_t incl = s;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    uint32_t t = __shfl_up_sync(0xffffffffu, incl, d);
-    if (lane >= (uint32_t)d) incl += t;
-  }
-  if (lane == 31) scratch[warp] = incl;
-  __syncthreads();
-  uint32_t w = lane < nwarps ? scratch[lane] : 0u, wi = w;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    uint32_t t = __shfl_up_sync(0xffffffffu, wi, d);
-    if (lane >= (uint32_t)d) wi += t;
-  }
-  const uint32_t total = __shfl_sync(0xffffffffu, wi, 31);
-  const uint32_t e0 = __shfl_sync(0xffffffffu, wi - w, warp) + incl - s;
-  const uint32_t e1 = e0 + v0, e2 = e1 + v1, e3 = e2 + v2;
-  ((uint2*)a)[tid] = make_uint2(e0 | (e1 << 16), e2 | (e3 << 16));
-  __syncthreads();
-  return total;
-}
+// Bins come from a ticket counter read ahead of time (below), so taking one adds no barrier; 7 barriers per bin
+// instead of 14.
 
 // MULTI: a bin is gathered from one segment per source rank (after the all-to-all); a small
 // descriptor (cumulative counts + rebased segment addresses) is built by warp 0 one bin ahead.
@@ -596,7 +561,7 @@ __global__ void __launch_bounds__(kSortThreads, 2) k_sort_reduce_u64(ShuffleBuff
   SortSmem sm = carve(smem_raw, RB);
   const uint32_t tid = threadIdx.x;
   uint32_t* bcnt = sm.cnt;
-  uint16_t* heads = (uint16_t*)sm.red + 4 * 80;
+  uint16_t* heads = sm.heads;
   const uint4* src = (const uint4*)b.src;
   const uint4 zero4 = make_uint4(0, 0, 0, 0);
   ((uint4*)bcnt)[2 * tid] = zero4;
@@ -606,12 +571,7 @@ __global__ void __launch_bounds__(kSortThreads, 2) k_sort_reduce_u64(ShuffleBuff
   const uint32_t lane = tid & 31, warp = tid >> 5, nseg = b.nseg;
   // warp 0: descriptor of bin `bn` from the per-source offsets (so, sn) each lane < nseg holds
   auto desc_store = [&](uint32_t so, uint32_t sn) {
-    uint32_t c = lane < nseg ? sn - so : 0u, incl = c;
-#pragma unroll
-    for (int d = 1; d < 8; d <<= 1) {
-      uint32_t t = __shfl_up_sync(0xffffffffu, incl, d);
-      if (lane >= (uint32_t)d) incl += t;
-    }
+    const uint32_t c = lane < nseg ? sn - so : 0u, incl = warp_inscan<8>(c);
     if (lane < nseg) {
       s_cum[lane] = incl - c;
       s_addr[lane] = b.seg_base[lane] + so - (incl - c);
@@ -646,7 +606,6 @@ __global__ void __launch_bounds__(kSortThreads, 2) k_sort_reduce_u64(ShuffleBuff
   const int bits_h = 64 - __clzll((long long)(b.hint_q + hint_S));
   const int sh0_h = bits_h > 32 ? bits_h - 32 : 0, sh1_h = (bits_h > kLogNB ? bits_h - kLogNB : 0) - sh0_h;
   uint32_t sub = bin % hint_S;
-  __shared__ unsigned long long s_mm[2][kSortThreads / 32];  // MINMAX: per-warp min / max of the bin's keys
   // After its first bin (blockIdx.x) a CTA takes the next bin nobody has from a ticket counter: the CTAs do not run at
   // one speed (with equal static shares the first CTA ends well before the last).  Thread 0
   // fetches a ticket two bins ahead and publishes (bin, bin % S) one bin ahead, so neither the L2 round trip nor the
@@ -692,39 +651,21 @@ __global__ void __launch_bounds__(kSortThreads, 2) k_sort_reduce_u64(ShuffleBuff
     if (cnt == 0 || cnt > cap) {  // empty, or oversized (k_big_bins): nothing was loaded
       if (cnt == 0 && tid == 0) b.ucount[bin] = 0;
     } else {
-      ChunkOut out{b.out_keys, b.out_sums, out_start(b, bin), b.counters + CNT_ERR, b.no_reduce};
+      ChunkOut out{b.out_keys, b.out_sums, out_start(b, bin), b.no_reduce};
       uint64_t pmin = (uint64_t)sub * b.hint_q;
       int sh0 = sh0_h, sh1 = sh1_h;
       if (MINMAX) {
-        unsigned long long lo = ~0ull, hi = 0ull;
+        uint64_t lo = ~0ull, hi = 0ull;
 #pragma unroll
         for (int k = 0; k < ITEMS; k++)
           if (tid + k * T < cnt) {
-            const unsigned long long key = (unsigned long long)rg[k].x | ((unsigned long long)rg[k].y << 32);
+            const uint64_t key = (uint64_t)rg[k].x | ((uint64_t)rg[k].y << 32);
             lo = key < lo ? key : lo;
             hi = key > hi ? key : hi;
           }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-          const unsigned long long l2 = __shfl_xor_sync(0xffffffffu, lo, o), h2 = __shfl_xor_sync(0xffffffffu, hi, o);
-          lo = l2 < lo ? l2 : lo;
-          hi = h2 > hi ? h2 : hi;
-        }
-        if (lane == 0) {
-          s_mm[0][warp] = lo;
-          s_mm[1][warp] = hi;
-        }
-        __syncthreads();
-        lo = lane < T / 32 ? s_mm[0][lane] : ~0ull;
-        hi = lane < T / 32 ? s_mm[1][lane] : 0ull;
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-          const unsigned long long l2 = __shfl_xor_sync(0xffffffffu, lo, o), h2 = __shfl_xor_sync(0xffffffffu, hi, o);
-          lo = l2 < lo ? l2 : lo;
-          hi = h2 > hi ? h2 : hi;
-        }
+        cta_minmax_u64(lo, hi);
         pmin = lo;
-        const unsigned long long range = hi - lo;
+        const uint64_t range = hi - lo;
         const int bits = range ? 64 - __clzll((long long)range) : 0;
         sh0 = bits > 32 ? bits - 32 : 0;
         sh1 = (bits > kLogNB ? bits - kLogNB : 0) - sh0;
@@ -749,7 +690,7 @@ __global__ void __launch_bounds__(kSortThreads, 2) k_sort_reduce_u64(ShuffleBuff
         for (int k = 0; k < ITEMS; k++)
           if (tid + k * T < cnt) sm.rec[tid + k * T] = rg[k];
         __syncthreads();
-        uint32_t g = process_loaded<RB, MODE_FINAL>(sm, cnt, out, false);
+        uint32_t g = process_loaded<RB, MODE_FINAL>(sm, cnt, out);
         if (tid == 0) b.ucount[bin] = g;
         __syncthreads();
         ((uint4*)bcnt)[2 * tid] = zero4;
@@ -881,14 +822,10 @@ __global__ void __launch_bounds__(kSortThreads, 2) k_big_bins(ShuffleBuffers b, 
   uint32_t off = (uint32_t)bin_start(b, bin), n = bin_count(b, bin);
   uint4* base = (uint4*)b.mid + (uint64_t)off * Rec<RB>::kVec;
   if (b.src != b.mid) {  // after an exchange: make the bin contiguous inside the (free) send buffer
-    uint64_t filled = 0;
-    for (uint32_t sgm = 0; sgm < b.nseg; sgm++) {
-      uint32_t so = b.seg_off[sgm][bin], sc = b.seg_off[sgm][bin + 1] - so;
-      const uint4* src = (const uint4*)b.src + (b.seg_base[sgm] + so) * Rec<RB>::kVec;
-      for (uint64_t v = threadIdx.x; v < (uint64_t)sc * Rec<RB>::kVec; v += blockDim.x)
-        base[filled * Rec<RB>::kVec + v] = src[v];
-      filled += sc;
-    }
+    for_each_segment<RB>(b, bin, [&](uint32_t first, const uint4* src, uint32_t sc) {
+      uint4* dst = base + (uint64_t)first * Rec<RB>::kVec;
+      for (uint64_t v = threadIdx.x; v < (uint64_t)sc * Rec<RB>::kVec; v += blockDim.x) dst[v] = src[v];
+    });
     __syncthreads();
   }
   if (b.no_reduce) {
@@ -897,8 +834,8 @@ __global__ void __launch_bounds__(kSortThreads, 2) k_big_bins(ShuffleBuffers b, 
     // iterator merges (it knows the oversized bins from big_list).
     for (uint32_t c = 0; c < n; c += cap) {
       uint32_t m = n - c < cap ? n - c : cap;
-      ChunkOut out{b.out_keys, b.out_sums, (uint64_t)off + c, b.counters + CNT_ERR, 1u};
-      process_chunk<RB, MODE_FINAL, false>(sm, base + (uint64_t)c * Rec<RB>::kVec, m, out);
+      ChunkOut out{b.out_keys, b.out_sums, (uint64_t)off + c, 1u};
+      process_chunk<RB, MODE_FINAL>(sm, base + (uint64_t)c * Rec<RB>::kVec, m, out);
     }
     if (threadIdx.x == 0) b.ucount[bin] = n;
     return;
@@ -910,11 +847,11 @@ __global__ void __launch_bounds__(kSortThreads, 2) k_big_bins(ShuffleBuffers b, 
     uint32_t w = 0;
     for (uint32_t c = 0; c < n; c += cap) {
       uint32_t m = n - c < cap ? n - c : cap;
-      ChunkOut out{base, side, w, b.counters + CNT_ERR};
+      ChunkOut out{base, side, w};
       out.wide = wide;
       // groups of a chunk never outnumber the records consumed so far: w + g <= c + m
       if constexpr (Rec<RB>::kU64)
-        w += process_chunk<RB, MODE_PARTIAL, false>(sm, base + (uint64_t)c * Rec<RB>::kVec, m, out);
+        w += process_chunk<RB, MODE_PARTIAL>(sm, base + (uint64_t)c * Rec<RB>::kVec, m, out);
       else
         w += process_chunk_wide<RB, MODE_PARTIAL>(sm, wide, base + (uint64_t)c * Rec<RB>::kVec,
                                                   carried ? side + c : nullptr, m, out);
@@ -930,11 +867,11 @@ __global__ void __launch_bounds__(kSortThreads, 2) k_big_bins(ShuffleBuffers b, 
     n = w;
     carried = true;
   }
-  ChunkOut out{b.out_keys, b.out_sums, off, b.counters + CNT_ERR, b.no_reduce};
+  ChunkOut out{b.out_keys, b.out_sums, off, b.no_reduce};
   out.wide = wide;
   uint32_t g;
   if constexpr (Rec<RB>::kU64)
-    g = process_chunk<RB, MODE_FINAL, false>(sm, base, n, out);
+    g = process_chunk<RB, MODE_FINAL>(sm, base, n, out);
   else
     g = process_chunk_wide<RB, MODE_FINAL>(sm, wide, base, carried ? side : nullptr, n, out);
   if (threadIdx.x == 0) b.ucount[bin] = g;
