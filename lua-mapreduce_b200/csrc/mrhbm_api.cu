@@ -1051,11 +1051,11 @@ int collect_sources(mrhbm_ctx* c, std::vector<Src>& srcs, uint64_t* N, mrhbm_sta
   bool checked = c->combine_checked;
   for (;;) {
     const uint32_t glog = kGtabLog + c->gtab_extra;
-    const uint64_t tab_bytes = gtab_bytes_host(c->rb, glog);
-    const uint64_t slots = (1ull << glog) + (c->rb == 16 ? 0 : 1ull << (glog - 4));  // records the compaction can emit
+    const GtabLayout tab{c->rb, glog};
+    const uint64_t tab_bytes = tab.bytes();
     int rc = ensure_records(c, &c->gtab, &c->gtab_cap, (tab_bytes + c->rb - 1) / c->rb);
     if (rc) return rc;
-    rc = ensure_records(c, &c->comb, &c->comb_cap, slots);
+    rc = ensure_records(c, &c->comb, &c->comb_cap, tab.records());
     if (rc) return rc;
     CU(c, cudaMemsetAsync(c->gtab, 0, tab_bytes, s));
     CU(c, cudaMemsetAsync(c->d_small, 0, 3 * sizeof(uint32_t), s));  // [0] flags, [1] records out, [2] largest value
@@ -1075,7 +1075,7 @@ int collect_sources(mrhbm_ctx* c, std::vector<Src>& srcs, uint64_t* N, mrhbm_sta
       c->no_combine = true;  // the partition / sort / reduce stages take the raw pairs
       return 0;
     }
-    if (!checked && c->rb != 16 && (uint64_t)c->h_small[2] * n >= 0xfffffff0ull) {
+    if (!checked && c->rb != 16 && (uint64_t)c->h_small[2] * n > kMaxCombinedSum) {
       // the fire-and-forget adds could have wrapped a u32 sum unnoticed: again, with checked adds (sticky)
       checked = c->combine_checked = true;
       continue;

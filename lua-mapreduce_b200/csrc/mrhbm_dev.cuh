@@ -149,10 +149,9 @@ __device__ __forceinline__ uint32_t fnv_lua_hash(const uint32_t* r) {
 }
 // 64-bit word hash over the little-endian u32 words of the key bytes while non-zero
 // (length-exact for NUL-free keys, independent of the slot width)
-template <int RB, bool EARLY = true>
+template <int RB>
 __device__ __forceinline__ uint64_t word_hash(const uint32_t* r) {
   uint64_t h = 0x9E3779B97F4A7C15ull;
-  bool live = true;
 #pragma unroll
   for (int i = 0; i < Rec<RB>::kKeyWords; i++) {
     uint32_t w;
@@ -160,12 +159,7 @@ __device__ __forceinline__ uint64_t word_hash(const uint32_t* r) {
       w = bswap32(i == 0 ? r[1] : r[0]);  // LE load of the 8 big-endian key bytes
     else
       w = r[i];
-    if (EARLY) {
-      if (w == 0) break;  // short keys leave early
-    } else {
-      live = live && (w != 0);
-      if (!live) continue;
-    }
+    if (w == 0) break;  // short keys leave early
     h = (h ^ w) * 0xBF58476D1CE4E5B9ull;
     h ^= h >> 29;
   }
@@ -240,39 +234,6 @@ __device__ __forceinline__ void key_mix2(const uint32_t* r, uint64_t& f1, uint64
   }
   f1 = a;
   f2 = mix64(b);
-}
-
-// ---- shared-memory hash tables of whole records (k_combine) --------------------------------
-// 128-bit volatile shared loads: one or two per probe instead of a word-by-word compare (a
-// record-strided word access hits only 4 bank groups)
-__device__ __forceinline__ uint4 lds128_volatile(const uint4* p) {
-  uint4 v;
-  uint32_t a = (uint32_t)__cvta_generic_to_shared(p);
-  asm volatile("ld.volatile.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(a));
-  return v;
-}
-// does table entry e hold the key of record w?  (the value/state word is ignored)
-template <int RB>
-__device__ __forceinline__ bool entry_key_eq_scalar(const uint32_t* e, const uint32_t* w) {
-  bool eq = true;
-#pragma unroll
-  for (int k = 0; k < Rec<RB>::kKeyWords; k++) eq &= (((volatile const uint32_t*)e)[k] == w[k]);
-  return eq;
-}
-template <int RB>
-__device__ __forceinline__ bool entry_key_eq(const uint32_t* e, const uint32_t* w) {
-  constexpr int KW = Rec<RB>::kKeyWords;
-  bool eq = true;
-#pragma unroll
-  for (int v = 0; v < Rec<RB>::kVec; v++) {
-    uint4 x = lds128_volatile((const uint4*)e + v);
-    uint32_t xs[4] = {x.x, x.y, x.z, x.w};
-#pragma unroll
-    for (int k = 0; k < 4; k++)
-      if (4 * v + k < KW) eq &= (xs[k] == w[4 * v + k]);
-    if (!eq) break;
-  }
-  return eq;
 }
 
 // ---- streaming global access ------------------------------------------------

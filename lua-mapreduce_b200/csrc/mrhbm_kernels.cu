@@ -697,17 +697,16 @@ __global__ void __launch_bounds__(1024) k_exscan_rows(const uint32_t* __restrict
 // A full table raises ERRF_SKEW and the host retries with a larger one (not L2 resident any more) or without
 // the combiner; a u32 sum about to wrap raises ERRF_OVERFLOW (string records carry u32 values), and the host then
 // hands the raw pairs on, whose sums the sort / reduce stages keep in u64.
-constexpr uint32_t kCombineLock = 0xffffffffu;
 constexpr int kCombineThreads = 1024;
 constexpr int kCombineSmem = 188 * 1024;  // (+ 38 KB of per-warp miss queues = 226 of the 227 KB)
 
-// cheap 32-bit hash of the key words (one IMAD per word); the shared table takes its top bits, the global
-// table a remix of it
-template <int RB>
+// cheap 32-bit hash of KW key words (one IMAD per word); the shared table (over the words of a key of up to 12
+// bytes) and the long entries of the global table (over all key words) take its top bits
+template <int KW>
 __device__ __forceinline__ uint32_t slot_hash(const uint32_t* w) {
   uint32_t h = 0x9E3779B9u;
 #pragma unroll
-  for (int k = 0; k < Rec<RB>::kKeyWords; k++) h = (h ^ w[k]) * 0x85EBCA6Bu + (h >> 15);
+  for (int k = 0; k < KW; k++) h = (h ^ w[k]) * 0x85EBCA6Bu + (h >> 15);
   h ^= h >> 16;
   h *= 0xC2B2AE35u;
   return h ^ (h >> 13);
@@ -747,11 +746,6 @@ __device__ __forceinline__ uint32_t ldv_u32(const uint32_t* p, uint64_t pol) {
   asm volatile("ld.relaxed.gpu.global.L2::cache_hint.u32 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(pol) : "memory");
   return v;
 }
-__device__ __forceinline__ unsigned long long ldv_u64(const unsigned long long* p, uint64_t pol) {
-  unsigned long long v;
-  asm volatile("ld.relaxed.gpu.global.L2::cache_hint.u64 %0, [%1], %2;" : "=l"(v) : "l"(p), "l"(pol) : "memory");
-  return v;
-}
 __device__ __forceinline__ uint4 ldv_v4(const uint4* p, uint64_t pol) {
   uint4 v;
   asm volatile("ld.relaxed.gpu.global.L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%4], %5;"
@@ -785,25 +779,67 @@ __device__ __forceinline__ void load_rec_hint(const uint4* p, uint32_t* w, uint6
 }
 
 // ---- the global table --------------------------------------------------------------------------------------
-// 2^glog SHORT entries of 16 bytes, open addressing with linear probing, ONE entry per probe:
-//   string keys of up to 12 bytes: {key word 0, 1, 2, u32 state}        u64 keys: {u64 key, u64 state}
-// state = 0 empty / all ones being written / sum + 1.  An entry is one aligned 16-byte vector: it is claimed with
-// a CAS on the state, written (key + lock) with one vector store, published with an exchange of the state after a
-// fence, and read with one vector load -- a reader that sees a published state sees its key.
-// String keys longer than 12 bytes (rare in word counts) go to 2^(glog-4) LONG entries of one record slot each
-// behind the short ones, walked entry by entry by the whole warp (state first, then the key).
+// Layout: GtabLayout (mrhbm_kernels.h).  SHORT entries: open addressing with linear probing, ONE entry per probe.
+// String keys longer than 12 bytes (rare in word counts) go to the LONG entries of one record slot each behind the
+// short ones, walked entry by entry by the whole warp (state first, then the key).
 // Why one 16-byte entry per probe: a random L2 read costs the SM per REQUEST, not per byte, and
 // a probe is never waited for: it is issued when 32 pairs have queued up and looked at when the next 32 have.
-// CHECKED: use the returned old value to catch a u32 sum about to wrap (otherwise the add is fire-and-forget and
-// the caller has bounded the sums: pairs x largest value < 2^32).
-__host__ __device__ inline uint64_t gtab_bytes(int rb, uint32_t glog) {
-  return ((uint64_t)16 << glog) + (rb == 16 ? 0ull : ((uint64_t)rb << (glog - 4)));
-}
 constexpr uint32_t kGtabMaxProbes = 192;  // linear probes before the table counts as full
 constexpr int kGtabMaxLongProbes = 128;
 
-// A pair on its way to the global table, 16 bytes: strings of up to 12 bytes {key word 0, 1, 2, u32 value},
-// u64 keys {key lo, key hi, value lo, value hi} -- also the layout of a short table entry (value -> state).
+// A pair on its way to the global table and a short entry share one 16-byte form: strings of up to 12 bytes
+// {key word 0, 1, 2, u32 value}, u64 keys {key lo, key hi, u64 value}.  In the table the value word is the entry's
+// state: 0 empty / kGtabLock being written / sum + 1.  A long entry is a record with the state in its value word.
+template <typename State>
+constexpr State kGtabLock = ~State(0);
+template <int RB>
+struct GtabEntry {
+  using State = std::conditional_t<Rec<RB>::kU64, unsigned long long, uint32_t>;
+  static __device__ __forceinline__ uint4 pack(uint32_t k0, uint32_t k1, uint32_t k2, State v) {
+    if constexpr (Rec<RB>::kU64)
+      return make_uint4(k0, k1, (uint32_t)v, (uint32_t)(v >> 32));
+    else
+      return make_uint4(k0, k1, k2, v);
+  }
+  static __device__ __forceinline__ State value(const uint4& x) {  // of a pair; of an entry: its state
+    if constexpr (Rec<RB>::kU64)
+      return (unsigned long long)x.z | ((unsigned long long)x.w << 32);
+    else
+      return x.w;
+  }
+  static __device__ __forceinline__ State* state(uint4* e) { return (State*)e + (Rec<RB>::kU64 ? 1 : 3); }
+  static __device__ __forceinline__ bool same_key(const uint4& a, const uint4& b) {
+    return a.x == b.x && a.y == b.y && (Rec<RB>::kU64 || a.z == b.z);
+  }
+};
+
+// The update protocol of an entry's state word.  An entry is claimed with a CAS of its state from 0 to the lock,
+// written (key + lock) with vector stores and published with an exchange of the state after a fence: a reader
+// that sees a published state sees its key.
+template <typename State>
+__device__ __forceinline__ bool gtab_claim(State* st) {
+  return atomicCAS(st, State(0), kGtabLock<State>) == State(0);
+}
+template <typename State>
+__device__ __forceinline__ void gtab_publish(State* st, State v) {
+  __threadfence();
+  atomicExch(st, v + State(1));
+}
+// CHECKED (u32 states only): use the returned old value to catch a sum about to pass kMaxCombinedSum (otherwise
+// the add is fire-and-forget and the caller has bounded the sums: pairs x largest value <= kMaxCombinedSum)
+template <bool CHECKED, typename State>
+__device__ __forceinline__ void gtab_add(State* st, State v, uint32_t* __restrict__ flags, uint64_t pol) {
+  if (!v) return;
+  if constexpr (CHECKED) {
+    const State old = atomicAdd(st, v);
+    if (old + v < old || old + v > kMaxCombinedSum) atomicOr(flags, (uint32_t)ERRF_OVERFLOW);
+  } else if constexpr (sizeof(State) == 8) {
+    red_add_u64(st, v, pol);
+  } else {
+    red_add_u32(st, v, pol);
+  }
+}
+
 template <int RB>
 __device__ __forceinline__ uint32_t gtab_slot(const uint4& E, uint32_t glog) {
   uint32_t g = (E.x ^ 0x9E3779B9u) * 0x85EBCA6Bu;
@@ -818,43 +854,20 @@ __device__ __forceinline__ uint32_t gtab_slot(const uint4& E, uint32_t glog) {
 // the empty entry), 1 = the entry holds another key (probe the next one), 2 = the entry is being written (look again).
 template <int RB, bool CHECKED>
 __device__ __forceinline__ int gtab_probe(uint4* e, const uint4& x, const uint4& E, uint32_t* __restrict__ flags, uint64_t pol) {
-  if constexpr (Rec<RB>::kU64) {
-    unsigned long long* st_p = (unsigned long long*)e + 1;
-    const unsigned long long st = (unsigned long long)x.z | ((unsigned long long)x.w << 32), lock = ~0ull;
-    const unsigned long long v = (unsigned long long)E.z | ((unsigned long long)E.w << 32);
-    if (st == 0) {
-      if (atomicCAS(st_p, 0ull, lock) != 0ull) return 2;
-      stv_v4(e, make_uint4(E.x, E.y, 0xffffffffu, 0xffffffffu), pol);
-      __threadfence();
-      atomicExch(st_p, v + 1ull);
-      return 0;
-    }
-    if (st == lock) return 2;
-    if (x.x != E.x || x.y != E.y) return 1;
-    if (v) red_add_u64(st_p, v, pol);
-    return 0;
-  } else {
-    uint32_t* st_p = (uint32_t*)e + 3;
-    const uint32_t v32 = E.w;
-    if (x.w == 0) {
-      if (atomicCAS(st_p, 0u, kCombineLock) != 0u) return 2;
-      stv_v4(e, make_uint4(E.x, E.y, E.z, kCombineLock), pol);
-      __threadfence();
-      atomicExch(st_p, v32 + 1u);
-      return 0;
-    }
-    if (x.w == kCombineLock) return 2;
-    if (x.x != E.x || x.y != E.y || x.z != E.z) return 1;
-    if (v32) {
-      if (CHECKED) {
-        const uint32_t old = atomicAdd(st_p, v32);
-        if (old + v32 < old || old + v32 >= 0xfffffff0u) atomicOr(flags, (uint32_t)ERRF_OVERFLOW);
-      } else {
-        red_add_u32(st_p, v32, pol);
-      }
-    }
+  using G = GtabEntry<RB>;
+  using State = typename G::State;
+  State* st_p = G::state(e);
+  const State st = G::value(x), v = G::value(E);
+  if (st == 0) {
+    if (!gtab_claim(st_p)) return 2;
+    stv_v4(e, G::pack(E.x, E.y, E.z, kGtabLock<State>), pol);
+    gtab_publish(st_p, v);
     return 0;
   }
+  if (st == kGtabLock<State>) return 2;
+  if (!G::same_key(x, E)) return 1;
+  gtab_add<CHECKED>(st_p, v, flags, pol);
+  return 0;
 }
 // WARP-COLLECTIVE: string keys longer than 12 bytes, one record slot per entry, state first, then the key
 template <int RB, bool CHECKED>
@@ -862,14 +875,11 @@ __device__ __forceinline__ void gtab_add_long(bool active, uint32_t* __restrict_
                                               uint32_t* __restrict__ flags, uint64_t pol) {
   using R = Rec<RB>;
   constexpr int W = R::kWords, KW = R::kKeyWords;
-  uint32_t* ltab = gtab + ((size_t)4 << glog);
-  const uint32_t lmask = (1u << (glog - 4)) - 1u;
-  uint32_t slot = slot_hash<RB>(w) >> (32 - (glog - 4));
+  constexpr uint32_t kLock = kGtabLock<uint32_t>;
+  const GtabLayout tab{RB, glog};
+  uint32_t* ltab = gtab + tab.long_offset() / sizeof(uint32_t);
+  uint32_t slot = slot_hash<KW>(w) >> (32 - tab.long_log());
   bool ldone = !active;
-  if (!ldone && v32 >= 0xfffffff0u) {
-    atomicOr(flags, (uint32_t)ERRF_OVERFLOW);
-    ldone = true;
-  }
 #pragma unroll 1
   for (int probe = 0; probe < kGtabMaxLongProbes; probe++) {
     if (__all_sync(0xffffffffu, ldone)) break;
@@ -877,18 +887,17 @@ __device__ __forceinline__ void gtab_add_long(bool active, uint32_t* __restrict_
       uint32_t* e = ltab + (size_t)slot * W;
       uint32_t st = ldv_u32(e + KW, pol);
       if (st == 0) {
-        if (atomicCAS(e + KW, 0u, kCombineLock) == 0u) {
+        if (gtab_claim(e + KW)) {
 #pragma unroll
           for (int i = 0; i < R::kVec; i++)  // the last vector rewrites the lock word with itself
-            stv_v4((uint4*)e + i, make_uint4(w[4 * i], w[4 * i + 1], w[4 * i + 2], 4 * i + 3 == KW ? kCombineLock : w[4 * i + 3]), pol);
-          __threadfence();
-          atomicExch(e + KW, v32 + 1u);
+            stv_v4((uint4*)e + i, make_uint4(w[4 * i], w[4 * i + 1], w[4 * i + 2], 4 * i + 3 == KW ? kLock : w[4 * i + 3]), pol);
+          gtab_publish(e + KW, v32);
           ldone = true;
         }
-        st = kCombineLock;
+        st = kLock;
       }
       if (!ldone) {
-        while (st == kCombineLock) st = ldv_u32(e + KW, pol);
+        while (st == kLock) st = ldv_u32(e + KW, pol);
         bool eq = true;
 #pragma unroll
         for (int i = 0; i < R::kVec; i++) {
@@ -896,18 +905,11 @@ __device__ __forceinline__ void gtab_add_long(bool active, uint32_t* __restrict_
           eq = eq && y.x == w[4 * i] && y.y == w[4 * i + 1] && y.z == w[4 * i + 2] && (4 * i + 3 == KW || y.w == w[4 * i + 3]);
         }
         if (eq) {
-          if (v32) {
-            if (CHECKED) {
-              const uint32_t old = atomicAdd(e + KW, v32);
-              if (old + v32 < old || old + v32 >= 0xfffffff0u) atomicOr(flags, (uint32_t)ERRF_OVERFLOW);
-            } else {
-              red_add_u32(e + KW, v32, pol);
-            }
-          }
+          gtab_add<CHECKED>(e + KW, v32, flags, pol);
           ldone = true;
         }
       }
-      slot = (slot + 1) & lmask;
+      slot = (slot + 1) & (tab.nlong() - 1u);
     }
   }
   if (!ldone) atomicOr(flags, (uint32_t)ERRF_SKEW);
@@ -922,6 +924,8 @@ __global__ void __launch_bounds__(kCombineThreads, 1)
               uint32_t glog, uint32_t* __restrict__ flags) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   using R = Rec<RB>;
+  using G = GtabEntry<RB>;
+  static_assert(!(CHECKED && R::kU64), "u64 keys keep u64 sums: their adds are never checked");
   constexpr int W = R::kWords, KW = R::kKeyWords;
   constexpr int KC = KW < 3 ? KW : 3;  // key words of a shared-table entry: only keys of up to 12 bytes live there
   // Shared table, ARRAY PER FIELD (32 lanes probing 32 random entries hit 32 random banks, not the four a record
@@ -958,7 +962,7 @@ __global__ void __launch_bounds__(kCombineThreads, 1)
   uint32_t vmax = 0;
   for (uint32_t i = tid; i < entries * (KC + 2); i += blockDim.x) tag[i] = 0;
   __syncthreads();
-  const uint32_t gmask = (1u << glog) - 1u;
+  const uint32_t gmask = GtabLayout{RB, glog}.nshort() - 1u;
   auto append = [&](bool p, const uint4& E, uint32_t probe) {  // collective: the entries of the lanes with p go to the tail
     const uint32_t m = __ballot_sync(0xffffffffu, p);
     if (p) {
@@ -1028,8 +1032,7 @@ __global__ void __launch_bounds__(kCombineThreads, 1)
       const bool out = e < entries && tag[e] > 1u && val[e] < below;
       uint4 E = make_uint4(0, 0, 0, 0);
       if (out) {
-        const uint32_t k0 = key[e], k1 = key[entries + e], k2 = KC > 2 ? key[2u * entries + e] : 0u;
-        E = R::kU64 ? make_uint4(k0, k1, val[e], 0u) : make_uint4(k0, k1, k2, val[e]);
+        E = G::pack(key[e], key[entries + e], KC > 2 ? key[2u * entries + e] : 0u, val[e]);
         tag[e] = 0;
       }
       if (__any_sync(0xffffffffu, out)) push(out, E);
@@ -1082,13 +1085,7 @@ __global__ void __launch_bounds__(kCombineThreads, 1)
       for (int k = 3; k < KW; k++) is_short = is_short && w[k] == 0;
     }
     if (need && is_short && v != 0 && v <= vcap) {  // (a zero would still have to create its key: left to the global table)
-      uint32_t h = 0x9E3779B9u;  // slot_hash over the KC words a short key has
-#pragma unroll
-      for (int k = 0; k < KC; k++) h = (h ^ w[k]) * 0x85EBCA6Bu + (h >> 15);
-      h ^= h >> 16;
-      h *= 0xC2B2AE35u;
-      h ^= h >> 13;
-      const uint32_t tg = h | 2u;
+      const uint32_t h = slot_hash<KC>(w), tg = h | 2u;
       const uint32_t s0 = __umulhi(h, entries), s1 = s0 + 1 == entries ? 0u : s0 + 1;
       const uint32_t t0 = ((volatile uint32_t*)tag)[s0], t1 = ((volatile uint32_t*)tag)[s1];
       if (t0 == tg || t1 == tg) {
@@ -1118,7 +1115,7 @@ __global__ void __launch_bounds__(kCombineThreads, 1)
     // misses: long string keys (rare) are remembered by index and walk their table 32 at a time, all lanes busy;
     // everything else queues up as a compact entry
     if (!R::kU64) {
-      if (need && v >= 0xfffffff0ull) {  // (its state word, value + 1, would read "being written")
+      if (need && v > kMaxCombinedSum) {  // (this test also keeps such values out of the long table)
         atomicOr(flags, (uint32_t)ERRF_OVERFLOW);
         need = false;
       }
@@ -1131,7 +1128,7 @@ __global__ void __launch_bounds__(kCombineThreads, 1)
       }
     }
     const bool p = need && is_short;
-    if (__any_sync(0xffffffffu, p)) push(p, R::kU64 ? make_uint4(w[0], w[1], w[2], w[3]) : make_uint4(w[0], w[1], w[2], (uint32_t)v));
+    if (__any_sync(0xffffffffu, p)) push(p, G::pack(w[0], w[1], w[2], v));
   }
   __syncthreads();
   evict(0xffffffffu);  // the shared table's entries take the same road as the misses
@@ -1152,31 +1149,21 @@ __global__ void __launch_bounds__(256) k_gtab_compact(const uint32_t* __restrict
                                                       uint32_t* __restrict__ count) {
   using R = Rec<RB>;
   constexpr int W = R::kWords, KW = R::kKeyWords;
-  const uint32_t nshort = 1u << glog, nlong = R::kU64 ? 0u : 1u << (glog - 4), lane = threadIdx.x & 31;
-  const uint32_t* ltab = gtab + ((size_t)4 << glog);
-  for (uint32_t base = (blockIdx.x * blockDim.x + threadIdx.x) & ~31u; base < nshort + nlong; base += gridDim.x * blockDim.x) {
+  const GtabLayout tab{RB, glog};
+  const uint32_t nshort = tab.nshort(), lane = threadIdx.x & 31;
+  const uint32_t* ltab = gtab + tab.long_offset() / sizeof(uint32_t);
+  for (uint32_t base = (blockIdx.x * blockDim.x + threadIdx.x) & ~31u; base < tab.records(); base += gridDim.x * blockDim.x) {
     const uint32_t s = base + lane;  // (nshort and nlong are multiples of 32: a warp never straddles the two tables)
     uint32_t w[W];
 #pragma unroll
     for (int k = 0; k < W; k++) w[k] = 0;
-    bool has;
+    uint64_t st;  // the entry's state: sum + 1, 0 = empty
     if (s < nshort) {
       const uint4 x = ((const uint4*)gtab)[s];
-      if constexpr (R::kU64) {
-        unsigned long long st = (unsigned long long)x.z | ((unsigned long long)x.w << 32);
-        has = st != 0;
-        st -= 1ull;
-        w[0] = x.x;
-        w[1] = x.y;
-        w[2] = (uint32_t)st;
-        w[3] = (uint32_t)(st >> 32);
-      } else {
-        has = x.w != 0;
-        w[0] = x.x;
-        w[1] = x.y;
-        w[2] = x.z;
-        w[KW] = x.w - 1u;
-      }
+      w[0] = x.x;
+      w[1] = x.y;
+      if (!R::kU64) w[2] = x.z;
+      st = GtabEntry<RB>::value(x);
     } else {
       const uint4* e = (const uint4*)(ltab + (size_t)(s - nshort) * W);
 #pragma unroll
@@ -1187,8 +1174,15 @@ __global__ void __launch_bounds__(256) k_gtab_compact(const uint32_t* __restrict
         w[4 * i + 2] = x.z;
         w[4 * i + 3] = x.w;
       }
-      has = w[KW] != 0;
-      w[KW] -= 1u;
+      st = rec_value<RB>(w);
+    }
+    const bool has = st != 0;
+    st -= 1ull;
+    if constexpr (R::kU64) {
+      w[2] = (uint32_t)st;
+      w[3] = (uint32_t)(st >> 32);
+    } else {
+      w[KW] = (uint32_t)st;
     }
     const uint32_t m = __ballot_sync(0xffffffffu, has);
     if (!m) continue;
@@ -1378,12 +1372,10 @@ cudaError_t kernels_configure() {
   if (e != cudaSuccess) return e;
   CFGS(false, false) CFGS(false, true) CFGS(true, false) CFGS(true, true)
 #undef CFGS
-#define CFGC1(RB, CH)                                                                                      \
+#define CFGC(RB, CH)                                                                                       \
   e = cudaFuncSetAttribute(k_combine<RB, CH>, cudaFuncAttributeMaxDynamicSharedMemorySize, kCombineSmem);  \
   if (e != cudaSuccess) return e;
-#define CFGC(RB) CFGC1(RB, false) CFGC1(RB, true)
-  CFGC(16) CFGC(32) CFGC(64) CFGC(128)
-#undef CFGC1
+  CFGC(16, false) CFGC(32, false) CFGC(32, true) CFGC(64, false) CFGC(64, true) CFGC(128, false) CFGC(128, true)
 #undef CFGC
 #define CFGT1(RB, SPEC)                                                                                  \
   e = cudaFuncSetAttribute(k_split_tma<RB, kTmaTileBytes, 2, kTmaSplitThreads, SPEC>,                    \
@@ -1450,22 +1442,21 @@ int launch_tok_emit(int rb, const unsigned char* text, uint64_t len, const uint3
   }
   return 1;
 }
-uint64_t gtab_bytes_host(int rb, uint32_t glog) { return gtab_bytes(rb, glog); }
 int launch_combine(int rb, const void* recs, uint64_t n, uint32_t* gtab, uint32_t glog, uint32_t* flags, bool checked,
                    int sm_count, cudaStream_t s) {
   if (!n) return 0;
-  // the shared table only takes values whose per-CTA sum cannot wrap 32 bits
+  // the shared table only takes values whose per-CTA sum stays within kMaxCombinedSum
   const uint64_t per_cta = (n + sm_count - 1) / sm_count + kCombineThreads;
-  const uint32_t vcap = (uint32_t)std::min<uint64_t>(0xffffull, 0xffffffefull / per_cta);
-  if (checked) {
-    DISPATCH_RB(rb, (k_combine<RB, true><<<sm_count, kCombineThreads, kCombineSmem, s>>>((const uint4*)recs, n, (uint32_t)kPrefetchTrips, vcap, gtab, glog, flags)));
+  const uint32_t vcap = (uint32_t)std::min<uint64_t>(0xffffull, kMaxCombinedSum / per_cta);
+  if (checked) {  // (u64 keys keep u64 sums: never checked)
+    DISPATCH_RB(rb, (k_combine<RB, !Rec<RB>::kU64><<<sm_count, kCombineThreads, kCombineSmem, s>>>((const uint4*)recs, n, (uint32_t)kPrefetchTrips, vcap, gtab, glog, flags)));
   } else {
     DISPATCH_RB(rb, (k_combine<RB, false><<<sm_count, kCombineThreads, kCombineSmem, s>>>((const uint4*)recs, n, (uint32_t)kPrefetchTrips, vcap, gtab, glog, flags)));
   }
   return 1;
 }
 int launch_gtab_compact(int rb, const uint32_t* gtab, uint32_t glog, void* out, uint32_t* count, cudaStream_t s) {
-  const uint32_t slots = (1u << glog) + (rb == 16 ? 0u : 1u << (glog - 4));
+  const uint32_t slots = GtabLayout{rb, glog}.records();
   int grid = (int)std::min<uint32_t>((slots + 255) / 256, (uint32_t)g_sm_count * 8);
   DISPATCH_RB(rb, (k_gtab_compact<RB><<<grid, 256, 0, s>>>(gtab, glog, (uint4*)out, count)));
   return 1;

@@ -104,15 +104,29 @@ int launch_tok_count(const unsigned char* text, uint64_t len, uint32_t* block_co
 int launch_tok_emit(int rb, const unsigned char* text, uint64_t len, const uint32_t* block_off, void* recs,
                     uint32_t* flags, cudaStream_t s);
 inline uint64_t tok_blocks(uint64_t len) { return (len + 255) / 256; }
-// map-side combine of one committed range into the global table gtab (2^glog 16-byte short entries + 2^(glog-4)
-// record-sized long ones = gtab_bytes_host(rb, glog) bytes, zeroed by the caller); flags[0] |= ERRF_SKEW when the table is full, ERRF_OVERFLOW when a u32 sum would wrap (checked
-// mode only: unchecked adds are fire-and-forget and the caller verifies afterwards that pairs x flags[2], the
-// largest value seen, stays below 2^32)
+// The map-side combiner's global table for records of rb bytes: 2^glog short entries of 16 bytes, then, for string
+// records only, 2^(glog-4) long entries of one record each.  The compaction emits at most one record per entry.
+struct GtabLayout {
+  int rb;
+  uint32_t glog;
+  MRHBM_HD uint32_t nshort() const { return 1u << glog; }
+  MRHBM_HD uint32_t long_log() const { return glog - 4; }
+  MRHBM_HD uint32_t nlong() const { return rb == 16 ? 0u : 1u << long_log(); }
+  MRHBM_HD uint64_t long_offset() const { return (uint64_t)16 << glog; }  // bytes
+  MRHBM_HD uint64_t bytes() const { return long_offset() + (uint64_t)rb * nlong(); }
+  MRHBM_HD uint32_t records() const { return nshort() + nlong(); }
+};
+// Largest sum (and so largest value) a combined string record carries in its u32 value: the table keeps sum + 1,
+// and all ones marks an entry being written.
+constexpr uint32_t kMaxCombinedSum = 0xffffffefu;
+// map-side combine of one committed range into the global table gtab (GtabLayout{rb, glog}.bytes(), zeroed by the
+// caller); flags[0] |= ERRF_SKEW when the table is full, ERRF_OVERFLOW when a u32 sum would pass kMaxCombinedSum
+// (checked mode only: unchecked adds are fire-and-forget and the caller verifies afterwards that pairs x flags[2],
+// the largest value seen, stays within it)
 int launch_combine(int rb, const void* recs, uint64_t n, uint32_t* gtab, uint32_t glog, uint32_t* flags, bool checked,
                    int sm_count, cudaStream_t s);
 // one record per non-empty table entry appended to out; *count (zeroed by the caller) += entries
 int launch_gtab_compact(int rb, const uint32_t* gtab, uint32_t glog, void* out, uint32_t* count, cudaStream_t s);
-uint64_t gtab_bytes_host(int rb, uint32_t glog);
 // tot[b] = sum over s < world of all[s * stride + base + b], b < n; *nover += bins (of all `stride`
 // bins) whose global total exceeds cap
 int launch_sum_src(const uint32_t* all, uint32_t world, uint32_t stride, uint32_t base, uint32_t n,
