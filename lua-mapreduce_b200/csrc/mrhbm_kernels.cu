@@ -737,9 +737,12 @@ __device__ __forceinline__ uint4 ldg_stream_hint(const uint4* p, uint64_t pol) {
 __device__ __forceinline__ void bulk_prefetch_l2(const void* p, uint32_t bytes, uint64_t pol) {
   asm volatile("cp.async.bulk.prefetch.L2.global.L2::cache_hint [%0], %1, %2;" ::"l"(p), "r"(bytes), "l"(pol) : "memory");
 }
-constexpr int kPrefetchTrips = 2;  // x 32 KB per CTA x 132 CTAs = 8.4 MB of the stream in L2 ahead of its use, beside the 32 MB
-                                    // global table in the 50 MB L2.  Config 3 on one H100 SXM at 700 W, ms per 10^9 pairs for
-                                    // 1 / 2 / 3 / 4 trips: 17.3 / 17.1 / 17.7 / 19.0 (more trips push the table out of L2)
+// Distance in trips of the L2 bulk prefetch ahead of the trip in hand (0: none).  Prefetched pairs compete with the
+// 32 MB global table for the 50 MB L2.  Config 3 (32-byte records) on one H100 SXM at 700 W, ms of k_combine per 10^9
+// pairs, alternating runs in one call: no prefetch 15.47 against 16.61 with 2 trips (earlier sweep, 1 / 2 / 3 / 4
+// trips: 17.3 / 17.1 / 17.7 / 19.0).  Records of 64 and 128 bytes keep the 2 trips; they were not swept.
+template <int RB>
+constexpr uint32_t kPrefetchTrips = RB <= 32 ? 0u : 2u;
 constexpr uint32_t kEpochTrips = 256;  // shared-table clean-up period: 256 trips = 262,144 pairs per CTA
 __device__ __forceinline__ uint32_t ldv_u32(const uint32_t* p, uint64_t pol) {
   uint32_t v;
@@ -935,7 +938,7 @@ __global__ void __launch_bounds__(kCombineThreads, 1)
   // Every kEpochTrips trips the CTA stops at a barrier and evicts the entries that gathered less than two pairs
   // since they were admitted (into the global table, like a miss): the table is filled first come first served,
   // and without that the keys that happened to arrive first would keep out warmer keys that arrived later.
-  // (compile-time sizes: table addresses become immediates -- the kernel is issue bound and short of registers)
+  // (compile-time sizes: table addresses become immediates -- the kernel is short of registers)
   constexpr uint32_t entries = (uint32_t)(kCombineSmem / (R::kU64 ? 16 : 20));  // tag + value + 2 (u64) or 3 key words
   uint32_t* tag = (uint32_t*)smem_raw;
   uint32_t* val = tag + entries;
@@ -1044,14 +1047,14 @@ __global__ void __launch_bounds__(kCombineThreads, 1)
   const uint64_t slice_hi = slice_lo + slice < n ? slice_lo + slice : n;  // (this CTA's pairs: [slice_lo, slice_hi))
   const uint32_t ntrips = (uint32_t)((slice_hi - slice_lo + blockDim.x - 1) / blockDim.x);  // (the same for every thread: barriers inside)
   // the pair of the NEXT trip is requested before this one is processed.  Index arithmetic of the loop: running
-  // 64-bit pointers and 32-bit trip bounds (the kernel is issue bound; the per-trip 64-bit index, bounds checks and
+  // 64-bit pointers and 32-bit trip bounds (the per-trip 64-bit index, bounds checks and
   // prefetch address were a visible share of its instructions)
   const uint32_t npairs = (uint32_t)(slice_hi - slice_lo);                                  // pairs of this CTA (< 2^32)
   const uint32_t my_trips = tid < npairs ? (npairs - tid + blockDim.x - 1) / blockDim.x : 0u;  // trips in which this thread has a pair
   // the warp's 32 pairs of trip t + pf_trips lie inside the slice for t < pf_ok
   const uint32_t wbase = (tid & ~31u) + 32u;
   const uint32_t pf_full = npairs >= wbase ? (npairs - wbase) / blockDim.x + 1u : 0u;      // trips whose 32 pairs are all there
-  const uint32_t pf_ok = pf_full > pf_trips ? pf_full - pf_trips : 0u;
+  const uint32_t pf_ok = pf_trips && pf_full > pf_trips ? pf_full - pf_trips : 0u;
   const uint4* p_next = recs + (slice_lo + tid) * R::kVec;                                  // this thread's pair of the next trip
   const uint4* p_pf = recs + (slice_lo + (tid & ~31u) + (uint64_t)pf_trips * blockDim.x) * R::kVec;  // the warp's prefetch target
   const size_t p_step = (size_t)blockDim.x * R::kVec;
@@ -1069,7 +1072,7 @@ __global__ void __launch_bounds__(kCombineThreads, 1)
     for (int k = 0; k < W; k++) w[k] = wn[k];
     p_next += p_step;
     if (trip + 1 < my_trips) load_rec_hint<RB>(p_next, wn, pol.stream);
-    // ... and the warp's 32 pairs of kPrefetchTrips trips ahead are pulled from DRAM into L2 by the bulk-copy engine:
+    // ... and (pf_trips > 0) the warp's 32 pairs of pf_trips trips ahead are pulled from DRAM into L2 by the bulk-copy engine:
     // one trip of work does not cover a DRAM access under load, an L2 hit it does.  (One 32 KB request per CTA by a
     // single thread instead of 1 KB per warp saves instructions but is slower: the warps of a CTA are not in step.)
     if (lane == 0 && trip < pf_ok) bulk_prefetch_l2(p_pf, 32u * RB, pol.stream);
@@ -1449,9 +1452,9 @@ int launch_combine(int rb, const void* recs, uint64_t n, uint32_t* gtab, uint32_
   const uint64_t per_cta = (n + sm_count - 1) / sm_count + kCombineThreads;
   const uint32_t vcap = (uint32_t)std::min<uint64_t>(0xffffull, kMaxCombinedSum / per_cta);
   if (checked) {  // (u64 keys keep u64 sums: never checked)
-    DISPATCH_RB(rb, (k_combine<RB, !Rec<RB>::kU64><<<sm_count, kCombineThreads, kCombineSmem, s>>>((const uint4*)recs, n, (uint32_t)kPrefetchTrips, vcap, gtab, glog, flags)));
+    DISPATCH_RB(rb, (k_combine<RB, !Rec<RB>::kU64><<<sm_count, kCombineThreads, kCombineSmem, s>>>((const uint4*)recs, n, kPrefetchTrips<RB>, vcap, gtab, glog, flags)));
   } else {
-    DISPATCH_RB(rb, (k_combine<RB, false><<<sm_count, kCombineThreads, kCombineSmem, s>>>((const uint4*)recs, n, (uint32_t)kPrefetchTrips, vcap, gtab, glog, flags)));
+    DISPATCH_RB(rb, (k_combine<RB, false><<<sm_count, kCombineThreads, kCombineSmem, s>>>((const uint4*)recs, n, kPrefetchTrips<RB>, vcap, gtab, glog, flags)));
   }
   return 1;
 }
