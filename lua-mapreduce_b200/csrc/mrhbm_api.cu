@@ -43,7 +43,6 @@ struct Range {
 constexpr size_t kStageRecs = 1 << 16;
 enum { EV_START, EV_CSTART, EV_COMBINE, EV_HIST, EV_PLAN, EV_GATH, EV_SCATTER, EV_EXCH, EV_SORT, EV_BIG, EV_END, EV_PROBE, EV_N };
 constexpr uint32_t kSampleKeys = 1u << 18;      // keys sampled to decide between key-ordered and hash sub-bins
-constexpr uint64_t kSplitMaxBinsHost = 1024;    // bins one level of k_split_tma distinguishes
 }  // namespace
 
 struct mrhbm_ctx {
@@ -1112,32 +1111,73 @@ int agree_flags(mrhbm_ctx* c, uint32_t* ef) {
   return 0;
 }
 
+// The geometry of the split (k_split_tma) into the fine bins of ndest destination ranks, Bl[d] of them on rank d, as
+// seen by rank me: B, F, C1, C1_local, cap, rbase, fbase, ndest, me, sub_stride.  Returns the number of levels, or 0
+// when the split does not take these bins.
+//   optimistic layout: one level on one GPU with at most kSplitMaxBins bins (level 1 writes the fine bins, regions
+//     of `cap` slots); else F = the smallest power of two >= sqrt(B) (both levels see about the same fan-out), doubled
+//     until the regions of all ranks fit one level, and a region gets mean + 8 sigma + 64 slots for one rank's share
+//     (at most nmax records, hash balanced over the B bins).
+//   exact layout (one destination, also on several GPUs: the destination-major send buffer): two levels from 2048
+//     bins on; the regions are sized by their bins' capacity, F * cap.
+// (With one destination ceil(B / F) <= F, so the doubling never runs and F > kSplitMaxBins alone ends the search.)
+int plan_split(SplitPlan& pl, const uint64_t* Bl, uint32_t ndest, uint32_t me, uint32_t cap, uint64_t nmax, bool exact) {
+  uint64_t B = 0;
+  for (uint32_t d = 0; d < ndest; d++) B += Bl[d];
+  const int levels = !exact && ndest == 1 && B <= kSplitMaxBins ? 1 : 2;
+  if (exact && B < 2048) return 0;
+  uint32_t F = 1;
+  if (levels == 2) {
+    while ((uint64_t)F * F < B) F <<= 1;
+    for (; F <= kSplitMaxBins; F <<= 1) {
+      uint64_t c1 = 0;
+      for (uint32_t d = 0; d < ndest; d++) c1 += (Bl[d] + F - 1) / F;
+      if (c1 <= kSplitMaxBins) break;
+    }
+    if (F > kSplitMaxBins) return 0;  // more bins than two levels reach
+  }
+  pl.rbase[0] = pl.fbase[0] = 0;
+  for (uint32_t d = 0; d < 8; d++) {
+    const uint64_t bl = d < ndest ? Bl[d] : 0;
+    pl.rbase[d + 1] = pl.rbase[d] + (uint32_t)((bl + F - 1) / F);
+    pl.fbase[d + 1] = pl.fbase[d] + (uint32_t)bl;
+  }
+  pl.B = (uint32_t)B;
+  pl.F = F;
+  pl.C1 = pl.rbase[ndest];
+  pl.C1_local = pl.rbase[me + 1] - pl.rbase[me];
+  pl.cap = cap;
+  pl.ndest = ndest;
+  pl.me = me;
+  double ss = (double)F * cap;
+  if (!exact && levels == 2) {  // one rank's contribution to one region: F of the B bins, hash balanced
+    const double mean = (double)nmax * (double)F / (double)B;
+    ss = mean + 8.0 * std::sqrt(mean) + 64.0;
+  }
+  if (ss >= 4.0e9) return 0;
+  pl.sub_stride = ((uint64_t)ss + 7u) & ~7ull;
+  return levels;
+}
+
 // Exact layout (bin offsets in sb.bin_off after k_hist + k_exscan): the records of `live` go to their B bins in sb.mid
 // (on several GPUs: the destination-major send buffer), through the two-level coalesced split when there are enough
 // bins (claims relative to bin_off), else the direct scatter.
 int exact_split(mrhbm_ctx* c, const std::vector<Src>& live, const BinParams& bp, uint64_t B, uint64_t N, mrhbm_stats& st) {
   cudaStream_t s = c->stream;
-  uint32_t F = 1;
-  while ((uint64_t)F * F < B) F <<= 1;
-  const uint32_t C1 = (uint32_t)((B + F - 1) / F);
-  if (B >= 2048 && F <= 1024 && C1 <= 1024) {
+  SplitPlan pl{};
+  if (plan_split(pl, &B, 1, 0, c->cap, 0, true)) {
     int rc = ensure_records(c, &c->l1buf, &c->l1_cap, N);
     if (rc) return rc;
     // relative fill levels: coarse levels live in hist (dead after the scan), fine levels in cursor
-    CU(c, cudaMemsetAsync(c->sb.hist, 0, ((uint64_t)C1 << c->ctr_shift) * sizeof(uint32_t), s));
+    CU(c, cudaMemsetAsync(c->sb.hist, 0, ((uint64_t)pl.C1 << c->ctr_shift) * sizeof(uint32_t), s));
     CU(c, cudaMemsetAsync(c->sb.cursor, 0, (B << c->ctr_shift) * sizeof(uint32_t), s));
-    SplitPlan pl{};
-    pl.B = (uint32_t)B;
-    pl.F = F;
-    pl.C1 = pl.C1_local = C1;
-    pl.cap = c->cap;
     pl.cursor1 = c->sb.hist;
     pl.cursor = c->sb.cursor;
+    pl.ctr_shift = bp.ctr_shift;
     pl.l1 = c->l1buf;
     pl.mid = c->sb.mid;
     pl.err_flags = c->sb.counters + CNT_ERR;
     pl.base_off = c->sb.bin_off;
-    pl.ndest = 1;
     for (auto& r : live) st.launches += launch_split_l1(c->rb, r.p, r.n, bp, pl, s);
     st.launches += launch_split_l2(c->rb, bp, pl, s);
   } else {
@@ -1259,38 +1299,9 @@ int shuffle_fast(mrhbm_ctx* c, std::vector<Src>& live, uint64_t N, uint64_t N_in
   const uint32_t bin_stride = c->cap;  // slots per fine bin: what one CTA sorts in shared memory
   // ---- levels.  One GPU, few bins: level 1 goes straight into the fine bins.
   SplitPlan pl{};
-  const bool single_level = G == 1 && B <= kSplitMaxBinsHost;
-  uint32_t F = 1;
-  if (!single_level) {
-    while ((uint64_t)F * F < B) F <<= 1;  // power of two >= sqrt(B): both levels see about the same fan-out
-    for (;; F <<= 1) {
-      uint64_t c1 = 0;
-      for (int r = 0; r < G; r++) c1 += (Bl_of[r] + F - 1) / F;
-      if (c1 <= kSplitMaxBinsHost) break;
-    }
-    if (F > kSplitMaxBinsHost) return 0;  // more bins than two levels reach: exact path
-  }
-  pl.rbase[0] = 0;
-  for (int r = 0; r < 8; r++) {
-    const uint64_t bl = r < G ? Bl_of[r] : 0;
-    pl.rbase[r + 1] = pl.rbase[r] + (uint32_t)((bl + F - 1) / F);
-    pl.fbase[r] = c->pbase[r] * S;
-  }
-  pl.fbase[8] = c->pbase[8] * S;
-  pl.B = (uint32_t)B;
-  pl.F = F;
-  pl.C1 = pl.rbase[G];
-  pl.C1_local = pl.rbase[me + 1] - pl.rbase[me];
-  pl.cap = bin_stride;
-  pl.ndest = (uint32_t)G;
-  pl.me = (uint32_t)me;
-  {
-    // one rank's contribution to one region: F of the B bins, hash balanced
-    const double mean = (double)Nmax * (double)F / (double)B;
-    const double ss = single_level ? (double)bin_stride : mean + 8.0 * std::sqrt(mean) + 64.0;
-    if (ss >= 4.0e9) return 0;
-    pl.sub_stride = ((uint64_t)ss + 7u) & ~7ull;
-  }
+  const int levels = plan_split(pl, Bl_of, (uint32_t)G, (uint32_t)me, bin_stride, Nmax, false);
+  if (!levels) return 0;  // more bins than two levels reach: exact path
+  const bool single_level = levels == 1;
   // ---- buffers
   rc = ensure_small_arrays(c, std::max<uint64_t>(Bl, pl.C1));
   if (rc) return rc;
@@ -1318,6 +1329,7 @@ int shuffle_fast(mrhbm_ctx* c, std::vector<Src>& live, uint64_t N, uint64_t N_in
   }
   pl.cursor1 = c->sb.hist;
   pl.cursor = c->sb.cursor;
+  pl.ctr_shift = c->ctr_shift;
   pl.l1 = single_level ? c->sb.mid : c->regions;
   pl.mid = c->sb.mid;
   pl.err_flags = c->sb.counters + CNT_ERR;

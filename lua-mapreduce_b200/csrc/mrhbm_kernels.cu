@@ -252,43 +252,10 @@ __global__ void __launch_bounds__(256) k_sample_u64(const uint4* __restrict__ re
 // overlap inside one kernel, and the sort then runs on local data only.  Replaces
 // mapreduce/job.lua:203-221 (partitionfn + spill) and the GridFS / scp transport (job.lua:255-260,
 // fs.lua:143-160).
-constexpr int kSplitMaxBins = 1024;
-
-struct SplitArgs {
-  const uint4* src;       // level 1: records
-  uint64_t n;             // level 1: number of records
-  // level 2 source: region y = blockIdx.y of this rank as filled by source rank z = blockIdx.z:
-  // seg_stride records at peer[z] + (region_first + y) * seg_stride, holding
-  // seg_counts[z * seg_zstride + ((region_first + y) << ctr_shift)] records
-  unsigned long long peer[8];  // every rank's region buffer as mapped into this process (one GPU: peer[0] = l1)
-  const uint32_t* seg_counts;
-  uint64_t seg_zstride;
-  uint64_t seg_stride;
-  uint32_t region_first;
-  uint4* dst;             // destination regions
-  uint64_t dst_stride;    // records per destination region (optimistic layout)
-  uint32_t* cursor;       // destination fill levels (index << ctr_shift)
-  uint32_t capacity;      // records a destination region can take
-  uint32_t F;             // fine bins per coarse region (a power of two)
-  uint32_t logF;
-  uint32_t nbins;         // bins this level distinguishes inside one tile (<= kSplitMaxBins)
-  uint32_t level;         // 1 or 2
-  uint32_t ctr_shift;
-  uint32_t* err_flags;
-  // exact layout (after k_hist + k_exscan): bin f starts at base_off[f]; nullptr = the optimistic fixed-stride layout
-  const uint32_t* base_off;
-  uint32_t B;
-  // optimistic layout: rank d owns the coarse regions [rbase[d], rbase[d+1]) = its fine bins
-  // [fbase[d], fbase[d+1]) in blocks of F (one GPU: rbase = {0, C1}, fbase = {0, B})
-  uint32_t rbase[9], fbase[9];
-  uint32_t ndest, me;
-  uint32_t* ticket;          // level 1, optimistic layout: {next tile - gridDim.x, CTAs that have left}, both 0 at launch
-};
 
 constexpr int kTmaSplitThreads = 512;
-constexpr int kTmaTileBytes = kSplitTileBytes;
-__host__ __device__ constexpr size_t tma_split_smem(int rb, int tile_bytes = kTmaTileBytes) {
-  return 2 * (size_t)tile_bytes + (size_t)(tile_bytes / rb) * sizeof(uint32_t);
+__host__ __device__ constexpr size_t tma_split_smem(int rb) {
+  return 2 * (size_t)kSplitTileBytes + (size_t)(kSplitTileBytes / rb) * sizeof(uint32_t);
 }
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -324,22 +291,25 @@ __device__ __forceinline__ void bulk_load(void* dst_smem, const void* src_gmem, 
 // tile through it.
 // The kernel is issue bound (its time follows the instruction count), so
 // what is known at launch time is folded at compile time.  SPEC = 0: level, number of GPUs and layout are read from
-// the arguments (exact layouts, the rare paths).  Otherwise the optimistic layout with bits 0-1 = level and
+// the plan (exact layouts, the rare paths).  Otherwise the optimistic layout with bits 0-1 = level and
 // bit 2 = several GPUs.
-template <int RB, int TILE_BYTES = kTmaTileBytes, int MINB = 2, int THREADS_ = kTmaSplitThreads, int SPEC = 0>
-__global__ void __launch_bounds__(THREADS_, MINB) k_split_tma(SplitArgs a, BinParams bp) {
+// Arguments: the plan as the host made it, the level (1 or 2; folded when SPEC != 0) and, at level 1, the records
+// it splits (src, n).  Level 2 reads the regions of the plan's region buffers (l1, peer[]).
+template <int RB, int SPEC = 0>
+__global__ void __launch_bounds__(kTmaSplitThreads, 2)
+    k_split_tma(SplitPlan pl, uint32_t level_arg, const uint4* src, uint64_t n, BinParams bp) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   using R = Rec<RB>;
-  constexpr int THREADS = THREADS_;
-  constexpr int T = TILE_BYTES / RB;              // records per tile
+  constexpr int THREADS = kTmaSplitThreads;
+  constexpr int T = kSplitTileBytes / RB;            // records per tile
   constexpr int U = (T + THREADS - 1) / THREADS;     // records per thread
   constexpr int IPT = kSplitMaxBins / THREADS;       // bins per thread in the scan
   constexpr int WORLD = SPEC ? ((SPEC & 4) ? 2 : 1) : 0;
   constexpr bool DYN = SPEC != 0 && (SPEC & 3) == 1;  // tiles from a ticket counter (level 1, optimistic layout)
   static_assert(T < 65536 && kSplitMaxBins <= 65536, "perm packs (raw index, bin) into 16 + 16 bits");
-  uint32_t* perm = (uint32_t*)(smem_raw + 2 * TILE_BYTES);  // output position -> raw index | bin << 16
+  uint32_t* perm = (uint32_t*)(smem_raw + 2 * kSplitTileBytes);  // output position -> raw index | bin << 16
   __shared__ uint32_t scnt[kSplitMaxBins], soff[kSplitMaxBins];
-  // this tile: the slot (record index in a.dst, 32-bit wrap-around arithmetic) output position 0 would have in the bin's run
+  // this tile: the slot (record index in dst, 32-bit wrap-around arithmetic) output position 0 would have in the bin's run
   __shared__ uint32_t sbase[kSplitMaxBins];
   __shared__ uint32_t s_rbase[9], s_fbase[9];  // (kernel-parameter arrays indexed by a register would be copied to local memory)
   __shared__ unsigned long long s_src[8];      // byte address and length (records) of the tile streams of this CTA
@@ -347,34 +317,48 @@ __global__ void __launch_bounds__(THREADS_, MINB) k_split_tma(SplitArgs a, BinPa
   __shared__ __align__(8) uint64_t mbar[2];
   __shared__ uint32_t s_next_len[2];
   const uint32_t tid = threadIdx.x;
-  const uint32_t level = SPEC ? (uint32_t)(SPEC & 3) : a.level;
-  const bool exact = SPEC ? false : a.base_off != nullptr;
-  const bool multi = SPEC ? (SPEC & 4) != 0 : a.ndest > 1;
+  const uint32_t level = SPEC ? (uint32_t)(SPEC & 3) : level_arg;
+  const bool exact = SPEC ? false : pl.base_off != nullptr;
+  const bool multi = SPEC ? (SPEC & 4) != 0 : pl.ndest > 1;
 #pragma unroll
   for (int i = 0; i < 9; i++)
     if (tid == (uint32_t)i) {
-      s_rbase[i] = a.rbase[i];
-      s_fbase[i] = a.fbase[i];
+      s_rbase[i] = pl.rbase[i];
+      s_fbase[i] = pl.fbase[i];
     }
-  const uint4* src = a.src;
-  uint64_t n = a.n;
+  // This level: level 1 claims slots in the coarse regions of l1 (sub_stride slots each) through cursor1, level 2 in
+  // the fine bins of mid (cap slots each) through cursor; in the optimistic layout a destination takes at most
+  // dst_stride records.  (The two pointers are picked where they are used, once per tile: held in registers across
+  // the tile loop they cost the run-time form more registers than the parameter reads.)
+  const uint32_t dst_stride = level == 1 ? (uint32_t)pl.sub_stride : pl.cap;
+  const uint32_t logF = __ffs(pl.F) - 1;
+  uint32_t region_first = pl.rbase[0], fine_base = pl.fbase[0];  // first coarse region / fine bin of this rank
+  if (multi) {
+#pragma unroll
+    for (int z = 1; z < 8; z++)
+      if (pl.me == (uint32_t)z) {
+        region_first = pl.rbase[z];
+        fine_base = pl.fbase[z];
+      }
+  }
   uint32_t coarse = 0;
   if (level == 2) {
     coarse = blockIdx.y;
     if (exact) {  // the coarse region is the union of its fine bins
-      uint32_t f0 = coarse * a.F, f1 = f0 + a.F < a.B ? f0 + a.F : a.B;
-      uint32_t o0 = a.base_off[f0], o1 = a.base_off[f1];
-      src += (size_t)o0 * R::kVec;
+      uint32_t f0 = coarse * pl.F, f1 = f0 + pl.F < pl.B ? f0 + pl.F : pl.B;
+      uint32_t o0 = pl.base_off[f0], o1 = pl.base_off[f1];
+      src = (const uint4*)pl.l1 + (size_t)o0 * R::kVec;
       n = o1 - o0;
     }
   }
   // The tile streams this CTA splits: one (the source range) or, for optimistic level 2, region `coarse` as every
-  // rank filled it -- ndest streams, the remote ones read over NVLink.  The CTA takes tiles x, x + gridDim.x, ... of
-  // EVERY stream, round-robin over the streams, so that its remote bulk copies fly while it splits local tiles
-  // (with one CTA per source the ranks first did all their local tiles, then sat on the link: level 2 took
-  // local time + link time).
+  // rank filled it -- ndest streams, the remote ones read over NVLink: sub_stride slots at peer[z] + (region_first +
+  // coarse) * sub_stride holding l1_counts[z * l1_zstride + ((region_first + coarse) << ctr_shift)] records.  The CTA
+  // takes tiles x, x + gridDim.x, ... of EVERY stream, round-robin over the streams, so that its remote bulk copies
+  // fly while it splits local tiles (with one CTA per source the ranks first did all their local tiles, then sat on
+  // the link: level 2 took local time + link time).
   const bool region_streams = level == 2 && !exact;
-  const uint32_t nsrc = (region_streams && multi) ? a.ndest : 1u;
+  const uint32_t nsrc = (region_streams && multi) ? pl.ndest : 1u;
 #pragma unroll
   for (int z = 0; z < 8; z++) {
     if (tid == (uint32_t)z && (uint32_t)z < nsrc) {
@@ -382,17 +366,11 @@ __global__ void __launch_bounds__(THREADS_, MINB) k_split_tma(SplitArgs a, BinPa
         s_src[0] = (unsigned long long)(uintptr_t)src;
         s_n[0] = (uint32_t)n;
       } else {
-        s_src[z] = a.peer[z] + (unsigned long long)(a.region_first + coarse) * a.seg_stride * RB;
-        const uint32_t c = a.seg_counts[(size_t)z * a.seg_zstride + ((size_t)(a.region_first + coarse) << a.ctr_shift)];
-        s_n[z] = c < a.seg_stride ? c : (uint32_t)a.seg_stride;
+        s_src[z] = pl.peer[z] + (unsigned long long)(region_first + coarse) * pl.sub_stride * RB;
+        const uint32_t c = pl.l1_counts[(size_t)z * pl.l1_zstride + ((size_t)(region_first + coarse) << bp.ctr_shift)];
+        s_n[z] = c < pl.sub_stride ? c : (uint32_t)pl.sub_stride;
       }
     }
-  }
-  uint32_t fine_base = a.fbase[0];  // first fine bin of this rank
-  if (multi) {
-#pragma unroll
-    for (int z = 1; z < 8; z++)
-      if (a.me == (uint32_t)z) fine_base = a.fbase[z];
   }
   if (tid == 0) {
     mbar_init(&mbar[0], 1);
@@ -407,7 +385,7 @@ __global__ void __launch_bounds__(THREADS_, MINB) k_split_tma(SplitArgs a, BinPa
   const uint32_t rounds = ntmax > blockIdx.x ? (ntmax - blockIdx.x + gridDim.x - 1) / gridDim.x : 0u;
   // the CTA's steps in order: round r = 0, 1, ... (tile blockIdx.x + r * gridDim.x), inside a round the streams
   // zrot, zrot + 1, ... (mod nsrc); kept as counters, advanced without a division
-  const uint32_t zrot = nsrc > 1 ? (blockIdx.x + a.me) % nsrc : 0u;
+  const uint32_t zrot = nsrc > 1 ? (blockIdx.x + pl.me) % nsrc : 0u;
   uint32_t st_r = 0, st_zi = 0, st_z = zrot;
   const uint4* cur_p = nullptr;
   uint32_t cur_len = 0;
@@ -453,11 +431,11 @@ __global__ void __launch_bounds__(THREADS_, MINB) k_split_tma(SplitArgs a, BinPa
         const uint32_t fine = bin_of<RB, WORLD>((const uint32_t*)(raw + (size_t)i * R::kVec), bp, nullptr, &dest);
         if (level == 1) {
           if (multi)
-            sub[k] = s_rbase[dest] + ((fine - s_fbase[dest]) >> a.logF);
+            sub[k] = s_rbase[dest] + ((fine - s_fbase[dest]) >> logF);
           else
-            sub[k] = fine >> a.logF;
+            sub[k] = fine >> logF;
         } else {
-          sub[k] = (fine - fine_base) & (a.F - 1u);
+          sub[k] = (fine - fine_base) & (pl.F - 1u);
         }
         rk[k] = atomicAdd(scnt + sub[k], 1u);
       }
@@ -467,7 +445,7 @@ __global__ void __launch_bounds__(THREADS_, MINB) k_split_tma(SplitArgs a, BinPa
     uint32_t v[IPT], ex[IPT], g[IPT], s = 0;
 #pragma unroll
     for (int i = 0; i < IPT; i++) {
-      v[i] = scnt[IPT * tid + i];  // (bins >= a.nbins stay zero)
+      v[i] = scnt[IPT * tid + i];  // (bins past this level's C1 / F stay zero)
       scnt[IPT * tid + i] = 0;     // ready for the next tile: every count of this one has been taken
       s += v[i];
     }
@@ -476,8 +454,8 @@ __global__ void __launch_bounds__(THREADS_, MINB) k_split_tma(SplitArgs a, BinPa
       g[i] = 0;
       const uint32_t b = IPT * tid + i;
       if (v[i]) {
-        const uint32_t dbin = level == 1 ? b : coarse * a.F + b;
-        g[i] = atomicAdd(a.cursor + ((size_t)dbin << a.ctr_shift), v[i]);  // result needed only after the placement
+        const uint32_t dbin = level == 1 ? b : coarse * pl.F + b;
+        g[i] = atomicAdd((level == 1 ? pl.cursor1 : pl.cursor) + ((size_t)dbin << pl.ctr_shift), v[i]);  // result needed only after the placement
       }
     }
     {
@@ -500,18 +478,18 @@ __global__ void __launch_bounds__(THREADS_, MINB) k_split_tma(SplitArgs a, BinPa
     for (int i = 0; i < IPT; i++) {
       const uint32_t b = IPT * tid + i;
       if (v[i]) {
-        const uint32_t dbin = level == 1 ? b : coarse * a.F + b;
+        const uint32_t dbin = level == 1 ? b : coarse * pl.F + b;
         uint32_t gg = g[i], first;
         if (exact) {  // absolute start of the destination region, always large enough
-          const uint32_t f = level == 1 ? b * a.F : dbin;
-          first = a.base_off[f];
+          const uint32_t f = level == 1 ? b * pl.F : dbin;
+          first = pl.base_off[f];
         } else {
-          first = dbin * (uint32_t)a.dst_stride;
-          if (gg + v[i] > a.capacity) {
+          first = dbin * dst_stride;
+          if (gg + v[i] > dst_stride) {
             // The run does not fit: the whole attempt is abandoned (ERRF_CAPACITY, the host redoes the shuffle with
             // the exact layout from the untouched input), so these records only have to land INSIDE the buffer:
             // at the start of the bin's region (the buffers carry one tile of slack behind the last region).
-            atomicOr(a.err_flags, (uint32_t)ERRF_CAPACITY);
+            atomicOr(pl.err_flags, (uint32_t)ERRF_CAPACITY);
             gg = 0;
           }
         }
@@ -527,7 +505,7 @@ __global__ void __launch_bounds__(THREADS_, MINB) k_split_tma(SplitArgs a, BinPa
         const uint32_t pb = perm[p];
         const uint32_t slot = sbase[pb >> 16] + p;
         const uint4* r = raw + (size_t)(pb & 0xffffu) * R::kVec;
-        uint4* d = a.dst + (size_t)slot * R::kVec;
+        uint4* d = (uint4*)(level == 1 ? pl.l1 : pl.mid) + (size_t)slot * R::kVec;
 #pragma unroll
         for (int vv = 0; vv < R::kVec; vv++) stg_stream(d + vv, r[vv]);
       }
@@ -538,10 +516,10 @@ __global__ void __launch_bounds__(THREADS_, MINB) k_split_tma(SplitArgs a, BinPa
   if (!DYN) {
     for (uint32_t it = 0; more; it++) {
       const uint32_t tn = cur_len;
-      const uint4* raw = (const uint4*)(smem_raw + (it & 1) * TILE_BYTES);
+      const uint4* raw = (const uint4*)(smem_raw + (it & 1) * kSplitTileBytes);
       // the other buffer was last read by the copy-out of the previous iteration (barrier at its end)
       more = advance();
-      if (tid == 0 && more) bulk_load(smem_raw + ((it & 1) ^ 1) * TILE_BYTES, cur_p, cur_len * RB, &mbar[(it & 1) ^ 1]);
+      if (tid == 0 && more) bulk_load(smem_raw + ((it & 1) ^ 1) * kSplitTileBytes, cur_p, cur_len * RB, &mbar[(it & 1) ^ 1]);
       mbar_wait(&mbar[it & 1], (it >> 1) & 1);
       if (tn == (uint32_t)T)
         split_tile(std::true_type{}, raw, tn);
@@ -563,16 +541,16 @@ __global__ void __launch_bounds__(THREADS_, MINB) k_split_tma(SplitArgs a, BinPa
     uint32_t tk = 0;  // (thread 0) the tile to prefetch next
     if (tid == 0) {
       if (tn) bulk_load(smem_raw, base + (uint64_t)blockIdx.x * T * R::kVec, tn * RB, &mbar[0]);
-      tk = gridDim.x + atomicAdd(a.ticket, 1u);
+      tk = gridDim.x + atomicAdd(pl.ticket, 1u);
     }
     for (uint32_t it = 0; tn; it++) {
-      const uint4* raw = (const uint4*)(smem_raw + (it & 1) * TILE_BYTES);
+      const uint4* raw = (const uint4*)(smem_raw + (it & 1) * kSplitTileBytes);
       if (tid == 0) {  // the other buffer was last read by the copy-out of the previous iteration (barrier at its end)
         const uint32_t len = tile_len(tk);
         s_next_len[(it & 1) ^ 1] = len;
         if (len) {
-          bulk_load(smem_raw + ((it & 1) ^ 1) * TILE_BYTES, base + (uint64_t)tk * T * R::kVec, len * RB, &mbar[(it & 1) ^ 1]);
-          tk = gridDim.x + atomicAdd(a.ticket, 1u);
+          bulk_load(smem_raw + ((it & 1) ^ 1) * kSplitTileBytes, base + (uint64_t)tk * T * R::kVec, len * RB, &mbar[(it & 1) ^ 1]);
+          tk = gridDim.x + atomicAdd(pl.ticket, 1u);
         }
       }
       mbar_wait(&mbar[it & 1], (it >> 1) & 1);
@@ -583,9 +561,9 @@ __global__ void __launch_bounds__(THREADS_, MINB) k_split_tma(SplitArgs a, BinPa
       tn = s_next_len[(it & 1) ^ 1];  // (written before the barriers of split_tile)
     }
     // the last CTA to leave resets the counters for the next launch on the stream
-    if (tid == 0 && atomicAdd(a.ticket + 1, 1u) == gridDim.x - 1) {
-      a.ticket[0] = 0;
-      a.ticket[1] = 0;
+    if (tid == 0 && atomicAdd(pl.ticket + 1, 1u) == gridDim.x - 1) {
+      pl.ticket[0] = 0;
+      pl.ticket[1] = 0;
     }
   }
 }
@@ -1381,7 +1359,7 @@ cudaError_t kernels_configure() {
   CFGC(16, false) CFGC(32, false) CFGC(32, true) CFGC(64, false) CFGC(64, true) CFGC(128, false) CFGC(128, true)
 #undef CFGC
 #define CFGT1(RB, SPEC)                                                                                  \
-  e = cudaFuncSetAttribute(k_split_tma<RB, kTmaTileBytes, 2, kTmaSplitThreads, SPEC>,                    \
+  e = cudaFuncSetAttribute(k_split_tma<RB, SPEC>,                                                        \
                            cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tma_split_smem(RB));        \
   if (e != cudaSuccess) return e;
 #define CFGT(RB) CFGT1(RB, 0) CFGT1(RB, 1) CFGT1(RB, 2) CFGT1(RB, 5) CFGT1(RB, 6)
@@ -1492,80 +1470,36 @@ int launch_scatter(int rb, const void* recs, uint64_t n, const BinParams& bp, ui
   DISPATCH_RB(rb, (k_scatter<RB><<<stream_grid(n, 256, 8), 256, 0, s>>>((const uint4*)recs, n, bp, cursor, (uint4*)mid)));
   return 1;
 }
-// level 1 (source -> coarse regions, possibly on peers) and level 2 (coarse regions -> fine bins) of the split
-static SplitArgs split_args(const BinParams& bp, const SplitPlan& pl) {
-  SplitArgs a{};
-  a.base_off = pl.base_off;
-  a.B = pl.B;
-  a.F = pl.F;
-  a.logF = 0;
-  while ((1u << a.logF) < pl.F) a.logF++;
-  a.ctr_shift = bp.ctr_shift;
-  a.err_flags = pl.err_flags;
-  a.ticket = pl.ticket;
-  a.ndest = pl.base_off ? 1u : pl.ndest;
-  a.me = pl.base_off ? 0u : pl.me;
-  for (int d = 0; d < 8; d++) a.peer[d] = pl.base_off ? 0ull : pl.peer[d];
-  for (int d = 0; d <= 8; d++) {
-    a.rbase[d] = pl.base_off ? (d ? pl.C1 : 0u) : pl.rbase[d];
-    a.fbase[d] = pl.base_off ? (d ? pl.B : 0u) : pl.fbase[d];
-  }
-  return a;
-}
-// the instantiation that has the launch-time facts folded in (k_split_tma's SPEC)
+// level 1 (source -> coarse regions, possibly on peers) and level 2 (coarse regions -> fine bins) of the split,
+// through the instantiation that has the launch-time facts folded in (k_split_tma's SPEC)
 template <int RB>
-static void launch_split_rb(dim3 grid, const SplitArgs& a, const BinParams& bp, cudaStream_t s) {
-  const int spec = a.base_off ? 0 : (int)a.level | (a.ndest > 1 ? 4 : 0);
+static void launch_split_rb(dim3 grid, const SplitPlan& pl, uint32_t level, const void* src, uint64_t n,
+                            const BinParams& bp, cudaStream_t s) {
+  const int spec = pl.base_off ? 0 : (int)level | (pl.ndest > 1 ? 4 : 0);
   const size_t smem = tma_split_smem(RB);
+  const uint4* r = (const uint4*)src;
   switch (spec) {
-    case 1: k_split_tma<RB, kTmaTileBytes, 2, kTmaSplitThreads, 1><<<grid, kTmaSplitThreads, smem, s>>>(a, bp); break;
-    case 2: k_split_tma<RB, kTmaTileBytes, 2, kTmaSplitThreads, 2><<<grid, kTmaSplitThreads, smem, s>>>(a, bp); break;
-    case 5: k_split_tma<RB, kTmaTileBytes, 2, kTmaSplitThreads, 5><<<grid, kTmaSplitThreads, smem, s>>>(a, bp); break;
-    case 6: k_split_tma<RB, kTmaTileBytes, 2, kTmaSplitThreads, 6><<<grid, kTmaSplitThreads, smem, s>>>(a, bp); break;
-    default: k_split_tma<RB, kTmaTileBytes, 2, kTmaSplitThreads, 0><<<grid, kTmaSplitThreads, smem, s>>>(a, bp); break;
+    case 1: k_split_tma<RB, 1><<<grid, kTmaSplitThreads, smem, s>>>(pl, level, r, n, bp); break;
+    case 2: k_split_tma<RB, 2><<<grid, kTmaSplitThreads, smem, s>>>(pl, level, r, n, bp); break;
+    case 5: k_split_tma<RB, 5><<<grid, kTmaSplitThreads, smem, s>>>(pl, level, r, n, bp); break;
+    case 6: k_split_tma<RB, 6><<<grid, kTmaSplitThreads, smem, s>>>(pl, level, r, n, bp); break;
+    default: k_split_tma<RB, 0><<<grid, kTmaSplitThreads, smem, s>>>(pl, level, r, n, bp); break;
   }
-}
-static void launch_split(int rb, dim3 grid, const SplitArgs& a, const BinParams& bp, cudaStream_t s) {
-  DISPATCH_RB(rb, (launch_split_rb<RB>(grid, a, bp, s)));
 }
 int launch_split_l1(int rb, const void* recs, uint64_t n, const BinParams& bp, const SplitPlan& pl, cudaStream_t s) {
   if (!n) return 0;
-  SplitArgs a = split_args(bp, pl);
-  const int ctas = 2 * g_sm_count;
-  a.src = (const uint4*)recs;
-  a.n = n;
-  a.dst = (uint4*)pl.l1;
-  a.dst_stride = pl.sub_stride;
-  a.cursor = pl.cursor1;
-  a.capacity = (uint32_t)std::min<uint64_t>(pl.sub_stride, 0xffffffffull);
-  a.nbins = pl.C1;
-  a.level = 1;
-  launch_split(rb, dim3(ctas), a, bp, s);
+  DISPATCH_RB(rb, (launch_split_rb<RB>(dim3(2 * g_sm_count), pl, 1, recs, n, bp, s)));
   return 1;
 }
 int launch_split_l2(int rb, const BinParams& bp, const SplitPlan& pl, cudaStream_t s) {
-  SplitArgs a = split_args(bp, pl);
   const int ctas = 2 * g_sm_count;
-  const uint32_t nsub = pl.base_off ? 1u : pl.ndest;
-  const uint32_t regions = pl.base_off ? pl.C1 : pl.C1_local;
+  const uint32_t regions = pl.C1_local;
   if (!regions) return 0;
-  a.src = (const uint4*)pl.l1;
-  a.seg_counts = pl.l1_counts;
-  a.seg_zstride = pl.l1_zstride;
-  a.seg_stride = pl.sub_stride;
-  a.region_first = a.rbase[a.me];
-  a.dst = (uint4*)pl.mid;
-  a.dst_stride = pl.cap;
-  a.cursor = pl.cursor;
-  a.capacity = pl.cap;
-  a.nbins = pl.F;
-  a.level = 2;
   // x CTAs per region (each takes every x-th tile of all the region's streams), chosen so that all CTAs fill whole waves of `ctas` resident CTAs
   // (e.g. C1 = 220, x = 2 on 264 slots would run 440 CTAs = 1.67 waves: a third of the second wave idle)
   int x = 1;
   double best = 0;
-  const uint64_t region_recs = pl.base_off ? (uint64_t)pl.F * pl.cap : pl.sub_stride;
-  const uint64_t tiles = nsub * ((region_recs * rb + kTmaTileBytes - 1) / kTmaTileBytes);
+  const uint64_t tiles = pl.ndest * ((pl.sub_stride * rb + kSplitTileBytes - 1) / kSplitTileBytes);
   for (int cand = 1; cand <= 16 && (uint64_t)cand <= std::max<uint64_t>(1, tiles / 4); cand++) {
     uint64_t total = (uint64_t)cand * regions, waves = (total + ctas - 1) / ctas;
     double eff = (double)total / (double)(waves * ctas);
@@ -1574,7 +1508,7 @@ int launch_split_l2(int rb, const BinParams& bp, const SplitPlan& pl, cudaStream
       x = cand;
     }
   }
-  launch_split(rb, dim3(x, regions), a, bp, s);
+  DISPATCH_RB(rb, (launch_split_rb<RB>(dim3(x, regions), pl, 2, nullptr, 0, bp, s)));
   return 1;
 }
 int launch_sort_reduce(int rb, const ShuffleBuffers& b, uint32_t B, uint32_t cap, int sm_count,

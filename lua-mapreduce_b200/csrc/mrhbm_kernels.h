@@ -31,6 +31,7 @@ MRHBM_HD inline uint32_t partition_slot(const BinParams& bp, uint32_t pid) {
 }
 
 constexpr int kSplitTileBytes = 40 * 1024;  // bytes of records k_split_tma partitions in shared memory at a time
+constexpr uint32_t kSplitMaxBins = 1024;    // bins one level of k_split_tma distinguishes
 constexpr int kCapBytes = 32 * 1024;  // record bytes one CTA sorts in shared memory (2 CTAs per SM)
 inline uint32_t cap_records(int rb) { return (uint32_t)(kCapBytes / rb); }
 
@@ -138,18 +139,22 @@ int launch_region_totals(const uint32_t* counts, uint64_t zstride, uint32_t G, u
                          uint32_t shift, uint32_t clamp, uint64_t* acc2, cudaStream_t s);
 int launch_exscan_rows(const uint32_t* all, uint32_t world, uint32_t stride, uint32_t base, uint32_t n,
                        uint32_t* out, uint32_t* totals, cudaStream_t s);
-// Two-level coalesced split.  Optimistic layout (base_off == nullptr): level 1 sends every record to the
-// coarse region of its bin inside this rank's region buffer l1 (all C1 regions of the job, sub_stride slots
-// each); level 2 of the rank that owns region y pulls it from every rank's buffer (peer[z], NVLink) and splits
-// it into fine bins of `cap` slots in mid.  C1 == B_local, F == 1 on one GPU = single level straight into mid.
-// Exact layout (base_off = bin offsets after k_hist + k_exscan): both levels write absolute slots, one GPU.
+// Two-level coalesced split, as the host plans it and k_split_tma reads it: the kernel takes this block as it is,
+// with the level and (level 1) its source records, and derives each level's destination, stride, cursor and
+// capacity from it.  Optimistic layout (base_off == nullptr): level 1 sends every record to the coarse region of
+// its bin inside this rank's region buffer l1 (all C1 regions of the job, sub_stride slots each); level 2 of the
+// rank that owns region y pulls it from every rank's buffer (peer[z], NVLink) and splits it into fine bins of `cap`
+// slots in mid.  C1 == B, F == 1 on one GPU with few bins = single level straight into mid.
+// Exact layout (base_off = bin offsets after k_hist + k_exscan): both levels write absolute slots into ONE
+// destination (on several GPUs the destination-major send buffer): ndest = 1, me = 0.
 struct SplitPlan {
   uint32_t B;                 // fine bins (of the whole job)
   uint32_t F;                 // fine bins per coarse region (power of two)
-  uint32_t C1;                // coarse regions of the whole job (bins level 1 distinguishes, <= 1024)
+  uint32_t C1;                // coarse regions of the whole job (bins level 1 distinguishes, <= kSplitMaxBins)
   uint32_t C1_local;          // regions this rank owns (level 2 splits these)
   uint32_t cap;               // slots per fine bin (optimistic)
-  uint64_t sub_stride;        // slots per coarse region in a rank's region buffer
+  uint64_t sub_stride;        // slots per coarse region in a rank's region buffer (exact layout: F * cap, what the
+                              // level-2 grid is sized by)
   uint32_t* cursor1;          // level-1 fill levels, [C1 << ctr_shift]
   uint32_t* cursor;           // fine fill levels, [B_local << ctr_shift]
   void* l1;                   // this rank's region buffer: C1 * sub_stride records
@@ -158,10 +163,12 @@ struct SplitPlan {
   const uint32_t* base_off;
   uint32_t ndest, me;         // ranks, this rank (1, 0 on a single GPU)
   unsigned long long peer[8]; // byte address of every rank's region buffer as mapped into this process
-  uint32_t rbase[9], fbase[9];  // first region / first fine bin of every rank
+  // rank d owns the coarse regions [rbase[d], rbase[d+1]) = its fine bins [fbase[d], fbase[d+1]) in blocks of F
+  uint32_t rbase[9], fbase[9];
   const uint32_t* l1_counts;  // level 2: fill of region r on rank z at l1_counts[z * l1_zstride + (r << ctr_shift)]
   uint64_t l1_zstride;
-  uint32_t* ticket;           // two zeroed words: level 1 hands out its tiles from a counter (the kernel zeroes them again)
+  uint32_t ctr_shift;         // spacing of the fill levels above (BinParams::ctr_shift)
+  uint32_t* ticket;          // two zeroed words: level 1 hands out its tiles from a counter (the kernel zeroes them again)
 };
 int launch_split_l1(int rb, const void* recs, uint64_t n, const BinParams& bp, const SplitPlan& pl, cudaStream_t s);
 int launch_split_l2(int rb, const BinParams& bp, const SplitPlan& pl, cudaStream_t s);
