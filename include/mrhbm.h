@@ -48,7 +48,16 @@ enum {
   MRHBM_PART_FNV_LUA = 0,  /* examples/WordCount/partitionfn.lua:8-16, bit-exact incl. the
                               double-precision rounding; pid = h % num_partitions */
   MRHBM_PART_MULHASH = 1,  /* u64 keys: mulhi(key * 0x9E3779B97F4A7C15, P) (SURVEY 8d cfg 4) */
-  MRHBM_PART_WORDHASH = 2  /* string keys: 64-bit word hash, mulhi(h, P) */
+  MRHBM_PART_WORDHASH = 2, /* string keys: 64-bit word hash, mulhi(h, P) */
+  /* u64 and string keys: key ranges.  num_partitions-1 non-decreasing splitters s_0 <= ... <= s_{P-2}
+     (duplicates allowed: they leave partitions empty); pid(key) = |{ i : s_i <= key }| (a key equal to a splitter
+     goes to the upper side).  Order is the library's key order: strings C-locale bytewise on the original bytes, a
+     proper prefix first; u64 keys numeric (= their 8 big-endian bytes).  A string splitter is any byte string (it may
+     be longer than the record class and hold 0x00 / 0x01); a u64 splitter is exactly 8 big-endian bytes.  With
+     P = 1 there are no splitters.  Partition k then holds the k-th slice of the key space, so the partitions read in
+     order 0 .. P-1 give every key in one global ascending order.  Set with mrhbm_set_splitters or
+     mrhbm_sample_splitters before the shuffle; a shuffle without them fails with MRHBM_E_INVAL. */
+  MRHBM_PART_RANGE = 3
 };
 /* built-in reducefn/combinerfn (examples/WordCount/reducefn.lua:1-15: integer sum,
  * associative + commutative + idempotent flags set) */
@@ -151,6 +160,18 @@ void mrhbm_map_abort(mrhbm_map *);
 int mrhbm_shuffle(mrhbm_ctx *);
 /* NON-EMPTY partitions owned by this rank, ascending -> red_jobs (server.lua:300-324) */
 int mrhbm_partitions(mrhbm_ctx *, uint32_t *ids, size_t cap, size_t *n);
+/* MRHBM_PART_RANGE: installs the num_partitions-1 splitters; splitter i is keys[off[i] .. off[i+1]) in original bytes
+ * (u64 keys: 8 big-endian bytes).  Kept across mrhbm_reset.  Several GPUs: every rank must install the same splitters
+ * (the next shuffle checks this and fails on all ranks with MRHBM_E_INVAL if they differ). */
+int mrhbm_set_splitters(mrhbm_ctx *, const void *keys, const uint64_t *off, size_t n);
+/* MRHBM_PART_RANGE: samples the committed pairs (collective on several GPUs, weighted by each rank's committed pairs),
+ * installs num_partitions-1 quantile splitters and returns them in the form above (*need receives the key bytes).
+ * They take at most (num_partitions-1) * key slot bytes (8 for u64 keys, mrhbm_record_bytes - 4 for strings): a
+ * buffer of that size needs no sizing call (keys = NULL, cap = 0), which does the whole sample too.  off has
+ * num_partitions entries.  Deterministic: the same committed pairs give the same splitters on every rank and call.
+ * Keys longer than the record class (host side, see mrhbm_emit_str) are not sampled.  mrhbm_checksum_result refuses
+ * (MRHBM_E_INVAL) once the splitters differ from those of the last shuffle. */
+int mrhbm_sample_splitters(mrhbm_ctx *, void *keys, size_t cap, uint64_t *off, size_t *need);
 
 /* ---- reduce side: utils.merge_iterator consumer (utils.lua:206-271, job.lua:264-284)
  *      and finalfn's pair iterator (server.lua:360-385) ---- */
@@ -170,7 +191,8 @@ typedef struct mrhbm_result_info {
   uint64_t pairs_recv; /* pairs this rank reduced (after the exchange) */
   uint64_t groups;     /* distinct keys owned by this rank */
   uint32_t key_bytes;  /* bytes per key slot in result_copy (8 or RB-4) */
-  uint32_t sorted;     /* 1: each partition is one ascending run on the device;
+  uint32_t sorted;     /* 1: each partition is one ascending run on the device (with MRHBM_PART_RANGE the
+                          partition-major rows are then ascending as a whole);
                           0: a partition is several ascending runs, merged by the iterator */
   uint32_t runs_per_partition;
   uint32_t partitions_nonempty;

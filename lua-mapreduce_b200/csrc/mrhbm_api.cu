@@ -85,6 +85,15 @@ struct mrhbm_ctx {
   uint64_t l1all_cap = 0;
   uint32_t *d_ipc = nullptr, *h_ipc = nullptr;  // 16 words per rank: the IPC handles
   uint32_t *d_sample = nullptr, *h_sample = nullptr;  // 256 buckets of the key sample
+  // MRHBM_PART_RANGE: the installed splitters (original bytes; u64 keys: 8 big-endian bytes), a digest that the shuffle
+  // compares across ranks, and their device form (RangeTable): prefixes, thresholds as key slots, per-partition inverse
+  // widths in one allocation
+  std::vector<std::string> spl;
+  bool spl_set = false;
+  uint64_t spl_digest = 0;
+  void* d_spl = nullptr;
+  uint32_t spl_fin = 0;  // finite thresholds (RangeBinParams::spl_n)
+  uint64_t shuffle_spl_digest = 0;  // the splitters the last shuffle partitioned with (mrhbm_checksum_result)
   std::recursive_mutex mu;                    // entry points serialise per ctx
   uint32_t *d_small = nullptr, *h_small = nullptr;  // 64 words each
   bool no_optimistic = false;  // sticky: a fixed-capacity bin overflowed once (skewed keys)
@@ -393,6 +402,8 @@ void unescape(const void* esc, size_t n, std::vector<unsigned char>& out) {
   }
 }
 
+int install_splitters(mrhbm_ctx* c, std::vector<std::string>&& spl);  // (with the shuffle, below)
+
 }  // namespace
 
 extern "C" {
@@ -427,7 +438,7 @@ int mrhbm_init(const mrhbm_config* cfg, mrhbm_ctx** out) {
   if (cfg->key_kind == MRHBM_KEY_U64) {
     c->rb = 16;
     c->kb = 8;
-    if (cfg->partitioner > MRHBM_PART_WORDHASH) return fail(c, MRHBM_E_INVAL, "unknown partitioner");
+    if (cfg->partitioner > MRHBM_PART_RANGE) return fail(c, MRHBM_E_INVAL, "unknown partitioner");
   } else if (cfg->key_kind == MRHBM_KEY_STR) {
     uint32_t m = cfg->max_key_bytes ? cfg->max_key_bytes : 27;
     if (m <= 27) c->rb = 32;
@@ -435,14 +446,18 @@ int mrhbm_init(const mrhbm_config* cfg, mrhbm_ctx** out) {
     else if (m <= 123) c->rb = 128;
     else return fail(c, MRHBM_E_KEY, "max_key_bytes %u exceeds the largest record class (123)", m);
     c->kb = c->rb - 4;
-    if (cfg->partitioner != MRHBM_PART_FNV_LUA && cfg->partitioner != MRHBM_PART_WORDHASH)
-      return fail(c, MRHBM_E_INVAL, "string keys need partitioner FNV_LUA or WORDHASH");
+    if (cfg->partitioner != MRHBM_PART_FNV_LUA && cfg->partitioner != MRHBM_PART_WORDHASH && cfg->partitioner != MRHBM_PART_RANGE)
+      return fail(c, MRHBM_E_INVAL, "string keys need partitioner FNV_LUA, WORDHASH or RANGE");
   } else
     return fail(c, MRHBM_E_INVAL, "unknown key_kind %u", cfg->key_kind);
   if (cfg->reducer != MRHBM_RED_SUM && cfg->reducer != MRHBM_RED_NONE) return fail(c, MRHBM_E_INVAL, "unknown reducer %u", cfg->reducer);
   if (cfg->reducer == MRHBM_RED_NONE && cfg->combiner) return fail(c, MRHBM_E_INVAL, "a general reducer cannot be combined on the device (combiner must be 0)");
   c->sb.no_reduce = cfg->reducer == MRHBM_RED_NONE;
   CU(c, cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
+  if (cfg->partitioner == MRHBM_PART_RANGE && cfg->num_partitions == 1) {  // one key range, no splitters: its table now
+    int rc = install_splitters(c, {});
+    if (rc) return rc;
+  }
   for (int i = 0; i < EV_N; i++) CU(c, cudaEventCreate(&c->ev[i]));
   CU(c, kernels_configure());
   CU(c, cudaMalloc((void**)&c->d_acc, 8 * sizeof(uint64_t)));
@@ -481,7 +496,7 @@ void mrhbm_destroy(mrhbm_ctx* c) {
                    c->csums,       c->d_acc,       c->d_table,    c->d_hd,        c->d_hall,    c->d_tot,
                    c->d_outoff,    c->d_segoff,    c->recvbuf,    c->bigbuf,      c->d_small,   c->comb,
                    c->gtab,        c->l1buf,       c->regions,    c->d_l1all,     c->d_sample,   c->d_tok_text[0],
-                   c->d_tok_text[1], c->d_tok_cnt, c->d_tok_off};
+                   c->d_tok_text[1], c->d_tok_cnt, c->d_tok_off, c->d_spl};
   for (void* p : frees)
     if (p) cudaFree(p);
   if (c->h_counters) cudaFreeHost(c->h_counters);
@@ -907,13 +922,15 @@ int mrhbm_reset(mrhbm_ctx* c) {
 // ---------------------------------------------------------------------------
 namespace {
 
-void set_range_hint(ShuffleBuffers& b, uint32_t S, uint32_t ordered) {
-  b.hint_S = (ordered && S > 1) ? S : 0;
+// The sort may take a bin's key range from its index only for the global key-ordered sub-bins (sub = mulhi(key, S));
+// the range partitioner's sub-bins are relative to their partition: min / max.
+void set_range_hint(const mrhbm_ctx* c, ShuffleBuffers& b, uint32_t S, uint32_t ordered) {
+  b.hint_S = (ordered && S > 1 && c->cfg.partitioner != MRHBM_PART_RANGE) ? S : 0;
   b.hint_q = S > 1 ? (uint64_t)(((unsigned __int128)1 << 64) / S) : 0;
 }
 
-BinParams make_bp(const mrhbm_ctx* c, uint32_t S, uint32_t ordered) {
-  BinParams bp{};
+RangeBinParams make_bp(const mrhbm_ctx* c, uint32_t S, uint32_t ordered) {
+  RangeBinParams bp{};
   bp.P = c->cfg.num_partitions;
   bp.S = S;
   bp.partitioner = c->cfg.partitioner;
@@ -924,10 +941,34 @@ BinParams make_bp(const mrhbm_ctx* c, uint32_t S, uint32_t ordered) {
   for (uint32_t k = 0; k < 4; k++)
     if ((1u << k) == bp.world) bp.wshift = k;
   for (int r = 0; r <= 8; r++) bp.pbase[r] = c->pbase[r];
+  if (c->cfg.partitioner == MRHBM_PART_RANGE && c->d_spl) {
+    const uint32_t n = (uint32_t)c->spl.size();
+    bp.spl_inv = (const ulonglong2*)c->d_spl;  // (first: 16-byte aligned)
+    bp.spl_pre = (const unsigned long long*)(bp.spl_inv + bp.P);
+    bp.spl_slot = (const uint32_t*)(bp.spl_pre + n);
+    bp.spl_n = c->spl_fin;
+    bp.spl_top = bp.spl_n ? 1u : 0u;
+    while (bp.spl_top && bp.spl_top * 2 <= bp.spl_n) bp.spl_top *= 2;
+  }
   return bp;
 }
 
-// all ranks: k <= 2 words from every rank (host values in, all[rank * k + i] out); synchronises the stream
+// The range partitioner's splitters must be the same on every rank: each shuffle's first all-gather carries two words
+// of their digest (all ones: none installed).  Fails on all ranks alike.
+uint32_t spl_word(const mrhbm_ctx* c, int i) {
+  return c->spl_set ? (uint32_t)(c->spl_digest >> (32 * i)) : 0xffffffffu;
+}
+int check_splitters(mrhbm_ctx* c, const uint32_t* all, int k, int first) {
+  bool ok = c->spl_set;
+  for (int r = 0; r < c->world; r++)
+    ok = ok && all[r * k + first] == spl_word(c, 0) && all[r * k + first + 1] == spl_word(c, 1);
+  if (!ok)
+    return fail(c, MRHBM_E_INVAL, c->spl_set ? "the ranks hold different splitters (mrhbm_set_splitters)"
+                                             : "MRHBM_PART_RANGE needs splitters: call mrhbm_set_splitters or mrhbm_sample_splitters");
+  return 0;
+}
+
+// all ranks: k <= 4 words from every rank (host values in, all[rank * k + i] out); synchronises the stream
 int gather_words(mrhbm_ctx* c, const uint32_t* mine, int k, uint32_t* all) {
   if (c->world == 1) {
     for (int i = 0; i < k; i++) all[i] = mine[i];
@@ -1096,6 +1137,29 @@ uint32_t pick_sub_bins(const mrhbm_ctx* c, uint64_t n_total, uint32_t copies = 1
   return (uint32_t)std::max<uint64_t>(1, (n_total + P * target - 1) / (P * target));
 }
 
+// The sub-bins of the exact layout's next attempt after a bin held more distinct keys than one CTA sorts (ERRF_SKEW):
+// twice as many.  Hash partitions are balanced, so that is enough; a key range may hold almost every key (splitters
+// inside a narrow key range), so the range partitioner sizes S at once from its fullest partition, whose records the
+// bin offsets of this attempt (h_bin_off, nb local bins of S per partition) already count: enough sub-bins that it
+// fills them to the mean pick_sub_bins aims at.  COLLECTIVE on several GPUs (the fullest partition of the job).
+// 0: more bins than the layout addresses.
+int next_sub_bins(mrhbm_ctx* c, uint32_t S, uint64_t nb, uint64_t* S_next) {
+  const uint64_t P = c->cfg.num_partitions;
+  uint64_t want = 2ull * S;
+  if (c->cfg.partitioner == MRHBM_PART_RANGE) {
+    uint32_t mx = 0;
+    for (uint64_t b = 0; b + S <= nb; b += S) mx = std::max(mx, c->h_bin_off[b + S] - c->h_bin_off[b]);
+    uint32_t all[8];
+    int rc = gather_words(c, &mx, 1, all);
+    if (rc) return rc;
+    for (int r = 0; r < c->world; r++) mx = std::max(mx, all[r]);
+    const double target = std::max(1.0, (double)c->cap - 6.0 * std::sqrt((double)c->cap));
+    while ((double)mx / (double)want > target && P * want < (1ull << 31)) want *= 2;
+  }
+  *S_next = P * want < (1ull << 31) ? want : 0;
+  return 0;
+}
+
 // The error flags of an attempt, OR-ed over all ranks: every rank must take the same branch.  The all-gather also
 // tells every rank whether any rank holds long keys (c->any_long).  One GPU: *ef stays as it is.
 int agree_flags(mrhbm_ctx* c, uint32_t* ef) {
@@ -1162,7 +1226,7 @@ int plan_split(SplitPlan& pl, const uint64_t* Bl, uint32_t ndest, uint32_t me, u
 // Exact layout (bin offsets in sb.bin_off after k_hist + k_exscan): the records of `live` go to their B bins in sb.mid
 // (on several GPUs: the destination-major send buffer), through the two-level coalesced split when there are enough
 // bins (claims relative to bin_off), else the direct scatter.
-int exact_split(mrhbm_ctx* c, const std::vector<Src>& live, const BinParams& bp, uint64_t B, uint64_t N, mrhbm_stats& st) {
+int exact_split(mrhbm_ctx* c, const std::vector<Src>& live, const RangeBinParams& bp, uint64_t B, uint64_t N, mrhbm_stats& st) {
   cudaStream_t s = c->stream;
   SplitPlan pl{};
   if (plan_split(pl, &B, 1, 0, c->cap, 0, true)) {
@@ -1224,6 +1288,7 @@ int publish(mrhbm_ctx* c, const ShuffleBuffers& v, uint64_t Bl, uint32_t S, uint
   c->groups = c->h_uoff[Bl];
   c->shuffled = true;
   c->compacted = false;
+  c->shuffle_spl_digest = c->spl_digest;
   st.bins = (uint32_t)Bl;
   st.sub_bins = S;
   st.big_bins = nbig;
@@ -1261,13 +1326,18 @@ int shuffle_fast(mrhbm_ctx* c, std::vector<Src>& live, uint64_t N, uint64_t N_in
   int rc = 0;
   // ---- would key-ordered sub-bins be balanced?  sample the keys before anything moves
   const bool want_ordered = c->cfg.key_kind == MRHBM_KEY_U64 && !(c->cfg.flags & MRHBM_F_FORCE_RUNS) && !c->no_ordered;
+  const bool range = c->cfg.partitioner == MRHBM_PART_RANGE;
   uint32_t nonuniform = 0;
-  if (want_ordered && N >= 4096) {
+  if (want_ordered && N >= 4096 && (!range || c->spl_set)) {
     CU(c, cudaMemsetAsync(c->d_sample, 0, 256 * sizeof(uint32_t), s));
     uint64_t total = 0;
+    const RangeBinParams sbp = make_bp(c, 1, 1);
     for (auto& r : live) {
       uint32_t ns = (uint32_t)std::min<uint64_t>(r.n, (uint64_t)((double)kSampleKeys * (double)r.n / (double)N) + 1);
-      st.launches += launch_sample_u64(r.p, r.n, ns, c->d_sample, s);
+      if (range)  // the position of the keys inside their partitions
+        st.launches += launch_sample_range_u64(r.p, r.n, ns, sbp, c->d_sample, s);
+      else
+        st.launches += launch_sample_u64(r.p, r.n, ns, c->d_sample, s);
       total += ns;
     }
     CU(c, cudaMemcpyAsync(c->h_sample, c->d_sample, 256 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
@@ -1279,14 +1349,17 @@ int shuffle_fast(mrhbm_ctx* c, std::vector<Src>& live, uint64_t N, uint64_t N_in
   }
   // ---- job-wide facts.  On several GPUs this all-gather is also the barrier that keeps a rank from refilling
   // its region buffer while a peer's level 2 of the previous shuffle may still read it.
-  uint32_t mine[2] = {(uint32_t)N, nonuniform}, all[16];
-  rc = gather_words(c, mine, 2, all);
+  // (range partitioner: two more words, the splitter digest)
+  const int k = range ? 4 : 2;
+  uint32_t mine[4] = {(uint32_t)N, nonuniform, spl_word(c, 0), spl_word(c, 1)}, all[32];
+  rc = gather_words(c, mine, k, all);
   if (rc) return rc;
+  if (range && (rc = check_splitters(c, all, k, 2))) return rc;
   uint64_t Nglobal = 0, Nmax = 0;
   for (int r = 0; r < G; r++) {
-    Nglobal += all[2 * r];
-    Nmax = std::max<uint64_t>(Nmax, all[2 * r]);
-    nonuniform |= all[2 * r + 1];
+    Nglobal += all[k * r];
+    Nmax = std::max<uint64_t>(Nmax, all[k * r]);
+    nonuniform |= all[k * r + 1];
   }
   if (Nglobal == 0) return 0;  // nothing to do here: the exact path handles the empty shuffle
   const uint32_t S = pick_sub_bins(c, Nglobal, c->cfg.combiner && G > 1 ? (uint32_t)G : 1u);
@@ -1338,7 +1411,7 @@ int shuffle_fast(mrhbm_ctx* c, std::vector<Src>& live, uint64_t N, uint64_t N_in
   for (int r = 0; r < 8; r++) pl.peer[r] = (unsigned long long)(uintptr_t)(G == 1 ? (r == 0 ? c->regions : nullptr) : c->peer_regions[r]);
   pl.l1_counts = G == 1 ? c->sb.hist : c->d_l1all;
   pl.l1_zstride = G == 1 ? 0 : ((uint64_t)pl.C1 << c->ctr_shift);
-  const BinParams bp = make_bp(c, S, ordered);
+  const RangeBinParams bp = make_bp(c, S, ordered);
   st.attempts++;
   CU(c, cudaMemsetAsync(c->sb.hist, 0, (((uint64_t)pl.C1) << c->ctr_shift) * sizeof(uint32_t), s));
   if (!single_level) CU(c, cudaMemsetAsync(c->sb.cursor, 0, (std::max<uint64_t>(Bl, 1) << c->ctr_shift) * sizeof(uint32_t), s));
@@ -1364,7 +1437,7 @@ int shuffle_fast(mrhbm_ctx* c, std::vector<Src>& live, uint64_t N, uint64_t N_in
   uint32_t* fine_cursor = single_level ? c->sb.hist : c->sb.cursor;
   ShuffleBuffers v = c->sb;
   v.cursor = fine_cursor;
-  set_range_hint(v, S, ordered);
+  set_range_hint(c, v, S, ordered);
   if (Bl) st.launches += launch_sort_reduce(c->rb, v, (uint32_t)Bl, c->cap, c->sm_count, s);
   CU(c, cudaEventRecord(c->ev[EV_SORT], s));
   CU(c, cudaEventRecord(c->ev[EV_BIG], s));
@@ -1422,7 +1495,7 @@ int shuffle_single_exact(mrhbm_ctx* c, std::vector<Src>& live, uint64_t N, uint6
     c->sb.stride = 0;
     for (;;) {
       st.attempts++;
-      BinParams bp = make_bp(c, S, ordered);
+      RangeBinParams bp = make_bp(c, S, ordered);
       CU(c, cudaMemsetAsync(c->sb.hist, 0, (B << c->ctr_shift) * sizeof(uint32_t), s));
       CU(c, cudaMemsetAsync(c->sb.counters, 0, 8 * sizeof(uint32_t), s));
       CU(c, cudaEventRecord(c->ev[EV_COMBINE], s));
@@ -1441,7 +1514,7 @@ int shuffle_single_exact(mrhbm_ctx* c, std::vector<Src>& live, uint64_t N, uint6
       c->sb.nseg = 1;
       c->sb.seg_off[0] = c->sb.bin_off;
       c->sb.seg_base[0] = 0;
-      set_range_hint(c->sb, S, ordered);
+      set_range_hint(c, c->sb, S, ordered);
       st.launches += launch_sort_reduce(c->rb, c->sb, (uint32_t)B, c->cap, c->sm_count, s);
       CU(c, cudaEventRecord(c->ev[EV_SORT], s));
       CU(c, cudaGetLastError());
@@ -1461,8 +1534,10 @@ int shuffle_single_exact(mrhbm_ctx* c, std::vector<Src>& live, uint64_t N, uint6
     rc = agree_flags(c, &ef);
     if (rc) return rc;
     if (ef & ERRF_SKEW) {
-      if (widen < 4 && (uint64_t)P * S * 2 < (1ull << 31)) {
-        S *= 2;
+      uint64_t S_next = 0;
+      if (widen < 4 && (rc = next_sub_bins(c, S, B, &S_next))) return rc;
+      if (S_next) {
+        S = (uint32_t)S_next;
         continue;
       }
       return fail(c, MRHBM_E_SKEW, "a bin holds more distinct keys than one SM can sort (%u oversized bins)", nbig);
@@ -1477,12 +1552,16 @@ int shuffle_single_exact(mrhbm_ctx* c, std::vector<Src>& live, uint64_t N, uint6
 int shuffle_multi_exact(mrhbm_ctx* c, std::vector<Src>& live, uint64_t N, uint64_t N_in, mrhbm_stats& st) {
   const int G = c->world, me = c->rank;
   const uint32_t P = c->cfg.num_partitions;
-  const uint32_t n32 = (uint32_t)N;
-  uint32_t all[8];
-  int rc = gather_words(c, &n32, 1, all);
+  // (range partitioner: two more words, the splitter digest)
+  const bool range = c->cfg.partitioner == MRHBM_PART_RANGE;
+  const int k = range ? 3 : 1;
+  const uint32_t mine[3] = {(uint32_t)N, spl_word(c, 0), spl_word(c, 1)};
+  uint32_t all[24];
+  int rc = gather_words(c, mine, k, all);
   if (rc) return rc;
+  if (range && (rc = check_splitters(c, all, k, 1))) return rc;
   uint64_t Nglobal = 0;
-  for (int r = 0; r < G; r++) Nglobal += all[r];
+  for (int r = 0; r < G; r++) Nglobal += all[k * r];
   uint32_t S = pick_sub_bins(c, Nglobal);
   uint32_t nbig = 0, ordered = 1;
   cudaStream_t s = c->stream;
@@ -1502,7 +1581,7 @@ int shuffle_multi_exact(mrhbm_ctx* c, std::vector<Src>& live, uint64_t N, uint64
     c->sb.stride = 0;
     for (;;) {
       st.attempts++;
-      BinParams bp = make_bp(c, S, ordered);
+      RangeBinParams bp = make_bp(c, S, ordered);
       CU(c, cudaMemsetAsync(c->sb.hist, 0, (B << c->ctr_shift) * sizeof(uint32_t), s));
       CU(c, cudaMemsetAsync(c->sb.counters, 0, 8 * sizeof(uint32_t), s));
       CU(c, cudaEventRecord(c->ev[EV_COMBINE], s));
@@ -1574,7 +1653,7 @@ int shuffle_multi_exact(mrhbm_ctx* c, std::vector<Src>& live, uint64_t N, uint64
     v.src = c->recvbuf;
     v.mid = nbig ? c->bigbuf : c->recvbuf;
     v.nseg = (uint32_t)G;
-    set_range_hint(v, S, ordered);
+    set_range_hint(c, v, S, ordered);
     for (int r = 0; r < G; r++) {
       v.seg_off[r] = c->d_segoff + (uint64_t)r * (Bl + 1);
       v.seg_base[r] = recv_off[r] / c->rb;
@@ -1594,8 +1673,10 @@ int shuffle_multi_exact(mrhbm_ctx* c, std::vector<Src>& live, uint64_t N, uint64
     rc = agree_flags(c, &ef);
     if (rc) return rc;
     if (ef & ERRF_SKEW) {
-      if (widen < 4 && (uint64_t)P * S * 2 < (1ull << 31)) {
-        S *= 2;
+      uint64_t S_next = 0;
+      if (widen < 4 && (rc = next_sub_bins(c, S, Bl, &S_next))) return rc;
+      if (S_next) {
+        S = (uint32_t)S_next;
         continue;
       }
       return fail(c, MRHBM_E_SKEW, "a bin holds more distinct keys than one SM can sort");
@@ -1617,8 +1698,15 @@ namespace {
 // ---- keys longer than a record slot: partitioned, exchanged and grouped on the host --------------------------
 // the partition bin_of (mrhbm_dev.cuh) would give the key if it fitted a slot: FNV-in-doubles over the ORIGINAL bytes
 // (examples/WordCount/partitionfn.lua:8-16), or the word hash over the little-endian words of the STORED bytes
+// (range partitioner: the original bytes against the original splitters, bisect_right)
 uint32_t host_partition(const mrhbm_ctx* c, const std::string& esc) {
   const uint32_t P = c->cfg.num_partitions;
+  if (c->cfg.partitioner == MRHBM_PART_RANGE) {
+    std::vector<unsigned char> raw;
+    unescape(esc.data(), esc.size(), raw);
+    const std::string key(raw.begin(), raw.end());
+    return (uint32_t)(std::upper_bound(c->spl.begin(), c->spl.end(), key) - c->spl.begin());
+  }
   if (c->cfg.partitioner == MRHBM_PART_FNV_LUA) {
     std::vector<unsigned char> raw;
     unescape(esc.data(), esc.size(), raw);
@@ -1636,6 +1724,86 @@ uint32_t host_partition(const mrhbm_ctx* c, const std::string& esc) {
   h ^= h >> 32;
   h *= 0x94D049BB133111EBull;
   return mulhi_u64_u32(h, P);
+}
+
+// ---- the range partitioner's splitters ------------------------------------------------------------------------
+// Checks the splitters (original bytes) and installs them with their device form (RangeBinParams):
+//   threshold t_i = the escaped splitter zero padded to the key slot, when it fits; else its first slot bytes plus one
+//   as a big-endian number: a key that fits a slot is >= a longer splitter iff its slot is STRICTLY greater than the
+//   splitter's first slot bytes (on equality the key is a proper prefix of it).  Then key >= s_i <=> slot >= t_i for
+//   every key a slot holds.  A threshold that would pass all ones lies above every slot key: it and the (equal or
+//   larger) splitters after it are left out of the device search (spl_n = the finite ones).
+//   u64 keys: t_i = the splitter; inv[p] = floor((2^128 - 1) / width_p) of partition p = [s_{p-1}, s_p) (s_{-1} = 0,
+//   s_{P-1} = 2^64) as {high, low} words, 0 for an empty partition: range_pos (mrhbm_dev.cuh) turns it into the key's
+//   position inside its partition as a 64-bit fraction.
+int install_splitters(mrhbm_ctx* c, std::vector<std::string>&& spl) {
+  const uint32_t P = c->cfg.num_partitions;
+  if (spl.size() != (size_t)P - 1)
+    return fail(c, MRHBM_E_INVAL, "%u partitions need %u splitters, got %zu", P, P - 1, spl.size());
+  const bool u64 = c->cfg.key_kind == MRHBM_KEY_U64;
+  for (size_t i = 0; i < spl.size(); i++) {
+    if (u64 && spl[i].size() != 8) return fail(c, MRHBM_E_INVAL, "u64 splitter %zu has %zu bytes (8 big-endian bytes)", i, spl[i].size());
+    if (i && spl[i] < spl[i - 1]) return fail(c, MRHBM_E_INVAL, "splitters must be non-decreasing (splitter %zu < splitter %zu)", i, i - 1);
+  }
+  const size_t n = spl.size(), kb = (size_t)c->kb;
+  std::vector<unsigned long long> pre(n), inv(2 * (size_t)P);
+  std::vector<unsigned char> slot(u64 ? 0 : n * kb);
+  uint32_t fin = 0;
+  if (u64) {
+    for (size_t i = 0; i < n; i++) {
+      uint64_t v = 0;
+      for (int b = 0; b < 8; b++) v = (v << 8) | (unsigned char)spl[i][b];
+      pre[i] = v;
+    }
+    fin = (uint32_t)n;
+    for (uint32_t p = 0; p < P; p++) {
+      const unsigned __int128 lo = p ? pre[p - 1] : 0, hi = p < n ? (unsigned __int128)pre[p] : (unsigned __int128)1 << 64;
+      const unsigned __int128 w = hi - lo, f = w ? ~(unsigned __int128)0 / w : 0;
+      inv[2 * p] = (unsigned long long)(f >> 64);
+      inv[2 * p + 1] = (unsigned long long)f;
+    }
+  } else {
+    std::vector<unsigned char> esc;
+    for (size_t i = 0; i < n; i++) {
+      esc.resize(2 * spl[i].size());
+      esc.resize(escape((const unsigned char*)spl[i].data(), spl[i].size(), esc.data()));
+      unsigned char* t = slot.data() + i * kb;
+      memcpy(t, esc.data(), std::min(esc.size(), kb));
+      if (esc.size() > kb) {  // + 1 in the last slot byte, carried
+        size_t j = kb;
+        while (j > 0 && t[j - 1] == 0xff) t[--j] = 0;
+        if (j == 0) break;  // above every slot key, and so is every later splitter
+        t[j - 1]++;
+      }
+      uint64_t v = 0;
+      for (int b = 0; b < 8; b++) v = (v << 8) | t[b];
+      pre[i] = v;
+      fin = (uint32_t)i + 1;
+    }
+  }
+  const size_t bytes = 8 * (2 * (size_t)P + n) + slot.size();
+  if (c->d_spl) CU(c, cudaFree(c->d_spl));
+  c->d_spl = nullptr;
+  c->spl_set = false;
+  CU(c, cudaMalloc(&c->d_spl, std::max<size_t>(bytes, 8)));
+  std::vector<unsigned char> host(bytes);
+  memcpy(host.data(), inv.data(), 16 * (size_t)P);
+  if (n) memcpy(host.data() + 16 * (size_t)P, pre.data(), 8 * n);
+  if (!slot.empty()) memcpy(host.data() + 16 * (size_t)P + 8 * n, slot.data(), slot.size());
+  CU(c, cudaMemcpyAsync(c->d_spl, host.data(), bytes, cudaMemcpyHostToDevice, c->stream));
+  CU(c, cudaStreamSynchronize(c->stream));
+  // digest (FNV-1a over the lengths and bytes): compared across ranks by the shuffle
+  uint64_t d = 0xcbf29ce484222325ull;
+  auto mixb = [&](unsigned char x) { d = (d ^ x) * 0x100000001b3ull; };
+  for (const std::string& sp : spl) {
+    for (int b = 0; b < 8; b++) mixb((unsigned char)(sp.size() >> (8 * b)));
+    for (unsigned char x : sp) mixb(x);
+  }
+  c->spl = std::move(spl);
+  c->spl_fin = fin;
+  c->spl_digest = d == ~0ull ? 0 : d;  // (all ones marks "none installed")
+  c->spl_set = true;
+  return MRHBM_OK;
 }
 
 int build_long_groups(mrhbm_ctx* c) {
@@ -1734,6 +1902,8 @@ int mrhbm_shuffle(mrhbm_ctx* c) {
   uint64_t N_in = 0, N = 0;
   for (auto& r : live_ranges(c)) N_in += r.second;
   if (N_in >= 0xfffffff0ull) return fail(c, MRHBM_E_INVAL, "more than 2^32 pairs on one GPU (%llu)", (unsigned long long)N_in);
+  if (c->cfg.partitioner == MRHBM_PART_RANGE && c->world == 1 && !c->spl_set)  // (several GPUs: at the first all-gather)
+    return fail(c, MRHBM_E_INVAL, "MRHBM_PART_RANGE needs splitters: call mrhbm_set_splitters or mrhbm_sample_splitters");
   mrhbm_stats st{};
   st.pairs = N_in;
   std::vector<Src> live;
@@ -1749,6 +1919,114 @@ int mrhbm_shuffle(mrhbm_ctx* c) {
   }
   rc = c->world > 1 ? shuffle_multi_exact(c, live, N, N_in, st) : shuffle_single_exact(c, live, N, N_in, st);
   return rc ? rc : build_long_groups(c);
+}
+
+int mrhbm_set_splitters(mrhbm_ctx* c, const void* keys, const uint64_t* off, size_t n) {
+  if (!c || (n && (!keys || !off))) return MRHBM_E_INVAL;
+  Entry g(c);
+  if (c->cfg.partitioner != MRHBM_PART_RANGE) return fail(c, MRHBM_E_INVAL, "splitters need partitioner MRHBM_PART_RANGE");
+  std::vector<std::string> spl(n);
+  for (size_t i = 0; i < n; i++) {
+    if (off[i + 1] < off[i]) return fail(c, MRHBM_E_INVAL, "splitter offsets must be non-decreasing");
+    spl[i].assign((const char*)keys + off[i], off[i + 1] - off[i]);
+  }
+  return install_splitters(c, std::move(spl));
+}
+
+int mrhbm_sample_splitters(mrhbm_ctx* c, void* keys, size_t cap, uint64_t* off, size_t* need) {
+  if (!c || !need) return MRHBM_E_INVAL;
+  Entry g(c);
+  if (c->cfg.partitioner != MRHBM_PART_RANGE) return fail(c, MRHBM_E_INVAL, "splitters need partitioner MRHBM_PART_RANGE");
+  const int G = c->world, me = c->rank;
+  const uint32_t P = c->cfg.num_partitions, KW = (uint32_t)c->kb / 4;
+  const auto live = live_ranges(c);
+  uint64_t N = 0;
+  for (auto& r : live) N += r.second;
+  // every rank's share of the sample follows its committed pairs (the same arithmetic on every rank)
+  const uint32_t n32 = (uint32_t)std::min<uint64_t>(N, 0xffffffffull);
+  uint32_t all[8];
+  int rc = gather_words(c, &n32, 1, all);
+  if (rc) return rc;
+  uint64_t Ntot = 0;
+  for (int r = 0; r < G; r++) Ntot += all[r];
+  if (!Ntot) return fail(c, MRHBM_E_INVAL, "no committed pairs to sample splitters from");
+  uint64_t m[8], mmax = 0, mtot = 0;
+  for (int r = 0; r < G; r++) {
+    m[r] = Ntot <= kSampleKeys ? all[r] : (uint64_t)(((unsigned __int128)kSampleKeys * all[r]) / Ntot);
+    mmax = std::max(mmax, m[r]);
+    mtot += m[r];
+  }
+  if (!mtot) return fail(c, MRHBM_E_INVAL, "no committed pairs to sample splitters from");
+  const size_t words = (size_t)std::max<uint64_t>(mmax, 1) * KW;
+  uint32_t* d_buf = nullptr;
+  CU(c, cudaMalloc((void**)&d_buf, words * 4 * (G + 1)));
+  uint32_t* d_recv = d_buf + words;
+  std::vector<uint32_t> h((size_t)words * G);
+  cudaError_t e = cudaMemsetAsync(d_buf, 0, words * 4, c->stream);
+  // evenly spaced over this rank's committed ranges, m[me] keys in all
+  uint64_t before = 0, taken = 0;
+  for (auto& r : live) {
+    const uint64_t upto = (uint64_t)(((unsigned __int128)m[me] * (before + r.second)) / N);
+    launch_sample_keys(c->rb, (const char*)c->pool + r.first * c->rb, r.second, (uint32_t)(upto - taken), d_buf + taken * KW, c->stream);
+    taken = upto;
+    before += r.second;
+  }
+  if (e == cudaSuccess) e = cudaGetLastError();
+  int rc2 = 0;
+  if (e == cudaSuccess) {
+    if (G > 1)
+      rc2 = comm_allgather_u32(c->comm, d_buf, d_recv, words, c->stream, &c->err);
+    else
+      e = cudaMemcpyAsync(d_recv, d_buf, words * 4, cudaMemcpyDeviceToDevice, c->stream);
+  }
+  if (e == cudaSuccess && !rc2) e = cudaMemcpyAsync(h.data(), d_recv, words * 4 * G, cudaMemcpyDeviceToHost, c->stream);
+  if (e == cudaSuccess && !rc2) e = cudaStreamSynchronize(c->stream);
+  cudaFree(d_buf);
+  if (rc2) return rc2;
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    return fail(c, MRHBM_E_CUDA, "splitter sample: %s", cudaGetErrorString(e));
+  }
+  // the sample in key order: u64 numerically, strings bytewise over the (order preserving) escaped slot
+  std::vector<const uint32_t*> smp;
+  smp.reserve(mtot);
+  for (int r = 0; r < G; r++)
+    for (uint64_t i = 0; i < m[r]; i++) smp.push_back(h.data() + (size_t)r * words + i * KW);
+  const bool u64 = c->cfg.key_kind == MRHBM_KEY_U64;
+  auto key64 = [](const uint32_t* w) { return (uint64_t)w[0] | ((uint64_t)w[1] << 32); };
+  std::sort(smp.begin(), smp.end(), [&](const uint32_t* a, const uint32_t* b) {
+    return u64 ? key64(a) < key64(b) : memcmp(a, b, (size_t)KW * 4) < 0;
+  });
+  std::vector<std::string> spl(P - 1);
+  std::vector<unsigned char> raw;
+  for (uint32_t i = 1; i < P; i++) {
+    const uint32_t* w = smp[(size_t)(((unsigned __int128)i * mtot) / P)];
+    if (u64) {
+      const uint64_t v = key64(w);
+      spl[i - 1].resize(8);
+      for (int b = 0; b < 8; b++) spl[i - 1][b] = (char)(v >> (56 - 8 * b));
+    } else {
+      const unsigned char* k = (const unsigned char*)w;
+      size_t len = 0;
+      while (len < (size_t)KW * 4 && k[len]) len++;
+      unescape(k, len, raw);
+      spl[i - 1].assign(raw.begin(), raw.end());
+    }
+  }
+  size_t total = 0;
+  for (auto& sp : spl) total += sp.size();
+  *need = total;
+  rc = install_splitters(c, std::move(spl));
+  if (rc) return rc;
+  if (keys && cap < total) return fail(c, MRHBM_E_INVAL, "the splitters need %zu bytes, the buffer holds %zu", total, cap);
+  size_t o = 0;
+  for (size_t i = 0; i < c->spl.size(); i++) {
+    if (off) off[i] = o;
+    if (keys) memcpy((char*)keys + o, c->spl[i].data(), c->spl[i].size());
+    o += c->spl[i].size();
+  }
+  if (off) off[c->spl.size()] = o;
+  return MRHBM_OK;
 }
 
 int mrhbm_stats_get(mrhbm_ctx* c, mrhbm_stats* out) {
@@ -1826,6 +2104,8 @@ int mrhbm_checksum_result(mrhbm_ctx* c, uint64_t out[6]) {
   if (!c || !out) return MRHBM_E_INVAL;
   Entry g(c);
   if (!c->shuffled) return fail(c, MRHBM_E_INVAL, "no shuffle result (call mrhbm_shuffle first)");
+  if (c->cfg.partitioner == MRHBM_PART_RANGE && c->spl_digest != c->shuffle_spl_digest)
+    return fail(c, MRHBM_E_INVAL, "the splitters changed after the shuffle: its partitions cannot be checked against them");
   CU(c, cudaMemsetAsync(c->d_acc, 0, 8 * sizeof(uint64_t), c->stream));
   launch_checksum_out(c->rb, c->rv, c->B, make_bp(c, c->S, c->ordered), c->bin_base, c->d_acc, c->stream);
   CU(c, cudaGetLastError());

@@ -9,6 +9,7 @@
 // u64 keys are the reference's 8-byte big-endian strings (SURVEY A.4) == numeric order.
 #pragma once
 #include <cstdint>
+#include <type_traits>
 #include <cuda_runtime.h>
 
 #include "mrhbm_kernels.h"
@@ -174,15 +175,59 @@ __host__ __device__ __forceinline__ uint32_t mulhi_u64_u32(uint64_t x, uint32_t 
   return (uint32_t)((hi + (lo >> 32)) >> 32);
 }
 
+// MRHBM_PART_RANGE: pid = number of thresholds t_i <= slot(key).  Binary search over the 64-bit prefixes (read through
+// the read-only cache: the first levels of the search are the same few words for every key), then, for string keys
+// whose prefix ties with thresholds, a walk down over the tied ones with the full slot compare.
+template <int RB>
+__device__ __forceinline__ uint32_t range_pid(const uint32_t* r, const RangeBinParams& bp) {
+  const uint64_t kp = key_prefix64<RB>(r);
+  uint32_t pos = 0;
+  for (uint32_t step = bp.spl_top; step; step >>= 1) {
+    const uint32_t q = pos + step;
+    if (q <= bp.spl_n && __ldg(bp.spl_pre + q - 1) <= kp) pos = q;
+  }
+  if constexpr (!Rec<RB>::kU64) {
+    constexpr int KW = Rec<RB>::kKeyWords;
+    while (pos > 0 && __ldg(bp.spl_pre + pos - 1) == kp) {
+      const uint32_t* t = bp.spl_slot + (size_t)(pos - 1) * KW;
+      int c = 0;
+#pragma unroll
+      for (int i = 2; i < KW; i++) {
+        const uint32_t x = be_word<RB>(r, i), y = bswap32(__ldg(t + i));
+        if (c == 0 && x != y) c = x < y ? -1 : 1;
+      }
+      if (c >= 0) break;  // key >= t_{pos-1}: so are all below it
+      pos--;
+    }
+  }
+  return pos;
+}
+
+// MRHBM_PART_RANGE, u64 keys: the position of key inside its partition [lo, lo + w) as a 64-bit fraction,
+// floor((key - lo) * F / 2^64) with F = floor((2^128 - 1) / w) = {hi, lo64}: q * hi + mulhi(q, lo64).  Monotone in the
+// key and < 2^64 (q < w); 128-bit F keeps it exact where floor(2^64 / w) alone would lose up to 1 / (2^64 / w).
+__device__ __forceinline__ uint64_t range_pos(const RangeBinParams& bp, uint64_t key, uint32_t pid) {
+  const uint64_t lo = pid ? __ldg(bp.spl_pre + pid - 1) : 0ull;
+  const ulonglong2 f = __ldg(bp.spl_inv + pid);
+  const uint64_t q = key - lo;
+  return q * f.x + __umul64hi(q, f.y);
+}
+
 // partition id, owning rank and bin (= slot(pid)*S + sub) of a record held in registers / smem words
 // WORLD: 0 = bp.world read at run time, 1 = one GPU, 2 = several (folded by the caller's template)
-template <int RB, int WORLD = 0>
-__device__ __forceinline__ uint32_t bin_of(const uint32_t* r, const BinParams& bp, uint32_t* pid_out,
+// BP = RangeBinParams: MRHBM_PART_RANGE, a compile-time variant (the hash instances do not carry its search).  Its
+// sub-bins: u64 keys with bp.ordered = mulhi(range_pos, S), monotone in the key and < S, so that a partition is one
+// ascending run; otherwise the word hash.
+template <int RB, int WORLD = 0, typename BP = BinParams>
+__device__ __forceinline__ uint32_t bin_of(const uint32_t* r, const BP& bp, uint32_t* pid_out,
                                            uint32_t* dest_out = nullptr) {
+  constexpr bool RANGE = std::is_same<BP, RangeBinParams>::value;
   uint32_t pid;
   uint64_t h = 0;  // uniform 64-bit hash; feeds the hash sub-bin (only computed further when needed)
   const bool mul = bp.partitioner == 1u && Rec<RB>::kU64;
-  if (mul) {  // MULHASH
+  if constexpr (RANGE) {
+    pid = range_pid<RB>(r, bp);
+  } else if (mul) {  // MULHASH
     uint64_t key = (uint64_t)r[0] | ((uint64_t)r[1] << 32);
     h = key * 0x9E3779B97F4A7C15ull;
     pid = mulhi_u64_u32(h, bp.P);
@@ -193,7 +238,17 @@ __device__ __forceinline__ uint32_t bin_of(const uint32_t* r, const BinParams& b
     pid = mulhi_u64_u32(h, bp.P);
   }
   uint32_t sub = 0;
-  if (bp.S > 1) {
+  if constexpr (RANGE) {
+    if (bp.S > 1) {
+      uint64_t src;
+      if (Rec<RB>::kU64 && bp.ordered) {
+        src = range_pos(bp, (uint64_t)r[0] | ((uint64_t)r[1] << 32), pid);
+      } else {
+        src = word_hash<RB>(r);
+      }
+      sub = mulhi_u64_u32(src, bp.S);
+    }
+  } else if (bp.S > 1) {
     uint64_t src;
     if (bp.ordered) {
       src = key_prefix64<RB>(r);

@@ -169,8 +169,8 @@ struct Unroll {
   static constexpr int U = RB == 16 ? 8 : RB == 32 ? 4 : RB == 64 ? 2 : 1;
 };
 
-template <int RB>
-__global__ void __launch_bounds__(256) k_hist(const uint4* __restrict__ recs, uint64_t n, BinParams bp,
+template <int RB, typename BP = BinParams>
+__global__ void __launch_bounds__(256) k_hist(const uint4* __restrict__ recs, uint64_t n, BP bp,
                                               uint32_t* __restrict__ hist) {
   constexpr int U = Unroll<RB>::U;
   uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
@@ -189,8 +189,8 @@ __global__ void __launch_bounds__(256) k_hist(const uint4* __restrict__ recs, ui
   }
 }
 
-template <int RB>
-__global__ void __launch_bounds__(256) k_scatter(const uint4* __restrict__ recs, uint64_t n, BinParams bp,
+template <int RB, typename BP = BinParams>
+__global__ void __launch_bounds__(256) k_scatter(const uint4* __restrict__ recs, uint64_t n, BP bp,
                                                  uint32_t* __restrict__ cursor, uint4* __restrict__ mid) {
   constexpr int U = Unroll<RB>::U;
   uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
@@ -234,6 +234,38 @@ __global__ void __launch_bounds__(256) k_sample_u64(const uint4* __restrict__ re
   }
   __syncthreads();
   if (h[threadIdx.x]) atomicAdd(hist256 + threadIdx.x, h[threadIdx.x]);
+}
+
+// The same decision for MRHBM_PART_RANGE: the top 8 bits of each sampled key's position inside its partition, the
+// source of the range-relative key-ordered sub-bin (bin_of).
+__global__ void __launch_bounds__(256) k_sample_range_u64(const uint4* __restrict__ recs, uint64_t n, uint32_t nsample,
+                                                          RangeBinParams bp, uint32_t* __restrict__ hist256) {
+  __shared__ uint32_t h[256];
+  h[threadIdx.x] = 0;
+  __syncthreads();
+  for (uint32_t i = blockIdx.x * 256 + threadIdx.x; i < nsample; i += gridDim.x * 256) {
+    const uint64_t idx = (uint64_t)(((unsigned __int128)i * n) / nsample);
+    const uint4 r = __ldg(recs + idx);
+    const uint32_t w[2] = {r.x, r.y};
+    const uint32_t pid = range_pid<16>(w, bp);
+    atomicAdd(&h[range_pos(bp, (uint64_t)r.x | ((uint64_t)r.y << 32), pid) >> 56], 1u);
+  }
+  __syncthreads();
+  if (h[threadIdx.x]) atomicAdd(hist256 + threadIdx.x, h[threadIdx.x]);
+}
+
+// Key slots of `nsample` evenly spaced records (the positions k_sample_u64 takes), for the splitter sample of
+// MRHBM_PART_RANGE: one thread per key word.
+template <int RB>
+__global__ void __launch_bounds__(256) k_sample_keys(const uint32_t* __restrict__ recs, uint64_t n, uint32_t nsample,
+                                                     uint32_t* __restrict__ out) {
+  constexpr int KW = Rec<RB>::kKeyWords;
+  const uint64_t total = (uint64_t)nsample * KW;
+  for (uint64_t j = (uint64_t)blockIdx.x * 256 + threadIdx.x; j < total; j += (uint64_t)gridDim.x * 256) {
+    const uint32_t i = (uint32_t)(j / KW), k = (uint32_t)(j % KW);
+    const uint64_t idx = (uint64_t)(((unsigned __int128)i * n) / nsample);
+    out[j] = __ldg(recs + idx * Rec<RB>::kWords + k);
+  }
 }
 
 // ============================================================================
@@ -292,20 +324,23 @@ __device__ __forceinline__ void bulk_load(void* dst_smem, const void* src_gmem, 
 // The kernel is issue bound (its time follows the instruction count), so
 // what is known at launch time is folded at compile time.  SPEC = 0: level, number of GPUs and layout are read from
 // the plan (exact layouts, the rare paths).  Otherwise the optimistic layout with bits 0-1 = level and
-// bit 2 = several GPUs.
+// bit 2 = several GPUs.  Bit 3 (added to either form) = MRHBM_PART_RANGE: those instances take a RangeBinParams and
+// carry the range search, the hash instances keep their parameters and code.
 // Arguments: the plan as the host made it, the level (1 or 2; folded when SPEC != 0) and, at level 1, the records
 // it splits (src, n).  Level 2 reads the regions of the plan's region buffers (l1, peer[]).
 template <int RB, int SPEC = 0>
 __global__ void __launch_bounds__(kTmaSplitThreads, 2)
-    k_split_tma(SplitPlan pl, uint32_t level_arg, const uint4* src, uint64_t n, BinParams bp) {
+    k_split_tma(SplitPlan pl, uint32_t level_arg, const uint4* src, uint64_t n,
+                typename std::conditional<(SPEC & 8) != 0, RangeBinParams, BinParams>::type bp) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   using R = Rec<RB>;
   constexpr int THREADS = kTmaSplitThreads;
   constexpr int T = kSplitTileBytes / RB;            // records per tile
   constexpr int U = (T + THREADS - 1) / THREADS;     // records per thread
   constexpr int IPT = kSplitMaxBins / THREADS;       // bins per thread in the scan
-  constexpr int WORLD = SPEC ? ((SPEC & 4) ? 2 : 1) : 0;
-  constexpr bool DYN = SPEC != 0 && (SPEC & 3) == 1;  // tiles from a ticket counter (level 1, optimistic layout)
+  constexpr int SP = SPEC & 7;
+  constexpr int WORLD = SP ? ((SP & 4) ? 2 : 1) : 0;
+  constexpr bool DYN = SP != 0 && (SP & 3) == 1;  // tiles from a ticket counter (level 1, optimistic layout)
   static_assert(T < 65536 && kSplitMaxBins <= 65536, "perm packs (raw index, bin) into 16 + 16 bits");
   uint32_t* perm = (uint32_t*)(smem_raw + 2 * kSplitTileBytes);  // output position -> raw index | bin << 16
   __shared__ uint32_t scnt[kSplitMaxBins], soff[kSplitMaxBins];
@@ -317,9 +352,9 @@ __global__ void __launch_bounds__(kTmaSplitThreads, 2)
   __shared__ __align__(8) uint64_t mbar[2];
   __shared__ uint32_t s_next_len[2];
   const uint32_t tid = threadIdx.x;
-  const uint32_t level = SPEC ? (uint32_t)(SPEC & 3) : level_arg;
-  const bool exact = SPEC ? false : pl.base_off != nullptr;
-  const bool multi = SPEC ? (SPEC & 4) != 0 : pl.ndest > 1;
+  const uint32_t level = SP ? (uint32_t)(SP & 3) : level_arg;
+  const bool exact = SP ? false : pl.base_off != nullptr;
+  const bool multi = SP ? (SP & 4) != 0 : pl.ndest > 1;
 #pragma unroll
   for (int i = 0; i < 9; i++)
     if (tid == (uint32_t)i) {
@@ -1276,8 +1311,8 @@ __global__ void __launch_bounds__(256) k_checksum_in(const uint4* __restrict__ r
   }
 }
 
-template <int RB>
-__global__ void __launch_bounds__(256) k_checksum_out(ShuffleBuffers b, uint32_t B, BinParams bp,
+template <int RB, typename BP = BinParams>
+__global__ void __launch_bounds__(256) k_checksum_out(ShuffleBuffers b, uint32_t B, BP bp,
                                                       uint32_t bin_base, unsigned long long* acc) {
   constexpr int KW = Rec<RB>::kKeyWords;
   uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
@@ -1362,7 +1397,8 @@ cudaError_t kernels_configure() {
   e = cudaFuncSetAttribute(k_split_tma<RB, SPEC>,                                                        \
                            cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tma_split_smem(RB));        \
   if (e != cudaSuccess) return e;
-#define CFGT(RB) CFGT1(RB, 0) CFGT1(RB, 1) CFGT1(RB, 2) CFGT1(RB, 5) CFGT1(RB, 6)
+#define CFGT(RB) CFGT1(RB, 0) CFGT1(RB, 1) CFGT1(RB, 2) CFGT1(RB, 5) CFGT1(RB, 6) \
+  CFGT1(RB, 8) CFGT1(RB, 9) CFGT1(RB, 10) CFGT1(RB, 13) CFGT1(RB, 14)
   CFGT(16) CFGT(32) CFGT(64) CFGT(128)
 #undef CFGT
 #undef CFGT1
@@ -1388,9 +1424,12 @@ int launch_gen_zipf32(void* dst, uint64_t seed, uint64_t start, uint64_t n, cons
   k_gen_zipf32<<<stream_grid(n, 256, 8), 256, 0, s>>>((uint4*)dst, seed, start, n, d_table, V);
   return 1;
 }
-int launch_hist(int rb, const void* recs, uint64_t n, const BinParams& bp, uint32_t* hist, cudaStream_t s) {
+int launch_hist(int rb, const void* recs, uint64_t n, const RangeBinParams& bp, uint32_t* hist, cudaStream_t s) {
   if (!n) return 0;
-  DISPATCH_RB(rb, (k_hist<RB><<<stream_grid(n, 256, 8), 256, 0, s>>>((const uint4*)recs, n, bp, hist)));
+  if (bp.partitioner == kPartRange)
+    DISPATCH_RB(rb, (k_hist<RB, RangeBinParams><<<stream_grid(n, 256, 8), 256, 0, s>>>((const uint4*)recs, n, bp, hist)))
+  else
+    DISPATCH_RB(rb, (k_hist<RB><<<stream_grid(n, 256, 8), 256, 0, s>>>((const uint4*)recs, n, (const BinParams&)bp, hist)))
   return 1;
 }
 int launch_exscan(const uint32_t* in, uint32_t n, uint32_t* out_excl, uint32_t* out_copy, uint32_t* out_dense,
@@ -1464,34 +1503,54 @@ int launch_sample_u64(const void* recs, uint64_t n, uint32_t nsample, uint32_t* 
   k_sample_u64<<<(nsample + 255) / 256 < 256 ? (nsample + 255) / 256 : 256, 256, 0, s>>>((const uint4*)recs, n, nsample, hist256);
   return 1;
 }
-int launch_scatter(int rb, const void* recs, uint64_t n, const BinParams& bp, uint32_t* cursor, void* mid,
+int launch_sample_range_u64(const void* recs, uint64_t n, uint32_t nsample, const RangeBinParams& bp, uint32_t* hist256,
+                            cudaStream_t s) {
+  if (!n || !nsample) return 0;
+  k_sample_range_u64<<<(nsample + 255) / 256 < 256 ? (nsample + 255) / 256 : 256, 256, 0, s>>>((const uint4*)recs, n, nsample, bp, hist256);
+  return 1;
+}
+int launch_sample_keys(int rb, const void* recs, uint64_t n, uint32_t nsample, uint32_t* out, cudaStream_t s) {
+  if (!n || !nsample) return 0;
+  DISPATCH_RB(rb, (k_sample_keys<RB><<<stream_grid((uint64_t)nsample * Rec<RB>::kKeyWords, 256, 4), 256, 0, s>>>((const uint32_t*)recs, n, nsample, out)));
+  return 1;
+}
+int launch_scatter(int rb, const void* recs, uint64_t n, const RangeBinParams& bp, uint32_t* cursor, void* mid,
                    cudaStream_t s) {
   if (!n) return 0;
-  DISPATCH_RB(rb, (k_scatter<RB><<<stream_grid(n, 256, 8), 256, 0, s>>>((const uint4*)recs, n, bp, cursor, (uint4*)mid)));
+  if (bp.partitioner == kPartRange)
+    DISPATCH_RB(rb, (k_scatter<RB, RangeBinParams><<<stream_grid(n, 256, 8), 256, 0, s>>>((const uint4*)recs, n, bp, cursor, (uint4*)mid)))
+  else
+    DISPATCH_RB(rb, (k_scatter<RB><<<stream_grid(n, 256, 8), 256, 0, s>>>((const uint4*)recs, n, (const BinParams&)bp, cursor, (uint4*)mid)))
   return 1;
 }
 // level 1 (source -> coarse regions, possibly on peers) and level 2 (coarse regions -> fine bins) of the split,
 // through the instantiation that has the launch-time facts folded in (k_split_tma's SPEC)
 template <int RB>
 static void launch_split_rb(dim3 grid, const SplitPlan& pl, uint32_t level, const void* src, uint64_t n,
-                            const BinParams& bp, cudaStream_t s) {
-  const int spec = pl.base_off ? 0 : (int)level | (pl.ndest > 1 ? 4 : 0);
+                            const RangeBinParams& bp, cudaStream_t s) {
+  const BinParams& hb = bp;  // the hash instances' parameter block
+  const int spec = (pl.base_off ? 0 : (int)level | (pl.ndest > 1 ? 4 : 0)) | (bp.partitioner == kPartRange ? 8 : 0);
   const size_t smem = tma_split_smem(RB);
   const uint4* r = (const uint4*)src;
   switch (spec) {
-    case 1: k_split_tma<RB, 1><<<grid, kTmaSplitThreads, smem, s>>>(pl, level, r, n, bp); break;
-    case 2: k_split_tma<RB, 2><<<grid, kTmaSplitThreads, smem, s>>>(pl, level, r, n, bp); break;
-    case 5: k_split_tma<RB, 5><<<grid, kTmaSplitThreads, smem, s>>>(pl, level, r, n, bp); break;
-    case 6: k_split_tma<RB, 6><<<grid, kTmaSplitThreads, smem, s>>>(pl, level, r, n, bp); break;
-    default: k_split_tma<RB, 0><<<grid, kTmaSplitThreads, smem, s>>>(pl, level, r, n, bp); break;
+    case 1: k_split_tma<RB, 1><<<grid, kTmaSplitThreads, smem, s>>>(pl, level, r, n, hb); break;
+    case 2: k_split_tma<RB, 2><<<grid, kTmaSplitThreads, smem, s>>>(pl, level, r, n, hb); break;
+    case 5: k_split_tma<RB, 5><<<grid, kTmaSplitThreads, smem, s>>>(pl, level, r, n, hb); break;
+    case 6: k_split_tma<RB, 6><<<grid, kTmaSplitThreads, smem, s>>>(pl, level, r, n, hb); break;
+    case 8: k_split_tma<RB, 8><<<grid, kTmaSplitThreads, smem, s>>>(pl, level, r, n, bp); break;
+    case 9: k_split_tma<RB, 9><<<grid, kTmaSplitThreads, smem, s>>>(pl, level, r, n, bp); break;
+    case 10: k_split_tma<RB, 10><<<grid, kTmaSplitThreads, smem, s>>>(pl, level, r, n, bp); break;
+    case 13: k_split_tma<RB, 13><<<grid, kTmaSplitThreads, smem, s>>>(pl, level, r, n, bp); break;
+    case 14: k_split_tma<RB, 14><<<grid, kTmaSplitThreads, smem, s>>>(pl, level, r, n, bp); break;
+    default: k_split_tma<RB, 0><<<grid, kTmaSplitThreads, smem, s>>>(pl, level, r, n, hb); break;
   }
 }
-int launch_split_l1(int rb, const void* recs, uint64_t n, const BinParams& bp, const SplitPlan& pl, cudaStream_t s) {
+int launch_split_l1(int rb, const void* recs, uint64_t n, const RangeBinParams& bp, const SplitPlan& pl, cudaStream_t s) {
   if (!n) return 0;
   DISPATCH_RB(rb, (launch_split_rb<RB>(dim3(2 * g_sm_count), pl, 1, recs, n, bp, s)));
   return 1;
 }
-int launch_split_l2(int rb, const BinParams& bp, const SplitPlan& pl, cudaStream_t s) {
+int launch_split_l2(int rb, const RangeBinParams& bp, const SplitPlan& pl, cudaStream_t s) {
   const int ctas = 2 * g_sm_count;
   const uint32_t regions = pl.C1_local;
   if (!regions) return 0;
@@ -1549,10 +1608,13 @@ int launch_checksum_in(int rb, const void* recs, uint64_t n, uint64_t* acc4, cud
                                                                            (unsigned long long*)acc4)));
   return 1;
 }
-int launch_checksum_out(int rb, const ShuffleBuffers& b, uint32_t B, const BinParams& bp, uint32_t bin_base,
+int launch_checksum_out(int rb, const ShuffleBuffers& b, uint32_t B, const RangeBinParams& bp, uint32_t bin_base,
                         uint64_t* acc6, cudaStream_t s) {
   int grid = g_sm_count * 8;
-  DISPATCH_RB(rb, (k_checksum_out<RB><<<grid, 256, 0, s>>>(b, B, bp, bin_base, (unsigned long long*)acc6)));
+  if (bp.partitioner == kPartRange)
+    DISPATCH_RB(rb, (k_checksum_out<RB, RangeBinParams><<<grid, 256, 0, s>>>(b, B, bp, bin_base, (unsigned long long*)acc6)))
+  else
+    DISPATCH_RB(rb, (k_checksum_out<RB><<<grid, 256, 0, s>>>(b, B, (const BinParams&)bp, bin_base, (unsigned long long*)acc6)))
   return 1;
 }
 

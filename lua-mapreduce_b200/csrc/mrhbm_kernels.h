@@ -25,6 +25,18 @@ struct BinParams {
   uint32_t wshift;       // log2(world) when world is a power of two, else 0xffffffff
   uint32_t pbase[9];
 };
+// MRHBM_PART_RANGE: the kernel instances compiled for it take this larger block (the hash instances keep BinParams, so
+// their parameter layout and code do not change).  The spl_n finite thresholds t_i, ascending, with
+// key >= splitter i  <=>  slot(key) >= t_i as big-endian numbers (see install_splitters in mrhbm_api.cu).
+struct RangeBinParams : BinParams {
+  const unsigned long long* spl_pre;  // [spl_n] the first 8 bytes of t_i, big endian (u64 keys: the splitter itself)
+  const uint32_t* spl_slot;           // [spl_n * key words] t_i as a zero-padded key slot (strings only)
+  const ulonglong2* spl_inv;          // [P] u64 keys: floor((2^128 - 1) / width of partition p) as {high, low} 64
+                                      // bits, 0 when the partition is empty (see range_pos)
+  uint32_t spl_n;                     // finite thresholds (splitters above every slot key are left out)
+  uint32_t spl_top;                   // largest power of two <= spl_n (0 when spl_n = 0)
+};
+constexpr uint32_t kPartRange = 3;  // MRHBM_PART_RANGE
 
 MRHBM_HD inline uint32_t partition_slot(const BinParams& bp, uint32_t pid) {
   return bp.world > 1 ? bp.pbase[pid % bp.world] + pid / bp.world : pid;
@@ -87,7 +99,7 @@ enum { ERRF_SKEW = 1, ERRF_OVERFLOW = 2, ERRF_CAPACITY = 4, ERRF_KEYLEN = 8 };
 int launch_gen_u64(void* dst, uint64_t seed, uint64_t start, uint64_t n, cudaStream_t s);
 int launch_gen_zipf32(void* dst, uint64_t seed, uint64_t start, uint64_t n, const uint64_t* d_table,
                       uint64_t V, cudaStream_t s);
-int launch_hist(int rb, const void* recs, uint64_t n, const BinParams& bp, uint32_t* hist, cudaStream_t s);
+int launch_hist(int rb, const void* recs, uint64_t n, const RangeBinParams& bp, uint32_t* hist, cudaStream_t s);
 // exclusive scan of in[i << shift], i < n: out_excl[n+1]; optional copies: out_copy[i << shift] (scatter
 // cursors), out_dense[i] (the counts, densely packed), entries > cap appended to big_list
 // scratch: kScanScratchWords words for the multi-CTA variant (nullptr: single CTA)
@@ -97,7 +109,12 @@ int launch_exscan(const uint32_t* in, uint32_t n, uint32_t* out_excl, uint32_t* 
                   uint32_t shift, cudaStream_t s, uint32_t* scratch = nullptr);
 // histogram of the top 8 key bits of `nsample` evenly spaced u64 records (hist256 += counts)
 int launch_sample_u64(const void* recs, uint64_t n, uint32_t nsample, uint32_t* hist256, cudaStream_t s);
-int launch_scatter(int rb, const void* recs, uint64_t n, const BinParams& bp, uint32_t* cursor, void* mid,
+// MRHBM_PART_RANGE, u64 keys: the same sample, histogram of the top 8 bits of each key's position inside its partition
+int launch_sample_range_u64(const void* recs, uint64_t n, uint32_t nsample, const RangeBinParams& bp, uint32_t* hist256,
+                            cudaStream_t s);
+// key slots (kKeyWords words each) of `nsample` evenly spaced records to out (splitter sampling)
+int launch_sample_keys(int rb, const void* recs, uint64_t n, uint32_t nsample, uint32_t* out, cudaStream_t s);
+int launch_scatter(int rb, const void* recs, uint64_t n, const RangeBinParams& bp, uint32_t* cursor, void* mid,
                    cudaStream_t s);
 // device-side tokeniser: word starts per 256-byte block, then (after an exclusive scan of the
 // block counts) one record per word; *flags gets ERRF_KEYLEN when a word exceeds the key slot
@@ -170,15 +187,15 @@ struct SplitPlan {
   uint32_t ctr_shift;         // spacing of the fill levels above (BinParams::ctr_shift)
   uint32_t* ticket;          // two zeroed words: level 1 hands out its tiles from a counter (the kernel zeroes them again)
 };
-int launch_split_l1(int rb, const void* recs, uint64_t n, const BinParams& bp, const SplitPlan& pl, cudaStream_t s);
-int launch_split_l2(int rb, const BinParams& bp, const SplitPlan& pl, cudaStream_t s);
+int launch_split_l1(int rb, const void* recs, uint64_t n, const RangeBinParams& bp, const SplitPlan& pl, cudaStream_t s);
+int launch_split_l2(int rb, const RangeBinParams& bp, const SplitPlan& pl, cudaStream_t s);
 int launch_sort_reduce(int rb, const ShuffleBuffers& b, uint32_t B, uint32_t cap, int sm_count,
                        cudaStream_t s);
 int launch_big_bins(int rb, const ShuffleBuffers& b, uint32_t nbig, uint32_t cap, cudaStream_t s);
 int launch_compact(int rb, const ShuffleBuffers& b, uint32_t B, void* dst_keys, uint64_t* dst_sums,
                    cudaStream_t s);
 int launch_checksum_in(int rb, const void* recs, uint64_t n, uint64_t* acc4, cudaStream_t s);
-int launch_checksum_out(int rb, const ShuffleBuffers& b, uint32_t B, const BinParams& bp, uint32_t bin_base,
+int launch_checksum_out(int rb, const ShuffleBuffers& b, uint32_t B, const RangeBinParams& bp, uint32_t bin_base,
                         uint64_t* acc6, cudaStream_t s);
 cudaError_t kernels_configure();  // opt-in shared memory sizes; call once per device
 

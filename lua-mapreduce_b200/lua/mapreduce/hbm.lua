@@ -13,9 +13,26 @@ local hbm = { _VERSION = "0.1", _NAME = "mapreduce.hbm" }
 -- what the device evaluates is declared on the plugin tables, like the reducer algebra flags
 -- (examples/WordCount/reducefn.lua:10-14):
 --   partitionfn module: hbm_partitionfn = "fnv_lua" | "wordhash" | "mulhash", NUM_REDUCERS = n
+--     or a key range: hbm_partitionfn = "range", hbm_splitters = { s_1, ..., s_{n-1} } (non-decreasing strings; u64
+--     keys as their 8 big-endian bytes; partition k takes the keys k splitters are <= to) or hbm_splitters = "sample"
+--     (quantiles of the map output, taken at the MAP -> REDUCE barrier).  The partitionfn must compute the same ranges.
 --   reducefn / combinerfn module: hbm_reducefn = "sum"
 local ctx -- one context per worker process (job.lua keeps `funcs`/`initialized` per process too)
+local sample_splitters = false -- hbm_splitters = "sample": hbm.prepare_reduce samples them before the shuffle
 local tuple_keys = false -- hbm.configure(..., { key_kind = "tuple" }); an upvalue of configure, map_job and groups
+
+-- the 8-byte big-endian string of a u64 key minus one; nil for key 0
+local function be_minus_one(s)
+  local b = { s:byte(1, #s) }
+  local i = #b
+  while i >= 1 and b[i] == 0 do
+    b[i] = 255
+    i = i - 1
+  end
+  if i < 1 then return nil end
+  b[i] = b[i] - 1
+  return string.char(table.unpack(b))
+end
 
 function hbm.configure(partition_mod, reduce_mod, combiner_mod, opts)
   -- hbm_reducefn = "sum": reduced on the device.  No declaration: general reducer -- the device
@@ -35,6 +52,35 @@ function hbm.configure(partition_mod, reduce_mod, combiner_mod, opts)
     device = opts.device,
   }
   ctx = assert(c, err)
+  sample_splitters = false
+  if partition_mod.hbm_partitionfn == "range" then
+    local spl = partition_mod.hbm_splitters
+    if spl == "sample" then
+      sample_splitters = true
+    else
+      assert(type(spl) == "table", "hbm_partitionfn = 'range' needs hbm_splitters = {...} or 'sample'")
+      assert(#spl + 1 == partition_mod.NUM_REDUCERS, "NUM_REDUCERS must equal the number of splitters + 1")
+      local u64 = opts.key_kind == "u64" -- u64 keys: 8-byte big-endian strings
+      for i = 1, #spl do
+        assert(not u64 or #spl[i] == 8, "u64 splitters are 8-byte big-endian strings")
+        assert(i == 1 or not (spl[i] < spl[i - 1]), "hbm_splitters must be non-decreasing")
+      end
+      -- the declaration must describe the same key ranges as partitionfn: the key of splitter i goes above every
+      -- splitter equal to it (bisect_right), and for u64 keys the key just below it goes below them
+      for i = 1, #spl do
+        local j = i
+        while spl[j + 1] == spl[i] do j = j + 1 end
+        assert(partition_mod.partitionfn(spl[i]) == j, "partitionfn disagrees with hbm_splitters at " .. spl[i])
+        local below = u64 and be_minus_one(spl[i])
+        if below then
+          local k = i - 1
+          while k >= 1 and not (spl[k] <= below) do k = k - 1 end
+          assert(partition_mod.partitionfn(below) == k, "partitionfn disagrees with hbm_splitters just below " .. spl[i])
+        end
+      end
+      assert(ctx:set_splitters(table.unpack(spl)))
+    end
+  end
   return ctx
 end
 
@@ -182,6 +228,7 @@ end
 
 -- server_prepare_reduce (server.lua:279-329)
 function hbm.prepare_reduce()
+  if sample_splitters then assert(ctx:sample_splitters()) end
   assert(ctx:shuffle())
   return assert(ctx:partitions())
 end

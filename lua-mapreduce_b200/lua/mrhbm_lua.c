@@ -22,7 +22,7 @@
 #define MAP_MT "mrhbm.map"
 #define ITER_MT "mrhbm.iter"
 
-typedef struct { mrhbm_ctx *h; } lctx;
+typedef struct { mrhbm_ctx *h; uint32_t nparts; } lctx;
 typedef struct { mrhbm_map *h; mrhbm_ctx *ctx; } lmap;
 typedef struct { mrhbm_iter *h; } liter;
 
@@ -33,7 +33,7 @@ static int fail(lua_State *L, mrhbm_ctx *c) { /* luamongo style: nil, msg */
 }
 
 /* mrhbm.new{ key_kind="str"|"u64", max_key_bytes=, num_partitions=, partitioner="fnv_lua"|"mulhash"|
- *            "wordhash", combiner=bool, reducer="sum"|"none", device= } */
+ *            "wordhash"|"range", combiner=bool, reducer="sum"|"none", device= } */
 static int l_new(lua_State *L) {
   mrhbm_config cfg;
   const char *s;
@@ -50,7 +50,8 @@ static int l_new(lua_State *L) {
   lua_getfield(L, 1, "partitioner");
   s = luaL_optstring(L, -1, cfg.key_kind == MRHBM_KEY_U64 ? "mulhash" : "fnv_lua");
   cfg.partitioner = strcmp(s, "fnv_lua") == 0 ? MRHBM_PART_FNV_LUA
-                  : strcmp(s, "mulhash") == 0 ? MRHBM_PART_MULHASH : MRHBM_PART_WORDHASH;
+                  : strcmp(s, "mulhash") == 0 ? MRHBM_PART_MULHASH
+                  : strcmp(s, "range") == 0 ? MRHBM_PART_RANGE : MRHBM_PART_WORDHASH;
   lua_getfield(L, 1, "combiner");
   cfg.combiner = lua_toboolean(L, -1);
   lua_getfield(L, 1, "device");
@@ -61,6 +62,7 @@ static int l_new(lua_State *L) {
   lua_pop(L, 7);
   lctx *u = (lctx *)lua_newuserdata(L, sizeof *u);
   u->h = NULL;
+  u->nparts = cfg.num_partitions;
   luaL_setmetatable(L, CTX_MT);
   if (mrhbm_init(&cfg, &u->h) != MRHBM_OK) {
     lua_pushnil(L);
@@ -182,6 +184,45 @@ static int ctx_partitions(lua_State *L) { /* server.lua:300-324: one reduce job 
   }
   return 1;
 }
+/* ctx:set_splitters(s_0, s_1, ..., s_{P-2}) -> true  (range partitioner: the splitters as strings, u64 keys as
+ * their 8 big-endian bytes; mapreduce/hbm.lua passes a table's elements with table.unpack) */
+static int ctx_set_splitters(lua_State *L) {
+  lctx *u = checkctx(L);
+  size_t n = 0, total = 0, len, i;
+  while (lua_type(L, (int)n + 2) > 0) { /* LUA_TNONE = -1 past the last argument, LUA_TNIL = 0 */
+    luaL_checklstring(L, (int)n + 2, &len);
+    total += len;
+    n++;
+  }
+  char *keys = (char *)lua_newuserdata(L, total ? total : 1);
+  uint64_t *off = (uint64_t *)lua_newuserdata(L, (n + 1) * sizeof(uint64_t));
+  off[0] = 0;
+  for (i = 0; i < n; i++) {
+    const char *k = luaL_checklstring(L, (int)i + 2, &len);
+    memcpy(keys + off[i], k, len);
+    off[i + 1] = off[i] + len;
+  }
+  if (mrhbm_set_splitters(u->h, keys, off, n) != MRHBM_OK) return fail(L, u->h);
+  lua_pushboolean(L, 1);
+  return 1;
+}
+/* ctx:sample_splitters() -> { s_0, ..., s_{P-2} }  (range partitioner: quantiles of a sample of the committed pairs,
+ * installed; collective on several GPUs) */
+static int ctx_sample_splitters(lua_State *L) {
+  lctx *u = checkctx(L);
+  size_t need = 0, n = u->nparts ? u->nparts - 1 : 0, i;
+  uint32_t rb = u->h ? mrhbm_record_bytes(u->h) : 16;
+  size_t cap = n * (rb == 16 ? 8 : rb - 4) + 1; /* a splitter takes at most one key slot: one call, no sizing call */
+  uint64_t *off = (uint64_t *)lua_newuserdata(L, (n + 1) * sizeof(uint64_t));
+  char *keys = (char *)lua_newuserdata(L, cap);
+  if (mrhbm_sample_splitters(u->h, keys, cap, off, &need) != MRHBM_OK) return fail(L, u->h);
+  lua_createtable(L, (int)n, 0);
+  for (i = 0; i < n; i++) {
+    lua_pushlstring(L, keys + off[i], (size_t)(off[i + 1] - off[i]));
+    lua_rawseti(L, -2, (int)i + 1);
+  }
+  return 1;
+}
 /* ctx:groups(partition) -> iterator yielding key, values  (utils.merge_iterator's consumer,
  * job.lua:264-284; also finalfn's pair iterator, server.lua:360-385) */
 static int iter_next(lua_State *L) {
@@ -223,7 +264,8 @@ static int ctx_groups(lua_State *L) {
 
 static const luaL_Reg ctx_methods[] = {{"map_begin", ctx_map_begin}, {"shuffle", ctx_shuffle},
                                        {"partitions", ctx_partitions}, {"groups", ctx_groups},
-                                       {"reset", ctx_reset}, {"__gc", ctx_gc}, {NULL, NULL}};
+                                       {"reset", ctx_reset}, {"set_splitters", ctx_set_splitters},
+                                       {"sample_splitters", ctx_sample_splitters}, {"__gc", ctx_gc}, {NULL, NULL}};
 static const luaL_Reg map_methods[] = {{"emit", map_emit}, {"wordcount", map_wordcount}, {"commit", map_commit},
                                        {"abort", map_abort}, {"__gc", map_abort}, {NULL, NULL}};
 static const luaL_Reg mod_funcs[] = {{"new", l_new}, {NULL, NULL}};

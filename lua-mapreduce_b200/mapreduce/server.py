@@ -2,6 +2,7 @@
 server_prepare_map (249-276), server_prepare_reduce (279-329), server_final (348-413).
 The MongoDB task/job collections are an in-process board; GridFS spill files are the HBM
 shuffle (storage "hbm").  Jobs run on attached workers or, when none is attached, inline."""
+import bisect
 import importlib
 import sys
 import time
@@ -10,7 +11,32 @@ from . import task as _task
 from .job import Job, get_func
 from .utils import STATUS, TASK_STATUS, get_storage_from, count_digits
 
-_BUILTIN_PART = {"fnv_lua": 0, "mulhash": 1, "wordhash": 2}
+_BUILTIN_PART = {"fnv_lua": 0, "mulhash": 1, "wordhash": 2, "range": 3}
+
+
+def range_splitters(part, nparts, key_kind):
+    """The splitters a partitionfn module declares with hbm_partitionfn = "range": hbm_splitters = [...] (checked
+    against the module's own partitionfn, since the declaration must mean what the function computes) or "sample"
+    (the splitters are sampled from the map output at the MAP -> REDUCE barrier).  Returns the list as the ctx takes
+    it (bytes, or ints for u64 keys) or "sample"."""
+    spl = getattr(part, "hbm_splitters", None)
+    if spl == "sample":
+        return "sample"
+    if not isinstance(spl, (list, tuple)):
+        raise ValueError("hbm_partitionfn = 'range' needs hbm_splitters = [...] or hbm_splitters = 'sample'")
+    if nparts != len(spl) + 1:
+        raise ValueError("NUM_REDUCERS (%d) must equal the number of splitters + 1 (%d)" % (nparts, len(spl) + 1))
+    u64 = key_kind == "u64"
+    norm = [int(x) if u64 else (x.encode() if isinstance(x, str) else bytes(x)) for x in spl]
+    if norm != sorted(norm):
+        raise ValueError("hbm_splitters must be non-decreasing")
+    for x in norm:
+        for k in ([x, x - 1] if u64 and x > 0 else [x]):
+            want, got = bisect.bisect_right(norm, k), part.partitionfn(k)
+            if got != want:
+                raise ValueError("partitionfn(%r) = %r, but the declared hbm_splitters put the key in partition %d: "
+                                 "the declaration must describe the same key ranges as partitionfn" % (k, got, want))
+    return norm
 
 
 class server:
@@ -66,6 +92,8 @@ class server:
             sys.stderr.write("# WARNING: combinerfn %s is not a device built-in (hbm_reducefn = 'sum'); it is skipped, "
                              "the reducefn sees the uncombined values\n" % params["combinerfn"])
         pname = getattr(part, "hbm_partitionfn", None)
+        # a partitionfn runs on the device when it is one of the hash built-ins or a key range ("range" with
+        # hbm_splitters)
         if pname not in _BUILTIN_PART:
             raise NotImplementedError("partitionfn module must declare hbm_partitionfn in %s" % sorted(_BUILTIN_PART))
         nparts = getattr(part, "NUM_REDUCERS", None) or getattr(part, "hbm_num_partitions", None)
@@ -73,7 +101,8 @@ class server:
         hbm = dict(key_kind="str", max_key_bytes=123, device=-1)
         hbm.update(params.get("hbm") or {})
         hbm.update(partitioner=_BUILTIN_PART[pname], num_partitions=nparts, combiner=device_combiner,
-                   reducer=0 if builtin_red == "sum" else 1)
+                   reducer=0 if builtin_red == "sum" else 1,
+                   splitters=range_splitters(part, nparts, hbm["key_kind"]) if pname == "range" else None)
         self.config = dict(mapfn=params["mapfn"], reducefn=params["reducefn"], partitionfn=params["partitionfn"],
                            combinerfn=params.get("combinerfn"), init_args=self.init_args,
                            storage=params["storage"], hbm=hbm)
@@ -85,8 +114,11 @@ class server:
             return self.ctx_factory(h)
         from .. import mrhbm
         kind = mrhbm.KEY_U64 if h["key_kind"] == "u64" else mrhbm.KEY_STR
-        return mrhbm.Ctx(kind, h["num_partitions"], h["partitioner"], max_key_bytes=h["max_key_bytes"],
-                         combiner=h["combiner"], device=h["device"], reducer=h["reducer"])
+        ctx = mrhbm.Ctx(kind, h["num_partitions"], h["partitioner"], max_key_bytes=h["max_key_bytes"],
+                        combiner=h["combiner"], device=h["device"], reducer=h["reducer"])
+        if isinstance(h.get("splitters"), list):  # (kept across reset)
+            ctx.set_splitters(h["splitters"])
+        return ctx
 
     # ---- polling (server.lua:186-234) with inline execution when no worker is attached
     def _wait(self, ns):
@@ -139,6 +171,8 @@ class server:
             sys.stderr.write("# Iteration %d\n# \t Preparing MAP\n" % it)
             failed_maps = self._wait("map_jobs")
             # server_prepare_reduce (server.lua:279-329): one reduce job per NON-EMPTY partition
+            if self.config["hbm"].get("splitters") == "sample":  # key ranges from this iteration's map output
+                b.ctx.sample_splitters()
             b.ctx.shuffle()
             parts = b.ctx.partitions()
             digits = count_digits(max(parts) if parts else 0)

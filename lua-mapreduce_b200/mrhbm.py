@@ -11,7 +11,7 @@ import numpy as np
 from . import build as _build
 
 KEY_U64, KEY_STR = 0, 1
-PART_FNV_LUA, PART_MULHASH, PART_WORDHASH = 0, 1, 2
+PART_FNV_LUA, PART_MULHASH, PART_WORDHASH, PART_RANGE = 0, 1, 2, 3
 RED_SUM, RED_NONE = 0, 1
 F_FORCE_RUNS, F_SMALL_BINS, F_NO_OPTIMISTIC = 1, 2, 4
 E_NODEVICE = -8
@@ -56,6 +56,7 @@ EXPORTS = [
     "mrhbm_map_abort", "mrhbm_shuffle", "mrhbm_partitions", "mrhbm_groups_open", "mrhbm_groups_next",
     "mrhbm_groups_close", "mrhbm_result_info_get", "mrhbm_result_copy", "mrhbm_checksum_input",
     "mrhbm_checksum_result", "mrhbm_stats_get", "mrhbm_reset", "mrhbm_comm_unique_id", "mrhbm_comm_init",
+    "mrhbm_set_splitters", "mrhbm_sample_splitters",
 ]
 
 _lib = None
@@ -115,6 +116,8 @@ def load(build_if_missing=True):
     sig("mrhbm_reset", i, vp)
     sig("mrhbm_comm_unique_id", i, vp, vp)
     sig("mrhbm_comm_init", i, vp, vp, i, i)
+    sig("mrhbm_set_splitters", i, vp, vp, C.POINTER(u64), sz)
+    sig("mrhbm_sample_splitters", i, vp, vp, sz, C.POINTER(u64), C.POINTER(sz))
     _lib = L
     return L
 
@@ -134,6 +137,15 @@ def synth_zipf_text(seed, first, n, table, words_per_line=25, out=None, threads=
     if rc != 0:
         raise MrhbmError(rc, "synth_zipf_text: the text needs %d bytes, the buffer holds %d" % (need.value, out.nbytes))
     return out[:need.value]
+
+
+def splitter_bytes(key_kind, x):
+    """A splitter in the C form: the original key bytes (u64 keys: 8 big-endian bytes)."""
+    if key_kind == KEY_U64:
+        if isinstance(x, (bytes, bytearray)):
+            return bytes(x)
+        return int(x).to_bytes(8, "big")
+    return x.encode() if isinstance(x, str) else bytes(x)
 
 
 def record_dtype(key_kind, max_key_bytes=27):
@@ -337,6 +349,34 @@ class Ctx:
         s = Stats()
         self._chk(self.L.mrhbm_stats_get(self.h, C.byref(s)))
         return s.asdict()
+
+    # -- range partitioner
+    def set_splitters(self, splitters):
+        """PART_RANGE: installs the num_partitions - 1 non-decreasing splitters (bytes / str for string keys, ints for
+        u64 keys); partition k then holds the keys k splitters are <= to (bisect_right)."""
+        raw = [splitter_bytes(self.key_kind, x) for x in splitters]
+        keys = b"".join(raw)
+        off = (C.c_uint64 * (len(raw) + 1))()
+        o = 0
+        for i, r in enumerate(raw):
+            off[i] = o
+            o += len(r)
+        off[len(raw)] = o
+        buf = C.create_string_buffer(keys, max(1, len(keys)))
+        self._chk(self.L.mrhbm_set_splitters(self.h, buf, off, len(raw)))
+
+    def sample_splitters(self):
+        """PART_RANGE: quantile splitters from a sample of the committed pairs (collective on several GPUs); installs
+        and returns them (bytes for string keys, ints for u64 keys)."""
+        n = self.num_partitions - 1
+        off = (C.c_uint64 * (n + 1))()
+        need = C.c_size_t()
+        slot = 8 if self.key_kind == KEY_U64 else self.record_bytes - 4  # a splitter takes at most one key slot
+        buf = C.create_string_buffer(max(1, n * slot))
+        self._chk(self.L.mrhbm_sample_splitters(self.h, buf, max(1, n * slot), off, C.byref(need)))
+        raw = buf.raw
+        out = [raw[off[i]:off[i + 1]] for i in range(n)]
+        return [int.from_bytes(x, "big") for x in out] if self.key_kind == KEY_U64 else out
 
     # -- multi-GPU
     def comm_unique_id(self):
