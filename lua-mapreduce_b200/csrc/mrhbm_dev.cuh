@@ -48,7 +48,7 @@ template <int RB>
 __device__ __forceinline__ uint64_t key_prefix64(const uint32_t* r) {
   return ((uint64_t)be_word<RB>(r, 0) << 32) | be_word<RB>(r, 1);
 }
-// nbits (<=51) of the key starting `bitpos` bits below the most significant bit
+// nbits (1..64; the LSD passes take kDigitBits = 52) of the key starting `bitpos` bits below the most significant bit
 template <int RB>
 __device__ __forceinline__ uint64_t key_bits(const uint32_t* r, int bitpos, int nbits) {
   int wi = bitpos >> 5, sh = bitpos & 31;
