@@ -17,7 +17,8 @@
 #include "../../include/mrhbm.h"
 #include "mrhbm_comm.h"
 #include "mrhbm_kernels.h"
-#include "mrhbm_dev.cuh"  // fnv_lua_step, mulhi_u64_u32: the host side partitions the keys that do not fit a slot
+#include "mrhbm_dev.cuh"  // splitmix64
+#include "mrhbm_keys.h"
 
 using namespace mrhbm;
 
@@ -150,7 +151,7 @@ struct RunCursor {
 struct mrhbm_iter {
   mrhbm_ctx* ctx;
   std::vector<uint64_t> valbuf;  // group-only mode: the values of the current key
-  std::vector<unsigned char> unesc;  // the current key with its 0x00 / 0x01 bytes restored
+  std::vector<unsigned char> unesc;  // the current key's original bytes (reserved: not null even for the empty key)
   std::vector<unsigned char> keys;
   std::vector<uint64_t> sums;
   std::vector<RunCursor> runs;
@@ -158,7 +159,6 @@ struct mrhbm_iter {
   uint64_t base = 0;
   const std::vector<LongGroup>* longs = nullptr;  // the partition's long-key groups and the next one to hand out
   size_t long_pos = 0;
-  unsigned char keybuf[8];
   bool sorted = true;
   size_t cur_run = 0;
 };
@@ -373,35 +373,6 @@ float ev_ms(mrhbm_ctx* c, int a, int b) {
   return ms;
 }
 
-// Key slots are zero padded, so a key byte 0x00 cannot be stored as such.  Bytes 0x00 and 0x01 travel escaped --
-// 0x00 -> 01 01, 0x01 -> 01 02 -- which keeps the bytewise order of the keys ("a" < "a\0" < "a\1" < "ab", SURVEY A.3)
-// and is the identity for text.  Record slots and the host-side store of long keys hold keys in this form; the
-// device partitioner hashes the unescaped bytes, the iterator unescapes.
-// escape: the escaped form of key[0..n) to dst (room for n + the number of bytes <= 1), returns its length
-size_t escape(const unsigned char* key, size_t n, unsigned char* dst) {
-  size_t o = 0;
-  for (size_t i = 0; i < n; i++) {
-    if (key[i] <= 1) {
-      dst[o++] = 1;
-      dst[o++] = (unsigned char)(key[i] + 1);
-    } else {
-      dst[o++] = key[i];
-    }
-  }
-  return o;
-}
-// unescape: out = the original bytes of the escaped key esc[0..n)
-void unescape(const void* esc, size_t n, std::vector<unsigned char>& out) {
-  const unsigned char* e = (const unsigned char*)esc;
-  out.clear();
-  for (size_t i = 0; i < n; i++) {
-    if (e[i] == 1 && i + 1 < n)
-      out.push_back((unsigned char)(e[++i] - 1));
-    else
-      out.push_back(e[i]);
-  }
-}
-
 int install_splitters(mrhbm_ctx* c, std::vector<std::string>&& spl);  // (with the shuffle, below)
 
 }  // namespace
@@ -552,8 +523,7 @@ int mrhbm_emit_str(mrhbm_map* m, const void* key, size_t klen, uint32_t value) {
   if (c->cfg.key_kind != MRHBM_KEY_STR) return fail(c, MRHBM_E_INVAL, "ctx holds u64 keys");
   // (keys are stored escaped, see escape)
   const unsigned char* k = (const unsigned char*)key;
-  size_t elen = klen;
-  for (size_t i = 0; i < klen; i++) elen += k[i] <= 1;
+  const size_t elen = esc_size(k, klen);
   if (elen >= (size_t)c->kb) {  // longer than a record slot: kept on the host (escaped like a slot would hold it)
     if (klen > kMaxLongKey) return fail(c, MRHBM_E_KEY, "key of %zu bytes (limit %zu)", klen, (size_t)kMaxLongKey);
     LongPair lp;
@@ -1695,47 +1665,8 @@ inline int64_t slot_of(const mrhbm_ctx* c, uint32_t p) {
 }  // namespace
 
 namespace {
-// ---- keys longer than a record slot: partitioned, exchanged and grouped on the host --------------------------
-// the partition bin_of (mrhbm_dev.cuh) would give the key if it fitted a slot: FNV-in-doubles over the ORIGINAL bytes
-// (examples/WordCount/partitionfn.lua:8-16), or the word hash over the little-endian words of the STORED bytes
-// (range partitioner: the original bytes against the original splitters, bisect_right)
-uint32_t host_partition(const mrhbm_ctx* c, const std::string& esc) {
-  const uint32_t P = c->cfg.num_partitions;
-  if (c->cfg.partitioner == MRHBM_PART_RANGE) {
-    std::vector<unsigned char> raw;
-    unescape(esc.data(), esc.size(), raw);
-    const std::string key(raw.begin(), raw.end());
-    return (uint32_t)(std::upper_bound(c->spl.begin(), c->spl.end(), key) - c->spl.begin());
-  }
-  if (c->cfg.partitioner == MRHBM_PART_FNV_LUA) {
-    std::vector<unsigned char> raw;
-    unescape(esc.data(), esc.size(), raw);
-    uint32_t h = 2166136261u;
-    for (unsigned char b : raw) h = fnv_lua_step(h, b);
-    return h % P;
-  }
-  uint64_t h = 0x9E3779B97F4A7C15ull;
-  for (size_t i = 0; i < esc.size(); i += 4) {
-    uint32_t w = 0;
-    memcpy(&w, esc.data() + i, std::min<size_t>(4, esc.size() - i));
-    h = (h ^ w) * 0xBF58476D1CE4E5B9ull;
-    h ^= h >> 29;
-  }
-  h ^= h >> 32;
-  h *= 0x94D049BB133111EBull;
-  return mulhi_u64_u32(h, P);
-}
-
 // ---- the range partitioner's splitters ------------------------------------------------------------------------
-// Checks the splitters (original bytes) and installs them with their device form (RangeBinParams):
-//   threshold t_i = the escaped splitter zero padded to the key slot, when it fits; else its first slot bytes plus one
-//   as a big-endian number: a key that fits a slot is >= a longer splitter iff its slot is STRICTLY greater than the
-//   splitter's first slot bytes (on equality the key is a proper prefix of it).  Then key >= s_i <=> slot >= t_i for
-//   every key a slot holds.  A threshold that would pass all ones lies above every slot key: it and the (equal or
-//   larger) splitters after it are left out of the device search (spl_n = the finite ones).
-//   u64 keys: t_i = the splitter; inv[p] = floor((2^128 - 1) / width_p) of partition p = [s_{p-1}, s_p) (s_{-1} = 0,
-//   s_{P-1} = 2^64) as {high, low} words, 0 for an empty partition: range_pos (mrhbm_dev.cuh) turns it into the key's
-//   position inside its partition as a 64-bit fraction.
+// Checks the splitters (original bytes) and installs them with their device form (range_table, mrhbm_keys.h)
 int install_splitters(mrhbm_ctx* c, std::vector<std::string>&& spl) {
   const uint32_t P = c->cfg.num_partitions;
   if (spl.size() != (size_t)P - 1)
@@ -1745,52 +1676,12 @@ int install_splitters(mrhbm_ctx* c, std::vector<std::string>&& spl) {
     if (u64 && spl[i].size() != 8) return fail(c, MRHBM_E_INVAL, "u64 splitter %zu has %zu bytes (8 big-endian bytes)", i, spl[i].size());
     if (i && spl[i] < spl[i - 1]) return fail(c, MRHBM_E_INVAL, "splitters must be non-decreasing (splitter %zu < splitter %zu)", i, i - 1);
   }
-  const size_t n = spl.size(), kb = (size_t)c->kb;
-  std::vector<unsigned long long> pre(n), inv(2 * (size_t)P);
-  std::vector<unsigned char> slot(u64 ? 0 : n * kb);
-  uint32_t fin = 0;
-  if (u64) {
-    for (size_t i = 0; i < n; i++) {
-      uint64_t v = 0;
-      for (int b = 0; b < 8; b++) v = (v << 8) | (unsigned char)spl[i][b];
-      pre[i] = v;
-    }
-    fin = (uint32_t)n;
-    for (uint32_t p = 0; p < P; p++) {
-      const unsigned __int128 lo = p ? pre[p - 1] : 0, hi = p < n ? (unsigned __int128)pre[p] : (unsigned __int128)1 << 64;
-      const unsigned __int128 w = hi - lo, f = w ? ~(unsigned __int128)0 / w : 0;
-      inv[2 * p] = (unsigned long long)(f >> 64);
-      inv[2 * p + 1] = (unsigned long long)f;
-    }
-  } else {
-    std::vector<unsigned char> esc;
-    for (size_t i = 0; i < n; i++) {
-      esc.resize(2 * spl[i].size());
-      esc.resize(escape((const unsigned char*)spl[i].data(), spl[i].size(), esc.data()));
-      unsigned char* t = slot.data() + i * kb;
-      memcpy(t, esc.data(), std::min(esc.size(), kb));
-      if (esc.size() > kb) {  // + 1 in the last slot byte, carried
-        size_t j = kb;
-        while (j > 0 && t[j - 1] == 0xff) t[--j] = 0;
-        if (j == 0) break;  // above every slot key, and so is every later splitter
-        t[j - 1]++;
-      }
-      uint64_t v = 0;
-      for (int b = 0; b < 8; b++) v = (v << 8) | t[b];
-      pre[i] = v;
-      fin = (uint32_t)i + 1;
-    }
-  }
-  const size_t bytes = 8 * (2 * (size_t)P + n) + slot.size();
+  const RangeTable rt = range_table(spl, P, (size_t)c->kb);  // (never empty: P >= 1)
   if (c->d_spl) CU(c, cudaFree(c->d_spl));
   c->d_spl = nullptr;
   c->spl_set = false;
-  CU(c, cudaMalloc(&c->d_spl, std::max<size_t>(bytes, 8)));
-  std::vector<unsigned char> host(bytes);
-  memcpy(host.data(), inv.data(), 16 * (size_t)P);
-  if (n) memcpy(host.data() + 16 * (size_t)P, pre.data(), 8 * n);
-  if (!slot.empty()) memcpy(host.data() + 16 * (size_t)P + 8 * n, slot.data(), slot.size());
-  CU(c, cudaMemcpyAsync(c->d_spl, host.data(), bytes, cudaMemcpyHostToDevice, c->stream));
+  CU(c, cudaMalloc(&c->d_spl, rt.image.size()));
+  CU(c, cudaMemcpyAsync(c->d_spl, rt.image.data(), rt.image.size(), cudaMemcpyHostToDevice, c->stream));
   CU(c, cudaStreamSynchronize(c->stream));
   // digest (FNV-1a over the lengths and bytes): compared across ranks by the shuffle
   uint64_t d = 0xcbf29ce484222325ull;
@@ -1800,7 +1691,7 @@ int install_splitters(mrhbm_ctx* c, std::vector<std::string>&& spl) {
     for (unsigned char x : sp) mixb(x);
   }
   c->spl = std::move(spl);
-  c->spl_fin = fin;
+  c->spl_fin = rt.fin;
   c->spl_digest = d == ~0ull ? 0 : d;  // (all ones marks "none installed")
   c->spl_set = true;
   return MRHBM_OK;
@@ -1871,7 +1762,7 @@ int build_long_groups(mrhbm_ctx* c) {
     memcpy(&v, &all_blobs[w + 1], 8);
     std::string esc((const char*)&all_blobs[w + 3], klen);
     w += 3 + (klen + 3) / 4;
-    const uint32_t pid = host_partition(c, esc);
+    const uint32_t pid = host_partition(c->cfg.partitioner, c->cfg.num_partitions, c->spl, esc);
     if ((int)(pid % (uint32_t)G) != c->rank) continue;
     const uint32_t slot = pid / (uint32_t)G;
     if (slot >= c->Pl) continue;
@@ -1987,31 +1878,18 @@ int mrhbm_sample_splitters(mrhbm_ctx* c, void* keys, size_t cap, uint64_t* off, 
     cudaGetLastError();
     return fail(c, MRHBM_E_CUDA, "splitter sample: %s", cudaGetErrorString(e));
   }
-  // the sample in key order: u64 numerically, strings bytewise over the (order preserving) escaped slot
-  std::vector<const uint32_t*> smp;
+  // the sample in key order
+  std::vector<const unsigned char*> smp;
   smp.reserve(mtot);
   for (int r = 0; r < G; r++)
-    for (uint64_t i = 0; i < m[r]; i++) smp.push_back(h.data() + (size_t)r * words + i * KW);
-  const bool u64 = c->cfg.key_kind == MRHBM_KEY_U64;
-  auto key64 = [](const uint32_t* w) { return (uint64_t)w[0] | ((uint64_t)w[1] << 32); };
-  std::sort(smp.begin(), smp.end(), [&](const uint32_t* a, const uint32_t* b) {
-    return u64 ? key64(a) < key64(b) : memcmp(a, b, (size_t)KW * 4) < 0;
-  });
+    for (uint64_t i = 0; i < m[r]; i++) smp.push_back((const unsigned char*)(h.data() + (size_t)r * words + i * KW));
+  const size_t kb = (size_t)c->kb;
+  std::sort(smp.begin(), smp.end(), [kb](const unsigned char* a, const unsigned char* b) { return slot_cmp(a, b, kb) < 0; });
   std::vector<std::string> spl(P - 1);
   std::vector<unsigned char> raw;
   for (uint32_t i = 1; i < P; i++) {
-    const uint32_t* w = smp[(size_t)(((unsigned __int128)i * mtot) / P)];
-    if (u64) {
-      const uint64_t v = key64(w);
-      spl[i - 1].resize(8);
-      for (int b = 0; b < 8; b++) spl[i - 1][b] = (char)(v >> (56 - 8 * b));
-    } else {
-      const unsigned char* k = (const unsigned char*)w;
-      size_t len = 0;
-      while (len < (size_t)KW * 4 && k[len]) len++;
-      unescape(k, len, raw);
-      spl[i - 1].assign(raw.begin(), raw.end());
-    }
+    slot_key(smp[(size_t)(((unsigned __int128)i * mtot) / P)], kb, raw);
+    spl[i - 1].assign(raw.begin(), raw.end());
   }
   size_t total = 0;
   for (auto& sp : spl) total += sp.size();
@@ -2118,21 +1996,11 @@ int mrhbm_checksum_result(mrhbm_ctx* c, uint64_t out[6]) {
 // ---------------------------------------------------------------------------
 // reduce side iteration
 // ---------------------------------------------------------------------------
-static inline int slot_cmp(const mrhbm_ctx* c, const unsigned char* a, const unsigned char* b) {
-  if (c->rb == 16) {
-    uint64_t x, y;
-    memcpy(&x, a, 8);
-    memcpy(&y, b, 8);
-    return (x > y) - (x < y);
-  }
-  return memcmp(a, b, c->kb);
-}
-
 // k-way merge of the partition's ascending runs (utils.lua:206-271 merges spill files the same way): a binary heap of
 // run indices ordered by the key each run stands on (ties: lower run first)
 static inline bool run_less(const mrhbm_iter* it, uint32_t a, uint32_t b) {
   const mrhbm_ctx* c = it->ctx;
-  const int x = slot_cmp(c, &it->keys[it->runs[a].pos * c->kb], &it->keys[it->runs[b].pos * c->kb]);
+  const int x = slot_cmp(&it->keys[it->runs[a].pos * c->kb], &it->keys[it->runs[b].pos * c->kb], c->kb);
   return x < 0 || (x == 0 && a < b);
 }
 static inline void heap_sift_down(mrhbm_iter* it, size_t i) {
@@ -2168,6 +2036,7 @@ int mrhbm_groups_open(mrhbm_ctx* c, uint32_t part, mrhbm_iter** out) {
   if (slot < 0) return fail(c, MRHBM_E_INVAL, "partition %u is owned by rank %u", part, part % (uint32_t)c->world);
   mrhbm_iter* it = new mrhbm_iter();
   it->ctx = c;
+  it->unesc.reserve(c->kb);
   uint64_t b0 = (uint64_t)slot * c->S;
   uint64_t lo = c->h_uoff[b0], hi = c->h_uoff[b0 + c->S];
   it->base = lo;
@@ -2212,15 +2081,12 @@ int mrhbm_groups_next(mrhbm_iter* it, const void** key, size_t* klen, const uint
   // k-way merge over the ascending runs of the partition (a single run when sorted): the smallest key is on top
   const int best = it->heap.empty() ? -1 : (int)it->heap[0];
   if (it->longs && it->long_pos < it->longs->size()) {
-    // a key longer than a slot comes next when it sorts before the smallest device key: both are compared as the
-    // escaped byte strings a slot holds (the device key ends at its zero padding; a proper prefix sorts first)
+    // a key longer than a slot comes next when it sorts before the smallest device key
     const LongGroup& lg = (*it->longs)[it->long_pos];
     bool take = best < 0;
     if (!take) {
       const unsigned char* dk = &it->keys[it->runs[best].pos * c->kb];
-      const size_t dl = strnlen((const char*)dk, c->kb);
-      const int cmp = memcmp(lg.esc.data(), dk, std::min(dl, lg.esc.size()));
-      take = cmp < 0 || (cmp == 0 && lg.esc.size() < dl);
+      take = esc_cmp((const unsigned char*)lg.esc.data(), lg.esc.size(), dk, slot_esc_len(dk, c->kb)) < 0;
     }
     if (take) {
       it->long_pos++;
@@ -2244,31 +2110,20 @@ int mrhbm_groups_next(mrhbm_iter* it, const void** key, size_t* klen, const uint
     it->valbuf.push_back(it->sums[i]);
     for (;;) {  // the run on top, then whichever run comes to the top with the same key
       RunCursor& rc = it->runs[it->heap[0]];
-      while (rc.pos < rc.end && slot_cmp(c, &it->keys[rc.pos * c->kb], k) == 0) it->valbuf.push_back(it->sums[rc.pos++]);
+      while (rc.pos < rc.end && slot_cmp(&it->keys[rc.pos * c->kb], k, c->kb) == 0) it->valbuf.push_back(it->sums[rc.pos++]);
       heap_fix_top(it);
       if (it->heap.empty()) break;
       const RunCursor& top = it->runs[it->heap[0]];
-      if (slot_cmp(c, &it->keys[top.pos * c->kb], k) != 0) break;
+      if (slot_cmp(&it->keys[top.pos * c->kb], k, c->kb) != 0) break;
     }
     nv = it->valbuf.size();
     gathered = true;
   } else {
     heap_fix_top(it);
   }
-  if (c->rb == 16) {
-    for (int b = 0; b < 8; b++) it->keybuf[b] = k[7 - b];  // 8-byte big-endian string (SURVEY A.4)
-    *key = it->keybuf;
-    *klen = 8;
-  } else {
-    size_t len = strnlen((const char*)k, c->kb);
-    if (memchr(k, 1, len)) {  // escaped 0x00 / 0x01 bytes
-      unescape(k, len, it->unesc);
-      k = it->unesc.data();
-      len = it->unesc.size();
-    }
-    *key = k;
-    *klen = len;
-  }
+  slot_key(k, c->kb, it->unesc);
+  *key = it->unesc.data();
+  *klen = it->unesc.size();
   *values = gathered ? it->valbuf.data() : &it->sums[i];
   *nvalues = nv;
   return 1;

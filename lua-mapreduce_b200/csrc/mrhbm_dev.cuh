@@ -149,10 +149,20 @@ __device__ __forceinline__ uint32_t fnv_lua_hash(const uint32_t* r) {
   return h;
 }
 // 64-bit word hash over the little-endian u32 words of the key bytes while non-zero
-// (length-exact for NUL-free keys, independent of the slot width)
+// (length-exact for NUL-free keys, independent of the slot width): kWordHashSeed, word_hash_step per word, then
+// word_hash_finish.  The host partitions keys longer than a slot with the same steps (mrhbm_keys.h).
+constexpr uint64_t kWordHashSeed = 0x9E3779B97F4A7C15ull;
+__host__ __device__ __forceinline__ uint64_t word_hash_step(uint64_t h, uint32_t w) {
+  h = (h ^ w) * 0xBF58476D1CE4E5B9ull;
+  return h ^ (h >> 29);
+}
+__host__ __device__ __forceinline__ uint64_t word_hash_finish(uint64_t h) {
+  h ^= h >> 32;
+  return h * 0x94D049BB133111EBull;
+}
 template <int RB>
 __device__ __forceinline__ uint64_t word_hash(const uint32_t* r) {
-  uint64_t h = 0x9E3779B97F4A7C15ull;
+  uint64_t h = kWordHashSeed;
 #pragma unroll
   for (int i = 0; i < Rec<RB>::kKeyWords; i++) {
     uint32_t w;
@@ -161,12 +171,9 @@ __device__ __forceinline__ uint64_t word_hash(const uint32_t* r) {
     else
       w = r[i];
     if (w == 0) break;  // short keys leave early
-    h = (h ^ w) * 0xBF58476D1CE4E5B9ull;
-    h ^= h >> 29;
+    h = word_hash_step(h, w);
   }
-  h ^= h >> 32;
-  h *= 0x94D049BB133111EBull;
-  return h;
+  return word_hash_finish(h);
 }
 
 // floor(x * m / 2^64) for a 32-bit m: two 32x32 multiplies instead of the four of __umul64hi

@@ -27,7 +27,7 @@ struct BinParams {
 };
 // MRHBM_PART_RANGE: the kernel instances compiled for it take this larger block (the hash instances keep BinParams, so
 // their parameter layout and code do not change).  The spl_n finite thresholds t_i, ascending, with
-// key >= splitter i  <=>  slot(key) >= t_i as big-endian numbers (see install_splitters in mrhbm_api.cu).
+// key >= splitter i  <=>  slot(key) >= t_i as big-endian numbers (see range_table in mrhbm_keys.h).
 struct RangeBinParams : BinParams {
   const unsigned long long* spl_pre;  // [spl_n] the first 8 bytes of t_i, big endian (u64 keys: the splitter itself)
   const uint32_t* spl_slot;           // [spl_n * key words] t_i as a zero-padded key slot (strings only)
