@@ -93,6 +93,18 @@ typedef struct mrhbm_config {
 #define MRHBM_F_FORCE_RUNS 1u   /* always use hash sub-bins (skip the key-ordered attempt) */
 #define MRHBM_F_SMALL_BINS 2u   /* test hook: tiny smem bins to exercise the overflow paths */
 #define MRHBM_F_NO_OPTIMISTIC 4u /* always run the exact two-pass (histogram) partition layout */
+/* Byte-string values (lua-mapreduce's emit(key, value) takes any Lua string or number, utils.lua:100-120): a value is
+ * opaque bytes, 0 to 1 GiB long, carried through group-only mode.  Needs reducer = MRHBM_RED_NONE and combiner = 0
+ * (else mrhbm_init fails with MRHBM_E_INVAL) and one GPU (mrhbm_comm_init with world > 1 fails).  On such a ctx:
+ *   - pairs are emitted with mrhbm_emit_str_value / mrhbm_emit_u64_value / mrhbm_emit_batch_values; the integer-valued
+ *     emits (emit_str, emit_u64, emit_batch, emit_device, map_gen_*, map_wordcount) fail with MRHBM_E_INVAL;
+ *   - groups are read with mrhbm_groups_next_values (mrhbm_groups_next fails) and rows with mrhbm_result_values;
+ *     mrhbm_result_copy needs sums = NULL;
+ *   - the value field of a record (pool_read, result_copy) holds the pair's value id, its index in the emit pool;
+ *     fewer than 2^32 pairs may be emitted between mrhbm_reset calls, those of aborted and replaced jobs included.
+ * The order of a key's values is unspecified, as for MRHBM_RED_NONE.  The new calls fail with MRHBM_E_INVAL on a ctx
+ * without the flag. */
+#define MRHBM_F_BYTE_VALUES 8u
 
 /* record layouts (little endian) moved by emit_batch / gen / result_copy:
  *   U64 : { uint64_t key; uint64_t value; }                             16 B
@@ -154,6 +166,14 @@ int mrhbm_pool_read(mrhbm_ctx *, uint64_t first, uint64_t n, void *host_out);
 int mrhbm_map_commit(mrhbm_map *);
 /* BROKEN job: nothing becomes visible (worker.lua:120-127).  Consumes the handle. */
 void mrhbm_map_abort(mrhbm_map *);
+/* MRHBM_F_BYTE_VALUES: one pair with the value bytes val[0 .. vlen) (copied before return; vlen <= 1 GiB, 0 allowed).
+ * Keys follow mrhbm_emit_str / mrhbm_emit_u64, long string keys included. */
+int mrhbm_emit_str_value(mrhbm_map *, const void *key, size_t klen, const void *val, size_t vlen);
+int mrhbm_emit_u64_value(mrhbm_map *, uint64_t key, const void *val, size_t vlen);
+/* MRHBM_F_BYTE_VALUES, bulk: n records in the ctx layout (their value field is ignored) and the value of record i at
+ * vals[voff[i] .. voff[i+1]) (voff has n + 1 non-decreasing entries).  Pinned and pageable memory as for
+ * mrhbm_emit_batch: all three buffers are pinned-or-pageable independently. */
+int mrhbm_emit_batch_values(mrhbm_map *, const void *records, size_t n, const void *vals, const uint64_t *voff);
 
 /* ---- barrier between MAP and REDUCE (server.lua:279-329) ---- */
 /* hash-partition [+ NCCL all-to-all] + sort + segmented reduce of everything committed */
@@ -183,6 +203,10 @@ int mrhbm_groups_open(mrhbm_ctx *, uint32_t partition, mrhbm_iter **out);
  * until the next call on this iterator. */
 int mrhbm_groups_next(mrhbm_iter *, const void **key, size_t *klen, const uint64_t **values,
                       size_t *nvalues);
+/* MRHBM_F_BYTE_VALUES: the next group as mrhbm_groups_next gives it (same key order, long keys merged in, same pointer
+ * lifetime), with its nvalues values packed in *vals: value i is (*vals)[(*voff)[i] .. (*voff)[i+1]). */
+int mrhbm_groups_next_values(mrhbm_iter *, const void **key, size_t *klen, const void **vals, const uint64_t **voff,
+                             size_t *nvalues);
 void mrhbm_groups_close(mrhbm_iter *);
 
 /* ---- bulk result access (finalfn feed without per-group calls) ---- */
@@ -205,6 +229,10 @@ int mrhbm_result_info_get(mrhbm_ctx *, mrhbm_result_info *);
  * Inside a partition the order is ascending iff info.sorted, else run-major.
  * MRHBM_E_KEY when the result holds keys longer than a slot (see mrhbm_emit_str): iterate instead. */
 int mrhbm_result_copy(mrhbm_ctx *, void *keys, uint64_t *sums, uint64_t *part_off);
+/* MRHBM_F_BYTE_VALUES: the value bytes of this rank's rows in mrhbm_result_copy row order; row r's value is
+ * vals[row_off[r] .. row_off[r+1]) (row_off: groups + 1 entries).  *need receives the bytes; vals = NULL only sizes
+ * (row_off is then not written); MRHBM_E_INVAL when cap < *need.  MRHBM_E_KEY as for mrhbm_result_copy. */
+int mrhbm_result_values(mrhbm_ctx *, void *vals, size_t cap, uint64_t *row_off, size_t *need);
 /* size-independent parity properties computed on the device:
  *  in[0..3]  = { sum f1(key)*v, sum f2(key)*v, sum v, pairs }       over committed pairs
  *  out[0..3] = { sum f1(key)*s, sum f2(key)*s, sum s, groups }      over reduced groups

@@ -29,6 +29,7 @@ constexpr size_t kMaxLongKey = 1u << 20;  // bytes; longer keys are refused (MRH
 struct LongPair {
   std::string esc;  // the key as a record slot would hold it: 0x00 / 0x01 escaped (order preserving, see escape)
   uint64_t value;
+  std::string bytes;  // MRHBM_F_BYTE_VALUES: the value
 };
 struct LongGroup {
   std::string esc;
@@ -40,8 +41,11 @@ struct Range {
   std::string job;
   int state;
   uint64_t owner;  // map handle serial
+  uint64_t aoff;   // MRHBM_F_BYTE_VALUES: the arena offset of the range's first value (its bytes follow in pool order)
 };
 constexpr size_t kStageRecs = 1 << 16;
+constexpr size_t kStageValBytes = 4u << 20;       // value bytes staged next to the records; a longer value goes alone
+constexpr uint64_t kMaxValue = 1ull << 30;        // bytes; longer values are refused (MRHBM_E_INVAL)
 enum { EV_START, EV_CSTART, EV_COMBINE, EV_HIST, EV_PLAN, EV_GATH, EV_SCATTER, EV_EXCH, EV_SORT, EV_BIG, EV_END, EV_PROBE, EV_N };
 constexpr uint32_t kSampleKeys = 1u << 18;      // keys sampled to decide between key-ordered and hash sub-bins
 }  // namespace
@@ -55,6 +59,18 @@ struct mrhbm_ctx {
   uint64_t pool_cap = 0, pool_used = 0;
   std::vector<Range> ranges;
   uint64_t map_serial = 0;
+  // MRHBM_F_BYTE_VALUES: a pair's value field holds its pool index (value id); value id i has the bytes
+  // arena[voff[i] .. voff[i+1]).  Values are appended in pool order, so voff[pool_used] == arena_used always; abort
+  // takes back the arena with the pool, dead ranges keep their bytes until mrhbm_reset.
+  bool bytevals = false;
+  unsigned char* arena = nullptr;
+  uint64_t arena_cap = 0, arena_used = 0;
+  uint64_t* voff = nullptr;  // pool_cap + 1 entries
+  // after the compaction: row r's value at cvals[row_off[r] .. row_off[r+1])
+  unsigned char* cvals = nullptr;
+  uint64_t *row_off = nullptr, *val_tile = nullptr, *val_pieces = nullptr;
+  uint64_t cvals_cap = 0, row_cap = 0, tile_cap = 0, pieces_cap = 0, cvals_bytes = 0;
+  std::vector<const std::string*> long_vals;  // values of the long-key groups (LongGroup::values index them)
   // Keys that do not fit a record slot (rare: the reference takes any key length, utils.lua:104-110) never reach the
   // device: their pairs wait on the host, per committed map job, are partitioned and grouped at the barrier (on several
   // GPUs after an all-gather) and merged into the reduce-side iteration at their place in the key order.
@@ -143,6 +159,10 @@ struct mrhbm_map {
   int cur = 0;
   size_t fill = 0;
   bool async_reads = false;  // pinned user memory still being read by the copy engine
+  // MRHBM_F_BYTE_VALUES: the staged records' value bytes and their offsets (fill + 1 of them), pinned, double
+  // buffered with the record stage
+  unsigned char* vstage[2] = {nullptr, nullptr};
+  uint64_t* vrel[2] = {nullptr, nullptr};
 };
 
 struct RunCursor {
@@ -161,6 +181,13 @@ struct mrhbm_iter {
   size_t long_pos = 0;
   bool sorted = true;
   size_t cur_run = 0;
+  std::vector<uint64_t> rows;  // the rows of the current key (indices into keys / sums)
+  // MRHBM_F_BYTE_VALUES: the partition's row offsets (rows + 1, relative to its first) and value bytes, and the
+  // current group's values packed
+  std::vector<uint64_t> roff;
+  std::vector<unsigned char> vbytes;
+  std::vector<unsigned char> vout;
+  std::vector<uint64_t> vout_off;
 };
 
 namespace {
@@ -202,16 +229,26 @@ struct Entry {
   }
 };
 
+// a device buffer of `want` elements of `elem` bytes that keeps its first `keep` elements
+int regrow(mrhbm_ctx* c, void** p, uint64_t want, uint64_t keep, size_t elem) {
+  void* np = nullptr;
+  CU(c, cudaMalloc(&np, want * elem));
+  if (keep) CU(c, cudaMemcpyAsync(np, *p, keep * elem, cudaMemcpyDeviceToDevice, c->stream));
+  CU(c, cudaStreamSynchronize(c->stream));
+  if (*p) CU(c, cudaFree(*p));
+  *p = np;
+  return 0;
+}
+
 int pool_reserve(mrhbm_ctx* c, uint64_t n, uint64_t* off) {
+  if (c->bytevals && c->pool_used + n >= 0xffffffffull)  // (value ids are u32 in string records)
+    return fail(c, MRHBM_E_INVAL, "byte values: 2^32 pairs emitted since the last reset");
   if (c->pool_used + n > c->pool_cap) {
     uint64_t want = std::max<uint64_t>(c->pool_used + n, c->pool_cap * 2);
     want = std::max<uint64_t>(want, 1 << 16);
-    void* np = nullptr;
-    CU(c, cudaMalloc(&np, want * c->rb));
-    if (c->pool_used) CU(c, cudaMemcpyAsync(np, c->pool, c->pool_used * c->rb, cudaMemcpyDeviceToDevice, c->stream));
-    CU(c, cudaStreamSynchronize(c->stream));
-    if (c->pool) CU(c, cudaFree(c->pool));
-    c->pool = np;
+    int rc = regrow(c, &c->pool, want, c->pool_used, (size_t)c->rb);
+    if (!rc && c->bytevals) rc = regrow(c, (void**)&c->voff, want + 1, c->voff ? c->pool_used + 1 : 0, sizeof(uint64_t));
+    if (rc) return rc;
     c->pool_cap = want;
   }
   *off = c->pool_used;
@@ -219,7 +256,23 @@ int pool_reserve(mrhbm_ctx* c, uint64_t n, uint64_t* off) {
   return 0;
 }
 
-void add_range(mrhbm_map* m, uint64_t off, uint64_t cnt) {
+// MRHBM_F_BYTE_VALUES: room for `bytes` value bytes at the end of the arena, *aoff the first.  Called right after the
+// pool_reserve of the pairs they belong to (values follow pool order).
+int arena_reserve(mrhbm_ctx* c, uint64_t bytes, uint64_t* aoff) {
+  if (c->arena_used + bytes > c->arena_cap) {
+    uint64_t want = std::max<uint64_t>(c->arena_used + bytes, c->arena_cap * 2);
+    want = std::max<uint64_t>(want, 1 << 20);
+    int rc = regrow(c, (void**)&c->arena, want, c->arena_used, 1);
+    if (rc) return rc;
+    c->arena_cap = want;
+  }
+  *aoff = c->arena_used;
+  c->arena_used += bytes;
+  return 0;
+}
+
+// aoff: the arena offset of the first pair's value (byte values; else 0)
+void add_range(mrhbm_map* m, uint64_t off, uint64_t cnt, uint64_t aoff = 0) {
   mrhbm_ctx* c = m->ctx;
   if (!c->ranges.empty()) {
     Range& r = c->ranges.back();
@@ -228,19 +281,41 @@ void add_range(mrhbm_map* m, uint64_t off, uint64_t cnt) {
       return;
     }
   }
-  c->ranges.push_back(Range{off, cnt, m->job, R_OPEN, m->serial});
+  c->ranges.push_back(Range{off, cnt, m->job, R_OPEN, m->serial, aoff});
 }
 
 int stage_flush(mrhbm_map* m) {
   mrhbm_ctx* c = m->ctx;
   if (!m->fill) return 0;
-  uint64_t off;
+  uint64_t off, aoff = 0;
   int rc = pool_reserve(c, m->fill, &off);
   if (rc) return rc;
+  if (c->bytevals) {
+    // the staged records get their value ids, the staged offsets become arena offsets
+    const uint64_t bytes = m->vrel[m->cur][m->fill];
+    rc = arena_reserve(c, bytes, &aoff);
+    if (rc) {
+      c->pool_used = off;
+      return rc;
+    }
+    unsigned char* st = m->stage[m->cur];
+    for (size_t i = 0; i < m->fill; i++) {
+      if (c->rb == 16) {
+        const uint64_t id = off + i;
+        memcpy(st + i * 16 + 8, &id, 8);
+      } else {
+        const uint32_t id = (uint32_t)(off + i);
+        memcpy(st + i * c->rb + c->kb, &id, 4);
+      }
+    }
+    for (size_t i = 0; i <= m->fill; i++) m->vrel[m->cur][i] += aoff;
+    if (bytes) CU(c, cudaMemcpyAsync(c->arena + aoff, m->vstage[m->cur], bytes, cudaMemcpyHostToDevice, c->stream));
+    CU(c, cudaMemcpyAsync(c->voff + off, m->vrel[m->cur], (m->fill + 1) * 8, cudaMemcpyHostToDevice, c->stream));
+  }
   CU(c, cudaMemcpyAsync((char*)c->pool + off * c->rb, m->stage[m->cur], m->fill * c->rb, cudaMemcpyHostToDevice, c->stream));
   CU(c, cudaEventRecord(m->stage_ev[m->cur], c->stream));
   m->stage_busy[m->cur] = true;
-  add_range(m, off, m->fill);
+  add_range(m, off, m->fill, aoff);
   m->fill = 0;
   m->cur ^= 1;
   if (m->stage_busy[m->cur]) {
@@ -256,6 +331,10 @@ int stage_slot(mrhbm_map* m, unsigned char** slot) {
     for (int i = 0; i < 2; i++) {
       CU(c, cudaHostAlloc((void**)&m->stage[i], kStageRecs * c->rb, cudaHostAllocDefault));
       CU(c, cudaEventCreateWithFlags(&m->stage_ev[i], cudaEventDisableTiming));
+      if (c->bytevals) {
+        CU(c, cudaHostAlloc((void**)&m->vstage[i], kStageValBytes, cudaHostAllocDefault));
+        CU(c, cudaHostAlloc((void**)&m->vrel[i], (kStageRecs + 1) * sizeof(uint64_t), cudaHostAllocDefault));
+      }
     }
   }
   if (m->fill == kStageRecs) {
@@ -265,6 +344,61 @@ int stage_slot(mrhbm_map* m, unsigned char** slot) {
   *slot = m->stage[m->cur] + m->fill * c->rb;
   m->fill++;
   return 0;
+}
+
+// MRHBM_F_BYTE_VALUES: one pair, its key written into the record slot by key_to_slot, its value staged next to it.  A
+// value larger than the value stage goes to the device on its own, behind what is staged.
+template <class F>
+int stage_value_pair(mrhbm_map* m, const void* val, size_t vlen, F key_to_slot) {
+  mrhbm_ctx* c = m->ctx;
+  if (vlen > kMaxValue) return fail(c, MRHBM_E_INVAL, "value of %zu bytes (limit %llu)", vlen, (unsigned long long)kMaxValue);
+  if (vlen && !val) return fail(c, MRHBM_E_INVAL, "null value");
+  if (vlen > kStageValBytes) {
+    int rc = stage_flush(m);
+    uint64_t off = 0, aoff = 0;
+    if (!rc) rc = pool_reserve(c, 1, &off);
+    if (rc) return rc;
+    rc = arena_reserve(c, vlen, &aoff);
+    if (rc) {
+      c->pool_used = off;
+      return rc;
+    }
+    unsigned char rec[128];
+    key_to_slot(rec);
+    if (c->rb == 16)
+      memcpy(rec + 8, &off, 8);
+    else {
+      const uint32_t id = (uint32_t)off;
+      memcpy(rec + c->kb, &id, 4);
+    }
+    const uint64_t vo[2] = {aoff, aoff + vlen};
+    CU(c, cudaMemcpyAsync(c->arena + aoff, val, vlen, cudaMemcpyHostToDevice, c->stream));
+    CU(c, cudaMemcpyAsync(c->voff + off, vo, sizeof vo, cudaMemcpyHostToDevice, c->stream));
+    CU(c, cudaMemcpyAsync((char*)c->pool + off * c->rb, rec, c->rb, cudaMemcpyHostToDevice, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));  // (the caller's value may be pinned memory: copied before return)
+    add_range(m, off, 1, aoff);
+    return MRHBM_OK;
+  }
+  if (m->stage[0] && m->fill && m->vrel[m->cur][m->fill] + vlen > kStageValBytes) {
+    int rc = stage_flush(m);
+    if (rc) return rc;
+  }
+  unsigned char* slot;
+  int rc = stage_slot(m, &slot);
+  if (rc) return rc;
+  const size_t i = m->fill - 1;
+  if (i == 0) m->vrel[m->cur][0] = 0;
+  key_to_slot(slot);
+  if (vlen) memcpy(m->vstage[m->cur] + m->vrel[m->cur][i], val, vlen);
+  m->vrel[m->cur][i + 1] = m->vrel[m->cur][i] + vlen;
+  return MRHBM_OK;
+}
+
+int refuse_int_values(mrhbm_ctx* c) {
+  return fail(c, MRHBM_E_INVAL, "the ctx carries byte values (MRHBM_F_BYTE_VALUES): use the *_value calls");
+}
+int refuse_byte_values(mrhbm_ctx* c) {
+  return fail(c, MRHBM_E_INVAL, "byte values need a ctx with MRHBM_F_BYTE_VALUES");
 }
 
 // room for n records of the map's output straight in the pool, behind what it has staged (emission order): *off is
@@ -279,6 +413,8 @@ void map_release(mrhbm_map* m) {
     if (m->stage_busy[i]) cudaEventSynchronize(m->stage_ev[i]);
     if (m->stage_ev[i]) cudaEventDestroy(m->stage_ev[i]);
     if (m->stage[i]) cudaFreeHost(m->stage[i]);
+    if (m->vstage[i]) cudaFreeHost(m->vstage[i]);
+    if (m->vrel[i]) cudaFreeHost(m->vrel[i]);
   }
   delete m;
 }
@@ -288,6 +424,7 @@ void invalidate(mrhbm_ctx* c) {
   c->compacted = false;
   c->long_groups.clear();
   c->long_group_count = 0;
+  c->long_vals.clear();
 }
 
 struct DevBuf {
@@ -359,6 +496,26 @@ int ensure_compact(mrhbm_ctx* c) {
   if (rc) return rc;
   launch_compact(c->rb, c->rv, c->B, c->ckeys, c->csums, c->stream);
   CU(c, cudaGetLastError());
+  if (c->bytevals) {
+    // the value id of every row is in csums: lengths, their offsets, then the bytes in row order
+    const uint64_t n = c->groups, nt = val_tiles(n);
+    rc = grow(c, &c->row_cap, n + 1, n + 1, {{(void**)&c->row_off, sizeof(uint64_t)}});
+    if (!rc) rc = grow(c, &c->tile_cap, nt + 1, nt + 1, {{(void**)&c->val_tile, sizeof(uint64_t)}});
+    if (rc) return rc;
+    launch_value_scan(c->csums, n, c->voff, c->row_off, c->val_tile, c->stream);
+    CU(c, cudaGetLastError());
+    CU(c, cudaMemcpyAsync(c->h_acc, c->row_off + n, 8, cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+    const uint64_t total = c->h_acc[0];
+    rc = grow(c, &c->cvals_cap, total + 1, total + 1, {{(void**)&c->cvals, 1}});
+    if (!rc) rc = grow(c, &c->pieces_cap, val_chunks_cap(total) + 1, val_chunks_cap(total) + 1, {{(void**)&c->val_pieces, sizeof(uint64_t)}});
+    if (rc) return rc;
+    CU(c, cudaMemsetAsync(c->d_acc, 0, 8, c->stream));
+    launch_value_gather(c->csums, n, c->voff, c->arena, c->row_off, c->val_tile, c->cvals, c->val_pieces,
+                        (unsigned long long*)c->d_acc, c->stream);
+    CU(c, cudaGetLastError());
+    c->cvals_bytes = total;
+  }
   CU(c, cudaStreamSynchronize(c->stream));
   c->compacted = true;
   return 0;
@@ -423,6 +580,9 @@ int mrhbm_init(const mrhbm_config* cfg, mrhbm_ctx** out) {
     return fail(c, MRHBM_E_INVAL, "unknown key_kind %u", cfg->key_kind);
   if (cfg->reducer != MRHBM_RED_SUM && cfg->reducer != MRHBM_RED_NONE) return fail(c, MRHBM_E_INVAL, "unknown reducer %u", cfg->reducer);
   if (cfg->reducer == MRHBM_RED_NONE && cfg->combiner) return fail(c, MRHBM_E_INVAL, "a general reducer cannot be combined on the device (combiner must be 0)");
+  if ((cfg->flags & MRHBM_F_BYTE_VALUES) && (cfg->reducer != MRHBM_RED_NONE || cfg->combiner))
+    return fail(c, MRHBM_E_INVAL, "byte values (MRHBM_F_BYTE_VALUES) need reducer MRHBM_RED_NONE and combiner 0");
+  c->bytevals = (cfg->flags & MRHBM_F_BYTE_VALUES) != 0;
   c->sb.no_reduce = cfg->reducer == MRHBM_RED_NONE;
   CU(c, cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
   if (cfg->partitioner == MRHBM_PART_RANGE && cfg->num_partitions == 1) {  // one key range, no splitters: its table now
@@ -467,7 +627,8 @@ void mrhbm_destroy(mrhbm_ctx* c) {
                    c->csums,       c->d_acc,       c->d_table,    c->d_hd,        c->d_hall,    c->d_tot,
                    c->d_outoff,    c->d_segoff,    c->recvbuf,    c->bigbuf,      c->d_small,   c->comb,
                    c->gtab,        c->l1buf,       c->regions,    c->d_l1all,     c->d_sample,   c->d_tok_text[0],
-                   c->d_tok_text[1], c->d_tok_cnt, c->d_tok_off, c->d_spl};
+                   c->d_tok_text[1], c->d_tok_cnt, c->d_tok_off, c->d_spl,     c->arena,       c->voff,
+                   c->cvals,       c->row_off,     c->val_tile,   c->val_pieces};
   for (void* p : frees)
     if (p) cudaFree(p);
   if (c->h_counters) cudaFreeHost(c->h_counters);
@@ -521,6 +682,7 @@ int mrhbm_emit_str(mrhbm_map* m, const void* key, size_t klen, uint32_t value) {
   mrhbm_ctx* c = m->ctx;
   Entry g(c);
   if (c->cfg.key_kind != MRHBM_KEY_STR) return fail(c, MRHBM_E_INVAL, "ctx holds u64 keys");
+  if (c->bytevals) return refuse_int_values(c);
   // (keys are stored escaped, see escape)
   const unsigned char* k = (const unsigned char*)key;
   const size_t elen = esc_size(k, klen);
@@ -547,6 +709,7 @@ int mrhbm_emit_u64(mrhbm_map* m, uint64_t key, uint64_t value) {
   mrhbm_ctx* c = m->ctx;
   Entry g(c);
   if (c->cfg.key_kind != MRHBM_KEY_U64) return fail(c, MRHBM_E_INVAL, "ctx holds string keys");
+  if (c->bytevals) return refuse_int_values(c);
   unsigned char* slot;
   int rc = stage_slot(m, &slot);
   if (rc) return rc;
@@ -555,10 +718,82 @@ int mrhbm_emit_u64(mrhbm_map* m, uint64_t key, uint64_t value) {
   return MRHBM_OK;
 }
 
+int mrhbm_emit_str_value(mrhbm_map* m, const void* key, size_t klen, const void* val, size_t vlen) {
+  if (!m || (!key && klen)) return MRHBM_E_INVAL;
+  mrhbm_ctx* c = m->ctx;
+  Entry g(c);
+  if (!c->bytevals) return refuse_byte_values(c);
+  if (c->cfg.key_kind != MRHBM_KEY_STR) return fail(c, MRHBM_E_INVAL, "ctx holds u64 keys");
+  const unsigned char* k = (const unsigned char*)key;
+  const size_t elen = esc_size(k, klen);
+  if (elen >= (size_t)c->kb) {  // longer than a record slot: on the host with its value (see mrhbm_emit_str)
+    if (klen > kMaxLongKey) return fail(c, MRHBM_E_KEY, "key of %zu bytes (limit %zu)", klen, (size_t)kMaxLongKey);
+    if (vlen > kMaxValue) return fail(c, MRHBM_E_INVAL, "value of %zu bytes (limit %llu)", vlen, (unsigned long long)kMaxValue);
+    if (vlen && !val) return fail(c, MRHBM_E_INVAL, "null value");
+    LongPair lp;
+    lp.esc.resize(elen);
+    escape(k, klen, (unsigned char*)&lp.esc[0]);
+    lp.value = 0;
+    lp.bytes.assign((const char*)val, vlen);
+    m->long_pairs.push_back(std::move(lp));
+    return MRHBM_OK;
+  }
+  return stage_value_pair(m, val, vlen, [&](unsigned char* slot) {
+    escape(k, klen, slot);
+    memset(slot + elen, 0, c->kb - elen);
+  });
+}
+
+int mrhbm_emit_u64_value(mrhbm_map* m, uint64_t key, const void* val, size_t vlen) {
+  if (!m) return MRHBM_E_INVAL;
+  mrhbm_ctx* c = m->ctx;
+  Entry g(c);
+  if (!c->bytevals) return refuse_byte_values(c);
+  if (c->cfg.key_kind != MRHBM_KEY_U64) return fail(c, MRHBM_E_INVAL, "ctx holds string keys");
+  return stage_value_pair(m, val, vlen, [&](unsigned char* slot) { memcpy(slot, &key, 8); });
+}
+
+int mrhbm_emit_batch_values(mrhbm_map* m, const void* recs, size_t n, const void* vals, const uint64_t* voff) {
+  if (!m || (n && (!recs || !voff))) return MRHBM_E_INVAL;
+  mrhbm_ctx* c = m->ctx;
+  Entry g(c);
+  if (!c->bytevals) return refuse_byte_values(c);
+  if (!n) return MRHBM_OK;
+  for (size_t i = 0; i < n; i++)
+    if (voff[i + 1] < voff[i] || voff[i + 1] - voff[i] > kMaxValue)
+      return fail(c, MRHBM_E_INVAL, "value %zu: offsets %llu .. %llu (non-decreasing, at most %llu bytes apart)", i,
+                  (unsigned long long)voff[i], (unsigned long long)voff[i + 1], (unsigned long long)kMaxValue);
+  const uint64_t bytes = voff[n] - voff[0];
+  if (bytes && !vals) return fail(c, MRHBM_E_INVAL, "null values");
+  uint64_t off, aoff;
+  int rc = pool_take(m, n, &off);
+  if (rc) return rc;
+  rc = arena_reserve(c, bytes, &aoff);
+  if (rc) {
+    c->pool_used = off;
+    return rc;
+  }
+  bool pinned = false;
+  for (const void* p : {recs, vals, (const void*)voff}) {
+    cudaPointerAttributes at{};
+    if (p && cudaPointerGetAttributes(&at, p) == cudaSuccess && at.type == cudaMemoryTypeHost) pinned = true;
+    cudaGetLastError();
+  }
+  CU(c, cudaMemcpyAsync((char*)c->pool + off * c->rb, recs, n * c->rb, cudaMemcpyHostToDevice, c->stream));
+  if (bytes) CU(c, cudaMemcpyAsync(c->arena + aoff, (const char*)vals + voff[0], bytes, cudaMemcpyHostToDevice, c->stream));
+  CU(c, cudaMemcpyAsync(c->voff + off, voff, (n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, c->stream));
+  launch_value_stamp(c->rb, (char*)c->pool + off * c->rb, n, off, c->voff + off, voff[0], aoff, c->stream);
+  CU(c, cudaGetLastError());
+  if (pinned) m->async_reads = true;  // pageable sources are fully staged before the call returns
+  add_range(m, off, n, aoff);
+  return MRHBM_OK;
+}
+
 int mrhbm_emit_batch(mrhbm_map* m, const void* recs, size_t n) {
   if (!m || (!recs && n)) return MRHBM_E_INVAL;
   mrhbm_ctx* c = m->ctx;
   Entry g(c);
+  if (c->bytevals) return refuse_int_values(c);
   if (!n) return MRHBM_OK;
   uint64_t off;
   int rc = pool_take(m, n, &off);
@@ -576,6 +811,7 @@ int mrhbm_emit_device(mrhbm_map* m, const void* drecs, size_t n) {
   if (!m || (!drecs && n)) return MRHBM_E_INVAL;
   mrhbm_ctx* c = m->ctx;
   Entry g(c);
+  if (c->bytevals) return refuse_int_values(c);
   if (!n) return MRHBM_OK;
   uint64_t off;
   int rc = pool_take(m, n, &off);
@@ -590,6 +826,7 @@ int mrhbm_map_gen_u64(mrhbm_map* m, uint64_t seed, uint64_t start, uint64_t n) {
   mrhbm_ctx* c = m->ctx;
   Entry g(c);
   if (c->rb != 16) return fail(c, MRHBM_E_INVAL, "gen_u64 needs a u64-key ctx");
+  if (c->bytevals) return refuse_int_values(c);
   uint64_t off;
   int rc = pool_take(m, n, &off);
   if (rc) return rc;
@@ -605,6 +842,7 @@ int mrhbm_map_gen_zipf(mrhbm_map* m, uint64_t seed, uint64_t start, uint64_t n, 
   mrhbm_ctx* c = m->ctx;
   Entry g(c);
   if (c->rb != 32) return fail(c, MRHBM_E_INVAL, "gen_zipf needs 32-byte string records (max_key_bytes <= 27)");
+  if (c->bytevals) return refuse_int_values(c);
   if (!c->d_table || c->d_table_V != V || c->d_table_first != table[0] || c->d_table_last != table[V - 1]) {
     if (c->d_table) CU(c, cudaFree(c->d_table));
     c->d_table = nullptr;
@@ -630,6 +868,7 @@ int mrhbm_map_wordcount(mrhbm_map* m, const void* text, size_t len, uint64_t* wo
   Entry g(c);
   if (words) *words = 0;
   if (c->cfg.key_kind != MRHBM_KEY_STR) return fail(c, MRHBM_E_INVAL, "wordcount needs a string-key ctx");
+  if (c->bytevals) return refuse_int_values(c);
   if (!len) return MRHBM_OK;
   int rc = stage_flush(m);
   if (rc) return rc;
@@ -870,6 +1109,7 @@ void mrhbm_map_abort(mrhbm_map* m) {
   while (!c->ranges.empty() && c->ranges.back().state == R_DEAD &&
          c->ranges.back().off + c->ranges.back().cnt == c->pool_used) {
     c->pool_used = c->ranges.back().off;
+    if (c->bytevals) c->arena_used = c->ranges.back().aoff;
     c->ranges.pop_back();
   }
   map_release(m);
@@ -880,6 +1120,7 @@ int mrhbm_reset(mrhbm_ctx* c) {
   Entry g(c);
   c->ranges.clear();
   c->pool_used = 0;
+  c->arena_used = 0;
   c->long_jobs.clear();
   invalidate(c);
   return MRHBM_OK;
@@ -1700,15 +1941,22 @@ int install_splitters(mrhbm_ctx* c, std::vector<std::string>&& spl) {
 int build_long_groups(mrhbm_ctx* c) {
   c->long_groups.clear();
   c->long_group_count = 0;
+  c->long_vals.clear();
   const int G = c->world;
   // this rank's committed long pairs as one blob: {u32 key bytes, u64 value, key bytes padded to 4}*
+  // (byte values, one GPU only: the value travels as its index in long_vals)
   std::vector<uint32_t> blob;
   for (auto& job : c->long_jobs)
     for (const LongPair& lp : job.second) {
       const size_t w0 = blob.size(), kw = (lp.esc.size() + 3) / 4;
       blob.resize(w0 + 3 + kw, 0u);
       blob[w0] = (uint32_t)lp.esc.size();
-      memcpy(&blob[w0 + 1], &lp.value, 8);
+      uint64_t v = lp.value;
+      if (c->bytevals) {
+        v = c->long_vals.size();
+        c->long_vals.push_back(&lp.bytes);
+      }
+      memcpy(&blob[w0 + 1], &v, 8);
       memcpy(&blob[w0 + 3], lp.esc.data(), lp.esc.size());
     }
   std::vector<uint32_t> all_blobs;
@@ -1949,6 +2197,7 @@ int mrhbm_result_info_get(mrhbm_ctx* c, mrhbm_result_info* info) {
 int mrhbm_result_copy(mrhbm_ctx* c, void* keys, uint64_t* sums, uint64_t* part_off) {
   if (!c) return MRHBM_E_INVAL;
   Entry g(c);
+  if (c->bytevals && sums) return fail(c, MRHBM_E_INVAL, "byte values: result_copy takes sums = NULL (see mrhbm_result_values)");
   int rc = ensure_compact(c);
   if (rc) return rc;
   if (c->long_group_count)
@@ -1962,6 +2211,24 @@ int mrhbm_result_copy(mrhbm_ctx* c, void* keys, uint64_t* sums, uint64_t* part_o
       uint64_t slots = p <= (uint32_t)c->rank ? 0 : ((uint64_t)p - c->rank + c->world - 1) / c->world;
       part_off[p] = c->h_uoff[std::min<uint64_t>(slots, c->Pl) * c->S];
     }
+  CU(c, cudaStreamSynchronize(c->stream));
+  return MRHBM_OK;
+}
+
+int mrhbm_result_values(mrhbm_ctx* c, void* vals, size_t cap, uint64_t* row_off, size_t* need) {
+  if (!c || !need || (vals && !row_off)) return MRHBM_E_INVAL;
+  Entry g(c);
+  if (!c->bytevals) return refuse_byte_values(c);
+  int rc = ensure_compact(c);
+  if (rc) return rc;
+  if (c->long_group_count)
+    return fail(c, MRHBM_E_KEY, "%llu groups have keys longer than the %d-byte slots of mrhbm_result_copy: iterate with mrhbm_groups_*",
+                (unsigned long long)c->long_group_count, c->kb);
+  *need = (size_t)c->cvals_bytes;
+  if (!vals) return MRHBM_OK;
+  if (cap < c->cvals_bytes) return fail(c, MRHBM_E_INVAL, "the values need %llu bytes, the buffer holds %zu", (unsigned long long)c->cvals_bytes, cap);
+  if (c->cvals_bytes) CU(c, cudaMemcpyAsync(vals, c->cvals, c->cvals_bytes, cudaMemcpyDeviceToHost, c->stream));
+  CU(c, cudaMemcpyAsync(row_off, c->row_off, (c->groups + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream));
   CU(c, cudaStreamSynchronize(c->stream));
   return MRHBM_OK;
 }
@@ -2045,6 +2312,17 @@ int mrhbm_groups_open(mrhbm_ctx* c, uint32_t part, mrhbm_iter** out) {
   if (hi > lo) {
     cudaError_t e = cudaMemcpyAsync(it->keys.data(), (char*)c->ckeys + lo * c->kb, (hi - lo) * c->kb, cudaMemcpyDeviceToHost, c->stream);
     if (e == cudaSuccess) e = cudaMemcpyAsync(it->sums.data(), c->csums + lo, (hi - lo) * 8, cudaMemcpyDeviceToHost, c->stream);
+    if (e == cudaSuccess && c->bytevals) {  // the partition's row offsets, then its value bytes
+      it->roff.resize(hi - lo + 1);
+      e = cudaMemcpyAsync(it->roff.data(), c->row_off + lo, (hi - lo + 1) * 8, cudaMemcpyDeviceToHost, c->stream);
+      if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+      if (e == cudaSuccess) {
+        const uint64_t v0 = it->roff[0], nb = it->roff[hi - lo] - v0;
+        for (uint64_t& o : it->roff) o -= v0;
+        it->vbytes.resize(nb);
+        if (nb) e = cudaMemcpyAsync(it->vbytes.data(), c->cvals + v0, nb, cudaMemcpyDeviceToHost, c->stream);
+      }
+    }
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
     if (e != cudaSuccess) {
       delete it;
@@ -2075,57 +2353,100 @@ int mrhbm_groups_open(mrhbm_ctx* c, uint32_t part, mrhbm_iter** out) {
   return MRHBM_OK;
 }
 
-int mrhbm_groups_next(mrhbm_iter* it, const void** key, size_t* klen, const uint64_t** values, size_t* nvalues) {
-  if (!it || !key || !klen || !values || !nvalues) return MRHBM_E_INVAL;
+// The next group of the iteration into it->unesc (its original key bytes) and either *lg (a key longer than a slot)
+// or it->rows (its device rows).  1 = one group, 0 = end.
+static int next_group(mrhbm_iter* it, const LongGroup** lg) {
   mrhbm_ctx* c = it->ctx;
+  *lg = nullptr;
   // k-way merge over the ascending runs of the partition (a single run when sorted): the smallest key is on top
   const int best = it->heap.empty() ? -1 : (int)it->heap[0];
   if (it->longs && it->long_pos < it->longs->size()) {
     // a key longer than a slot comes next when it sorts before the smallest device key
-    const LongGroup& lg = (*it->longs)[it->long_pos];
+    const LongGroup& g = (*it->longs)[it->long_pos];
     bool take = best < 0;
     if (!take) {
       const unsigned char* dk = &it->keys[it->runs[best].pos * c->kb];
-      take = esc_cmp((const unsigned char*)lg.esc.data(), lg.esc.size(), dk, slot_esc_len(dk, c->kb)) < 0;
+      take = esc_cmp((const unsigned char*)g.esc.data(), g.esc.size(), dk, slot_esc_len(dk, c->kb)) < 0;
     }
     if (take) {
       it->long_pos++;
-      unescape(lg.esc.data(), lg.esc.size(), it->unesc);
-      *key = it->unesc.data();
-      *klen = it->unesc.size();
-      *values = lg.values.data();
-      *nvalues = lg.values.size();
+      unescape(g.esc.data(), g.esc.size(), it->unesc);
+      *lg = &g;
       return 1;
     }
   }
   if (best < 0) return 0;
   uint64_t i = it->runs[best].pos++;
   const unsigned char* k = &it->keys[i * c->kb];
-  size_t nv = 1;
-  bool gathered = false;
+  it->rows.clear();
+  it->rows.push_back(i);
   if (c->cfg.reducer == MRHBM_RED_NONE) {
     // every row of this key: adjacent in its run, and -- for an oversized bin -- at the head of
     // sibling runs too
-    it->valbuf.clear();
-    it->valbuf.push_back(it->sums[i]);
     for (;;) {  // the run on top, then whichever run comes to the top with the same key
       RunCursor& rc = it->runs[it->heap[0]];
-      while (rc.pos < rc.end && slot_cmp(&it->keys[rc.pos * c->kb], k, c->kb) == 0) it->valbuf.push_back(it->sums[rc.pos++]);
+      while (rc.pos < rc.end && slot_cmp(&it->keys[rc.pos * c->kb], k, c->kb) == 0) it->rows.push_back(rc.pos++);
       heap_fix_top(it);
       if (it->heap.empty()) break;
       const RunCursor& top = it->runs[it->heap[0]];
       if (slot_cmp(&it->keys[top.pos * c->kb], k, c->kb) != 0) break;
     }
-    nv = it->valbuf.size();
-    gathered = true;
   } else {
     heap_fix_top(it);
   }
   slot_key(k, c->kb, it->unesc);
+  return 1;
+}
+
+int mrhbm_groups_next(mrhbm_iter* it, const void** key, size_t* klen, const uint64_t** values, size_t* nvalues) {
+  if (!it || !key || !klen || !values || !nvalues) return MRHBM_E_INVAL;
+  mrhbm_ctx* c = it->ctx;
+  if (c->bytevals) return fail(c, MRHBM_E_INVAL, "the ctx carries byte values (MRHBM_F_BYTE_VALUES): use mrhbm_groups_next_values");
+  const LongGroup* lg;
+  const int r = next_group(it, &lg);
+  if (r <= 0) return r;
   *key = it->unesc.data();
   *klen = it->unesc.size();
-  *values = gathered ? it->valbuf.data() : &it->sums[i];
-  *nvalues = nv;
+  if (lg) {
+    *values = lg->values.data();
+    *nvalues = lg->values.size();
+  } else if (c->cfg.reducer == MRHBM_RED_NONE) {
+    it->valbuf.clear();
+    for (uint64_t row : it->rows) it->valbuf.push_back(it->sums[row]);
+    *values = it->valbuf.data();
+    *nvalues = it->valbuf.size();
+  } else {
+    *values = &it->sums[it->rows[0]];
+    *nvalues = 1;
+  }
+  return 1;
+}
+
+int mrhbm_groups_next_values(mrhbm_iter* it, const void** key, size_t* klen, const void** vals, const uint64_t** voff,
+                             size_t* nvalues) {
+  if (!it || !key || !klen || !vals || !voff || !nvalues) return MRHBM_E_INVAL;
+  mrhbm_ctx* c = it->ctx;
+  if (!c->bytevals) return refuse_byte_values(c);
+  const LongGroup* lg;
+  const int r = next_group(it, &lg);
+  if (r <= 0) return r;
+  it->vout.clear();
+  it->vout_off.assign(1, 0);
+  auto add = [&](const unsigned char* p, uint64_t n) {
+    it->vout.insert(it->vout.end(), p, p + n);
+    it->vout_off.push_back(it->vout.size());
+  };
+  if (lg) {
+    for (uint64_t v : lg->values) add((const unsigned char*)c->long_vals[v]->data(), c->long_vals[v]->size());
+  } else {
+    for (uint64_t row : it->rows) add(it->vbytes.data() + it->roff[row], it->roff[row + 1] - it->roff[row]);
+  }
+  it->vout.reserve(1);  // (a valid pointer for a group of empty values)
+  *key = it->unesc.data();
+  *klen = it->unesc.size();
+  *vals = it->vout.data();
+  *voff = it->vout_off.data();
+  *nvalues = it->vout_off.size() - 1;
   return 1;
 }
 
@@ -2141,6 +2462,8 @@ int mrhbm_comm_unique_id(mrhbm_ctx* c, void* id) {
 int mrhbm_comm_init(mrhbm_ctx* c, const void* id, int rank, int world) {
   if (!c || !id || world < 1 || rank < 0 || rank >= world) return MRHBM_E_INVAL;
   Entry g(c);
+  // (before any communicator exists: the value ids are pool indices of this rank only)
+  if (c->bytevals && world > 1) return fail(c, MRHBM_E_INVAL, "byte values (MRHBM_F_BYTE_VALUES) run on one GPU");
   if (world > 8) return fail(c, MRHBM_E_INVAL, "at most 8 ranks (one NVSwitch box)");
   if (c->world != 1) return fail(c, MRHBM_E_INVAL, "communicator already initialised");
   if (world == 1) return MRHBM_OK;

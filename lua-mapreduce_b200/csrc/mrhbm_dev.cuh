@@ -314,32 +314,35 @@ __device__ __forceinline__ void stg_stream(uint4* p, const uint4& v) {
 
 // ---- CTA-wide exclusive scan --------------------------------------------------
 // inclusive prefix sum of v over the first WIDTH lanes of the warp (a power of two <= 32)
-template <int WIDTH = 32>
-__device__ __forceinline__ uint32_t warp_inscan(uint32_t v) {
+template <int WIDTH = 32, typename T = uint32_t>
+__device__ __forceinline__ T warp_inscan(T v) {
   const uint32_t lane = threadIdx.x & 31;
 #pragma unroll
   for (int d = 1; d < WIDTH; d <<= 1) {
-    const uint32_t t = __shfl_up_sync(0xffffffffu, v, d);
+    const T t = __shfl_up_sync(0xffffffffu, v, d);
     if (lane >= (uint32_t)d) v += t;
   }
   return v;
 }
-struct CtaScan {
-  uint32_t excl;   // sum of `mine` over the threads before this one
-  uint32_t total;  // sum of `mine` over the CTA
+template <typename T>
+struct CtaScanT {
+  T excl;   // sum of `mine` over the threads before this one
+  T total;  // sum of `mine` over the CTA
 };
+using CtaScan = CtaScanT<uint32_t>;
 // One value per thread, THREADS == blockDim.x threads, one barrier: every warp scans the warp totals itself.
 // The warp totals live in static scratch that every call in the kernel shares: it may be written again only
 // after a barrier that follows every read of it (a barrier after the call, before the next call).
-template <int THREADS>
-__device__ __forceinline__ CtaScan cta_exscan(uint32_t mine) {
+// T: uint32_t (bin counts) or uint64_t (byte offsets of the value gather).
+template <int THREADS, typename T = uint32_t>
+__device__ __forceinline__ CtaScanT<T> cta_exscan(T mine) {
   constexpr int kWarps = THREADS / 32;
-  __shared__ uint32_t s_warp[kWarps];
+  __shared__ T s_warp[kWarps];
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const uint32_t incl = warp_inscan(mine);
+  const T incl = warp_inscan(mine);
   if (lane == 31) s_warp[warp] = incl;
   __syncthreads();
-  const uint32_t w = lane < (uint32_t)kWarps ? s_warp[lane] : 0u, wi = warp_inscan<kWarps>(w);
+  const T w = lane < (uint32_t)kWarps ? s_warp[lane] : T(0), wi = warp_inscan<kWarps>(w);
   return {__shfl_sync(0xffffffffu, wi - w, warp) + incl - mine, __shfl_sync(0xffffffffu, wi, kWarps - 1)};
 }
 

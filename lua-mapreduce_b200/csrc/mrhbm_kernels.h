@@ -199,4 +199,27 @@ int launch_checksum_out(int rb, const ShuffleBuffers& b, uint32_t B, const Range
                         uint64_t* acc6, cudaStream_t s);
 cudaError_t kernels_configure();  // opt-in shared memory sizes; call once per device
 
+// ---- byte values (MRHBM_F_BYTE_VALUES, mrhbm_values.cu) ----
+// A pair's value field holds its value id (its pool index); value id i has the bytes arena[voff[i] .. voff[i+1]).
+// Rows of the value gather per scan tile (the first pass scans each tile, the second the tile totals).
+constexpr uint32_t kValTileLog = 13;
+// Values longer than this are copied in pieces of this size, one warp per piece, after the row gather.
+constexpr uint32_t kValChunk = 4096;
+inline uint64_t val_tiles(uint64_t rows) { return (rows + (1u << kValTileLog) - 1) >> kValTileLog; }
+// most pieces of the values longer than kValChunk that `bytes` value bytes can hold
+inline uint64_t val_chunks_cap(uint64_t bytes) { return 2 * (bytes / kValChunk) + 1; }
+// records [0, n) of the rb-byte records at recs get value id first + i; dvoff[i] (i <= n, the caller's offsets as
+// copied) becomes dvoff[i] - v0 + aoff, an offset into the arena
+int launch_value_stamp(int rb, void* recs, uint64_t n, uint64_t first, uint64_t* dvoff, uint64_t v0, uint64_t aoff,
+                       cudaStream_t s);
+// row_off[r] for rows r < n whose value id is ids[r]: value bytes of the rows before r inside its scan tile;
+// tile_pre[t] (val_tiles(n) + 1 entries) the bytes before tile t, row_off[n] the total.  The gather completes row_off.
+int launch_value_scan(const uint64_t* ids, uint64_t n, const uint64_t* voff, uint64_t* row_off, uint64_t* tile_pre,
+                      cudaStream_t s);
+// copies every row's value bytes from the arena to out at its row offset (row_off is final afterwards); pieces is
+// scratch of val_chunks_cap(total) entries, npieces one zeroed word
+int launch_value_gather(const uint64_t* ids, uint64_t n, const uint64_t* voff, const unsigned char* arena,
+                        uint64_t* row_off, const uint64_t* tile_pre, unsigned char* out, uint64_t* pieces,
+                        unsigned long long* npieces, cudaStream_t s);
+
 }  // namespace mrhbm

@@ -20,6 +20,7 @@ local hbm = { _VERSION = "0.1", _NAME = "mapreduce.hbm" }
 local ctx -- one context per worker process (job.lua keeps `funcs`/`initialized` per process too)
 local sample_splitters = false -- hbm_splitters = "sample": hbm.prepare_reduce samples them before the shuffle
 local tuple_keys = false -- hbm.configure(..., { key_kind = "tuple" }); an upvalue of configure, map_job and groups
+local byte_values = false -- hbm.configure(..., { value_kind = "bytes" }): string and number values, general reducefn
 
 -- the 8-byte big-endian string of a u64 key minus one; nil for key 0
 local function be_minus_one(s)
@@ -42,6 +43,9 @@ function hbm.configure(partition_mod, reduce_mod, combiner_mod, opts)
          "a combinerfn runs on the device: it (and the reducefn) must declare hbm_reducefn = 'sum'")
   opts = opts or {}
   tuple_keys = opts.key_kind == "tuple" -- composite keys travel as encoded byte strings
+  byte_values = opts.value_kind == "bytes" -- values travel as encoded byte strings (hbm.encode_value)
+  assert(not (byte_values and builtin),
+         "value_kind = 'bytes' hands string and number values to a general reducefn: the reducefn must not declare hbm_reducefn")
   local c, err = mrhbm.new{
     key_kind = tuple_keys and "str" or opts.key_kind or "str",
     max_key_bytes = opts.max_key_bytes or 123,
@@ -50,6 +54,7 @@ function hbm.configure(partition_mod, reduce_mod, combiner_mod, opts)
     combiner = combiner_mod ~= nil,
     reducer = builtin and "sum" or "none",
     device = opts.device,
+    values = byte_values and "bytes" or "int",
   }
   ctx = assert(c, err)
   sample_splitters = false
@@ -129,10 +134,15 @@ local function words_to_double(hi, lo)
   return neg and -x or x
 end
 
-local function enc_num(x, out)
-  assert(x == x, "NaN cannot be a key")
-  if x == 0 then x = 0 end -- -0 and 0 are the same table key
-  local hi, lo = double_to_words(x)
+local function enc_num(x, out, value)
+  assert(x == x, value and "NaN cannot be a value" or "NaN cannot be a key")
+  local hi, lo
+  if value and x == 0 and 1 / x < 0 then
+    hi, lo = 0x80000000, 0 -- a value keeps -0
+  else
+    if x == 0 then x = 0 end -- -0 and 0 are the same table key
+    hi, lo = double_to_words(x)
+  end
   if hi >= 0x80000000 then hi, lo = 0xFFFFFFFF - hi, 0xFFFFFFFF - lo else hi = hi + 0x80000000 end
   -- 64 bits -> groups of 1,7,7,...,7 bits
   local bits = {}
@@ -213,11 +223,28 @@ dec_key = function(s, i)
 end
 function hbm.decode_key(s) return (dec_key(s, 1)) end
 
+-- Values of value_kind = "bytes" (same format as encode_value / decode_value in ../../mapreduce/tuple.py):
+--   value := "\16" num10 (as above, but -0 stays -0) | "\32" bytes (a Lua string: any bytes, any length)
+function hbm.encode_value(v)
+  if type(v) == "string" then return "\32" .. v end
+  assert(type(v) == "number", "values are strings or numbers")
+  local out = {}
+  enc_num(v, out, true)
+  return table.concat(out)
+end
+function hbm.decode_value(s)
+  local tag = s:byte(1)
+  if tag == 32 then return s:sub(2) end
+  assert(tag == 16 and #s == 11, "bad value encoding")
+  return (dec_component(s, 1))
+end
+
 -- job_prepare_map (job.lua:154-228): returns the emit closure and the finisher
 function hbm.map_job(map_key)
   local m = assert(ctx:map_begin(tostring(map_key)))
   local emit = function(key, value)
     if tuple_keys then key = hbm.encode_key(key) end
+    if byte_values then value = hbm.encode_value(value) end
     assert(m:emit(key, value))
   end
   local finish = function(ok)
@@ -236,10 +263,15 @@ end
 -- job_prepare_reduce (job.lua:230-296): for k,v in hbm.groups(part_key) do ... end
 function hbm.groups(part_key)
   local it = assert(ctx:groups(part_key))
-  if not tuple_keys then return it end
+  if not tuple_keys and not byte_values then return it end
   return function()
     local k, v = it()
-    if k ~= nil then return hbm.decode_key(k), v end
+    if k == nil then return nil end
+    if byte_values then
+      for i = 1, #v do v[i] = hbm.decode_value(v[i]) end
+    end
+    if tuple_keys then k = hbm.decode_key(k) end
+    return k, v
   end
 end
 

@@ -22,9 +22,9 @@
 #define MAP_MT "mrhbm.map"
 #define ITER_MT "mrhbm.iter"
 
-typedef struct { mrhbm_ctx *h; uint32_t nparts; } lctx;
-typedef struct { mrhbm_map *h; mrhbm_ctx *ctx; } lmap;
-typedef struct { mrhbm_iter *h; } liter;
+typedef struct { mrhbm_ctx *h; uint32_t nparts; int bytes; } lctx; /* bytes: values = "bytes" */
+typedef struct { mrhbm_map *h; mrhbm_ctx *ctx; int bytes; } lmap;
+typedef struct { mrhbm_iter *h; int bytes; } liter;
 
 static int fail(lua_State *L, mrhbm_ctx *c) { /* luamongo style: nil, msg */
   lua_pushnil(L);
@@ -33,7 +33,9 @@ static int fail(lua_State *L, mrhbm_ctx *c) { /* luamongo style: nil, msg */
 }
 
 /* mrhbm.new{ key_kind="str"|"u64", max_key_bytes=, num_partitions=, partitioner="fnv_lua"|"mulhash"|
- *            "wordhash"|"range", combiner=bool, reducer="sum"|"none", device= } */
+ *            "wordhash"|"range", combiner=bool, reducer="sum"|"none", device=, values="int"|"bytes" }
+ * values = "bytes" (MRHBM_F_BYTE_VALUES, needs reducer = "none"): m:emit takes string values and ctx:groups yields
+ * tables of strings */
 static int l_new(lua_State *L) {
   mrhbm_config cfg;
   const char *s;
@@ -59,10 +61,14 @@ static int l_new(lua_State *L) {
   lua_getfield(L, 1, "reducer"); /* "sum" (built-in) | "none" (general reducefn on the host) */
   s = luaL_optstring(L, -1, "sum");
   cfg.reducer = strcmp(s, "none") == 0 ? MRHBM_RED_NONE : MRHBM_RED_SUM;
-  lua_pop(L, 7);
+  lua_getfield(L, 1, "values");
+  s = luaL_optstring(L, -1, "int");
+  if (strcmp(s, "bytes") == 0) cfg.flags |= MRHBM_F_BYTE_VALUES;
+  lua_pop(L, 8);
   lctx *u = (lctx *)lua_newuserdata(L, sizeof *u);
   u->h = NULL;
   u->nparts = cfg.num_partitions;
+  u->bytes = (cfg.flags & MRHBM_F_BYTE_VALUES) != 0;
   luaL_setmetatable(L, CTX_MT);
   if (mrhbm_init(&cfg, &u->h) != MRHBM_OK) {
     lua_pushnil(L);
@@ -87,6 +93,7 @@ static int ctx_map_begin(lua_State *L) {
   lmap *m = (lmap *)lua_newuserdata(L, sizeof *m);
   m->h = NULL;
   m->ctx = u->h;
+  m->bytes = u->bytes;
   luaL_setmetatable(L, MAP_MT);
   /* the map keeps its ctx alive (Lua 5.2 user values are tables): commit / abort / __gc dereference it */
   lua_createtable(L, 1, 0);
@@ -96,14 +103,41 @@ static int ctx_map_begin(lua_State *L) {
   if (mrhbm_map_begin(u->h, id, &m->h) != MRHBM_OK) return fail(L, u->h);
   return 1;
 }
+/* map:emit(key, value) with values = "bytes": value is a Lua string (any bytes, copied before return) */
+static int map_emit_bytes(lua_State *L, lmap *m, int u64) {
+  size_t vlen, len;
+  const char *v = luaL_checklstring(L, 3, &vlen);
+  int rc;
+  if (lua_type(L, 2) == LUA_TNUMBER) {
+    lua_Number kn = lua_tonumber(L, 2);
+    if (!u64 || !(kn >= 0 && kn == floor(kn) && kn < 9007199254740992.0)) {
+      lua_pushnil(L);
+      lua_pushstring(L, "mrhbm: number keys need key_kind = 'u64' and an integer in [0, 2^53)");
+      return 2;
+    }
+    rc = mrhbm_emit_u64_value(m->h, (uint64_t)kn, v, vlen);
+  } else {
+    const char *k = luaL_checklstring(L, 2, &len);
+    if (u64 && len == 8) {
+      uint64_t x = 0;
+      for (int i = 0; i < 8; i++) x = (x << 8) | (unsigned char)k[i];
+      rc = mrhbm_emit_u64_value(m->h, x, v, vlen);
+    } else
+      rc = mrhbm_emit_str_value(m->h, k, len, v, vlen);
+  }
+  if (rc != MRHBM_OK) return fail(L, m->ctx);
+  lua_pushboolean(L, 1);
+  return 1;
+}
 /* map:emit(key, value): key is a Lua string (copied before return) or, for u64 ctx, an 8-byte
  * big-endian string / an integer-valued number < 2^53 (SURVEY A.4) */
 static int map_emit(lua_State *L) {
   lmap *m = (lmap *)luaL_checkudata(L, 1, MAP_MT);
   int rc;
-  lua_Number vn = luaL_optnumber(L, 3, 1);
   int u64 = m->h && mrhbm_record_bytes(m->ctx) == 16;
   if (!m->h) return fail(L, NULL);
+  if (m->bytes) return map_emit_bytes(L, m, u64);
+  lua_Number vn = luaL_optnumber(L, 3, 1);
   /* values are unsigned integers: < 2^32 in string records, < 2^53 (exact Lua numbers) with u64 keys.  Anything
    * else is refused here -- a C cast of an out-of-range double is undefined behaviour, not a wrap-around. */
   if (!(vn >= 0 && vn == floor(vn) && vn < (u64 ? 9007199254740992.0 : 4294967296.0))) {
@@ -227,10 +261,12 @@ static int ctx_sample_splitters(lua_State *L) {
  * job.lua:264-284; also finalfn's pair iterator, server.lua:360-385) */
 static int iter_next(lua_State *L) {
   liter *it = (liter *)lua_touserdata(L, lua_upvalueindex(1));
-  const void *key;
-  const uint64_t *vals;
+  const void *key, *bytes = NULL;
+  const uint64_t *vals = NULL, *voff = NULL;
   size_t klen, nvals, i;
-  int r = it->h ? mrhbm_groups_next(it->h, &key, &klen, &vals, &nvals) : 0;
+  int r = !it->h ? 0
+        : it->bytes ? mrhbm_groups_next_values(it->h, &key, &klen, &bytes, &voff, &nvals)
+                    : mrhbm_groups_next(it->h, &key, &klen, &vals, &nvals);
   if (r <= 0) {
     if (it->h) mrhbm_groups_close(it->h);
     it->h = NULL;
@@ -239,7 +275,10 @@ static int iter_next(lua_State *L) {
   lua_pushlstring(L, (const char *)key, klen);
   lua_createtable(L, (int)nvals, 0);
   for (i = 0; i < nvals; i++) {
-    lua_pushnumber(L, (lua_Number)vals[i]); /* sums < 2^53 are exact Lua numbers */
+    if (it->bytes)
+      lua_pushlstring(L, (const char *)bytes + voff[i], (size_t)(voff[i + 1] - voff[i]));
+    else
+      lua_pushnumber(L, (lua_Number)vals[i]); /* sums < 2^53 are exact Lua numbers */
     lua_rawseti(L, -2, (int)i + 1);
   }
   return 2;
@@ -255,6 +294,7 @@ static int ctx_groups(lua_State *L) {
   uint32_t p = (uint32_t)luaL_checkinteger(L, 2);
   liter *it = (liter *)lua_newuserdata(L, sizeof *it);
   it->h = NULL;
+  it->bytes = u->bytes;
   luaL_setmetatable(L, ITER_MT);
   if (mrhbm_groups_open(u->h, p, &it->h) != MRHBM_OK) return fail(L, u->h);
   lua_pushvalue(L, 1); /* second upvalue: the ctx stays alive as long as the iterator function does */

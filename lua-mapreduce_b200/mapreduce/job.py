@@ -63,16 +63,18 @@ class Job:
                 with open(self.doc["value"], "rb") as fh:
                     m.wordcount(fh.read())
                 mapfn = None
-            if cfg["hbm"]["key_kind"] == "u64":
-                def emit(key, value=1):
-                    m.emit(int(key), int(value))
-            elif cfg["hbm"]["key_kind"] == "tuple":
-                # composite keys (tuple.lua): order-preserving byte strings across the C ABI
-                def emit(key, value=1):
-                    m.emit(tuple_keys.encode(key), int(value))
+            kind = cfg["hbm"]["key_kind"]
+            if kind == "u64":
+                enc_key = int
+            elif kind == "tuple":
+                enc_key = tuple_keys.encode  # composite keys (tuple.lua): order-preserving byte strings across the C ABI
             else:
-                def emit(key, value=1):
-                    m.emit(_key_bytes(key), int(value))
+                enc_key = _key_bytes
+            # value_kind = "bytes": Lua strings and numbers as tagged bytes (tuple.encode_value); else integers
+            enc_val = tuple_keys.encode_value if cfg["hbm"].get("value_kind") == "bytes" else int
+
+            def emit(key, value=1):
+                m.emit(enc_key(key), enc_val(value))
             if mapfn is not None:
                 mapfn(self.get_id(), self.doc["value"], emit)  # job.lua:182
             self.board.mark(self.doc, STATUS.FINISHED, finished_time=time.time())
@@ -130,6 +132,7 @@ class Job:
             result.append(v)
 
         decode = tuple_keys.decode if cfg["hbm"]["key_kind"] == "tuple" else None
+        byte_values = cfg["hbm"].get("value_kind") == "bytes"
         bulk = self._bulk_groups(part) if (aci and cfg["hbm"].get("reducer", 0) == 0 and decode is None) else None
         if bulk is not None:
             # built-in reducer + ACI flags: every value list is the singleton the device produced and the reference
@@ -141,6 +144,8 @@ class Job:
         for key, values in ctx.groups(part):
             if decode:
                 key = decode(key)
+            if byte_values:
+                values = [tuple_keys.decode_value(v) for v in values]
             # The device applied the declared built-in (combiner semantics).  The reference
             # skips the reducer on singletons when the ACI flags are set (job.lua:264-274),
             # otherwise it always calls it (job.lua:275-284).

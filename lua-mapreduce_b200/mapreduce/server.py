@@ -98,8 +98,14 @@ class server:
             raise NotImplementedError("partitionfn module must declare hbm_partitionfn in %s" % sorted(_BUILTIN_PART))
         nparts = getattr(part, "NUM_REDUCERS", None) or getattr(part, "hbm_num_partitions", None)
         assert isinstance(nparts, int) and nparts >= 1, "partitionfn module must expose NUM_REDUCERS"
-        hbm = dict(key_kind="str", max_key_bytes=123, device=-1)
+        hbm = dict(key_kind="str", max_key_bytes=123, device=-1, value_kind="int")
         hbm.update(params.get("hbm") or {})
+        # value_kind = "bytes": values are Lua strings and numbers (tuple.encode_value), handed to a general reducefn
+        if hbm["value_kind"] not in ("int", "bytes"):
+            raise ValueError("hbm value_kind must be 'int' or 'bytes', got %r" % (hbm["value_kind"],))
+        if hbm["value_kind"] == "bytes" and builtin_red is not None:
+            raise ValueError("hbm value_kind = 'bytes' hands string and number values to a general reducefn: "
+                             "the reducefn module must not declare hbm_reducefn (it declares %r)" % (builtin_red,))
         hbm.update(partitioner=_BUILTIN_PART[pname], num_partitions=nparts, combiner=device_combiner,
                    reducer=0 if builtin_red == "sum" else 1,
                    splitters=range_splitters(part, nparts, hbm["key_kind"]) if pname == "range" else None)
@@ -115,7 +121,8 @@ class server:
         from .. import mrhbm
         kind = mrhbm.KEY_U64 if h["key_kind"] == "u64" else mrhbm.KEY_STR
         ctx = mrhbm.Ctx(kind, h["num_partitions"], h["partitioner"], max_key_bytes=h["max_key_bytes"],
-                        combiner=h["combiner"], device=h["device"], reducer=h["reducer"])
+                        combiner=h["combiner"], device=h["device"], reducer=h["reducer"],
+                        flags=mrhbm.F_BYTE_VALUES if h.get("value_kind") == "bytes" else 0)
         if isinstance(h.get("splitters"), list):  # (kept across reset)
             ctx.set_splitters(h["splitters"])
         return ctx

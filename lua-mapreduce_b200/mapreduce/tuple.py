@@ -11,7 +11,12 @@ class) and is decoded again on the reduce side:
               | 0x20 bytes 0x01           -- Lua string (bytes >= 0x02), a proper prefix sorts first
               | 0x30 key                  -- nested tuple
 
-Bytewise order of the encoding = length first, then component-wise lexicographic.  The reference's
+Values (server:configure{hbm = {value_kind = "bytes"}}) cross the C ABI as opaque bytes that keep the Lua type:
+
+    value    := 0x10 num10                -- Lua number, the key encoding above, except that -0 stays -0
+              | 0x20 bytes                -- Lua string: any bytes, any length
+
+Bytewise order of the key encoding = length first, then component-wise lexicographic.  The reference's
 `__lt` (shorter first; same length: "no component greater") is only a partial order; this is a
 linear extension of it: whenever the reference says a < b, encode(a) < encode(b)
 (tests/test_tuple_keys.py checks that against `lt`, the restatement of tuple.lua:183-195).
@@ -51,15 +56,16 @@ def lt(a, b):
     return True
 
 
-def _enc_num(x, out):
+def _enc_num(x, out, key=True):
     if isinstance(x, bool) or not isinstance(x, (int, float)):
         raise TypeError("not a number: %r" % (x,))
     if isinstance(x, int) and abs(x) > (1 << 53):
         raise OverflowError("integer %d is not exact as a Lua number" % x)
     f = float(x)
     if math.isnan(f):
-        raise ValueError("NaN cannot be a key (Lua rejects it as a table index)")
-    if f == 0.0:
+        # (as a value: the reference's "%.14g" spill line cannot load() it back either)
+        raise ValueError("NaN cannot be a key (Lua rejects it as a table index)" if key else "NaN cannot be a value")
+    if key and f == 0.0:
         f = 0.0  # -0 and 0 are the same Lua table key
     (u,) = struct.unpack(">Q", struct.pack(">d", f))
     u = u ^ 0xFFFFFFFFFFFFFFFF if u >> 63 else u | (1 << 63)  # total order of doubles as unsigned
@@ -74,6 +80,8 @@ def _dec_num(b, i):
     u &= 0xFFFFFFFFFFFFFFFF
     u = u & ~(1 << 63) if u >> 63 else u ^ 0xFFFFFFFFFFFFFFFF
     (f,) = struct.unpack(">d", struct.pack(">Q", u))
+    if f == 0.0 and math.copysign(1.0, f) < 0:
+        return f, i + 10  # -0 (values only: keys fold it to 0)
     return (int(f) if f.is_integer() and abs(f) <= (1 << 53) else f), i + 10
 
 
@@ -145,3 +153,23 @@ def decode(b):
     if i != len(b):
         raise ValueError("trailing bytes after the key")
     return k
+
+
+def encode_value(v):
+    """Lua string (bytes / str) or number -> the opaque bytes of a byte-values shuffle (see the module text)."""
+    if isinstance(v, (bytes, bytearray, str)):
+        return bytes([_STR]) + (v.encode() if isinstance(v, str) else bytes(v))
+    out = bytearray()
+    _enc_num(v, out, key=False)
+    return bytes(out)
+
+
+def decode_value(b):
+    """inverse of encode_value (strings come back as bytes, integral numbers as ints, -0 as -0.0)."""
+    if not b:
+        raise ValueError("empty value encoding")
+    if b[0] == _STR:
+        return bytes(b[1:])
+    if b[0] == _NUM and len(b) == 11:
+        return _dec_num(b, 1)[0]
+    raise ValueError("bad value encoding (tag 0x%02x, %d bytes)" % (b[0], len(b)))

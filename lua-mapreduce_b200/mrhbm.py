@@ -13,7 +13,7 @@ from . import build as _build
 KEY_U64, KEY_STR = 0, 1
 PART_FNV_LUA, PART_MULHASH, PART_WORDHASH, PART_RANGE = 0, 1, 2, 3
 RED_SUM, RED_NONE = 0, 1
-F_FORCE_RUNS, F_SMALL_BINS, F_NO_OPTIMISTIC = 1, 2, 4
+F_FORCE_RUNS, F_SMALL_BINS, F_NO_OPTIMISTIC, F_BYTE_VALUES = 1, 2, 4, 8
 E_NODEVICE = -8
 UNIQUE_ID_BYTES = 128
 
@@ -56,7 +56,8 @@ EXPORTS = [
     "mrhbm_map_abort", "mrhbm_shuffle", "mrhbm_partitions", "mrhbm_groups_open", "mrhbm_groups_next",
     "mrhbm_groups_close", "mrhbm_result_info_get", "mrhbm_result_copy", "mrhbm_checksum_input",
     "mrhbm_checksum_result", "mrhbm_stats_get", "mrhbm_reset", "mrhbm_comm_unique_id", "mrhbm_comm_init",
-    "mrhbm_set_splitters", "mrhbm_sample_splitters",
+    "mrhbm_set_splitters", "mrhbm_sample_splitters", "mrhbm_emit_str_value", "mrhbm_emit_u64_value",
+    "mrhbm_emit_batch_values", "mrhbm_groups_next_values", "mrhbm_result_values",
 ]
 
 _lib = None
@@ -118,6 +119,11 @@ def load(build_if_missing=True):
     sig("mrhbm_comm_init", i, vp, vp, i, i)
     sig("mrhbm_set_splitters", i, vp, vp, C.POINTER(u64), sz)
     sig("mrhbm_sample_splitters", i, vp, vp, sz, C.POINTER(u64), C.POINTER(sz))
+    sig("mrhbm_emit_str_value", i, vp, C.c_char_p, sz, C.c_char_p, sz)
+    sig("mrhbm_emit_u64_value", i, vp, u64, C.c_char_p, sz)
+    sig("mrhbm_emit_batch_values", i, vp, vp, sz, vp, vp)
+    sig("mrhbm_groups_next_values", i, vp, C.POINTER(vp), C.POINTER(sz), C.POINTER(vp), C.POINTER(vp), C.POINTER(sz))
+    sig("mrhbm_result_values", i, vp, vp, sz, vp, C.POINTER(sz))
     _lib = L
     return L
 
@@ -164,6 +170,16 @@ class Map:
         ctx._chk(ctx.L.mrhbm_map_begin(ctx.h, str(job_id).encode(), C.byref(self.h)))
 
     def emit(self, key, value=1):
+        if self.ctx.byte_values:  # any bytes (F_BYTE_VALUES)
+            if not isinstance(value, (bytes, bytearray)):
+                raise MrhbmError(-1, "a byte-values ctx takes bytes values, got %r" % type(value).__name__)
+            v = bytes(value)
+            if isinstance(key, int):
+                rc = self.ctx.L.mrhbm_emit_u64_value(self.h, key, v, len(v))
+            else:
+                rc = self.ctx.L.mrhbm_emit_str_value(self.h, key, len(key), v, len(v))
+            self.ctx._chk(rc)
+            return
         # values are unsigned integers: < 2^32 in string records, < 2^53 (exact Lua numbers) with u64 keys;
         # ctypes would silently wrap or truncate anything else
         u64 = isinstance(key, int)
@@ -179,6 +195,20 @@ class Map:
         a = np.ascontiguousarray(recs)
         assert a.dtype.itemsize == self.ctx.record_bytes, "record layout mismatch"
         self.ctx._chk(self.ctx.L.mrhbm_emit_batch(self.h, a.ctypes.data, a.shape[0]))
+
+    def emit_batch_values(self, recs, blob, voff):
+        """F_BYTE_VALUES: records in the ctx layout (value field ignored); value i is blob[voff[i]:voff[i+1]].
+        numpy arrays (pinned ones from Ctx.pinned_array too) or bytes for the blob."""
+        a = np.ascontiguousarray(recs)
+        assert a.dtype.itemsize == self.ctx.record_bytes, "record layout mismatch"
+        b = np.frombuffer(blob, dtype=np.uint8) if isinstance(blob, (bytes, bytearray)) else np.ascontiguousarray(blob)
+        o = np.ascontiguousarray(voff, dtype=np.uint64)
+        if o.shape[0] != a.shape[0] + 1:
+            raise MrhbmError(-1, "emit_batch_values: %d records need %d offsets, got %d" % (a.shape[0], a.shape[0] + 1, o.shape[0]))
+        if a.shape[0] and int(o[-1]) > b.nbytes:
+            raise MrhbmError(-1, "emit_batch_values: offsets reach %d, the blob holds %d bytes" % (int(o[-1]), b.nbytes))
+        self.ctx._chk(self.ctx.L.mrhbm_emit_batch_values(self.h, a.ctypes.data, a.shape[0], b.ctypes.data if b.nbytes else None,
+                                                         o.ctypes.data))
 
     def emit_batch_ptr(self, ptr, n):
         self.ctx._chk(self.ctx.L.mrhbm_emit_batch(self.h, ptr, n))
@@ -237,6 +267,7 @@ class Ctx:
             raise MrhbmError(rc, msg)
         self.key_kind = key_kind
         self.num_partitions = num_partitions
+        self.byte_values = bool(flags & F_BYTE_VALUES)
         self.record_bytes = self.L.mrhbm_record_bytes(self.h)
 
     def _chk(self, rc):
@@ -302,17 +333,27 @@ class Ctx:
 
     # -- reduce side
     def groups(self, partition):
-        """Yields (key bytes, [values]) in ascending key order (utils.merge_iterator order)."""
+        """Yields (key bytes, [values]) in ascending key order (utils.merge_iterator order); with F_BYTE_VALUES the
+        values are bytes."""
         it = C.c_void_p()
         self._chk(self.L.mrhbm_groups_open(self.h, partition, C.byref(it)))
-        kp, kl, vp, vn = C.c_void_p(), C.c_size_t(), C.c_void_p(), C.c_size_t()
+        kp, kl, vp, vn, op = C.c_void_p(), C.c_size_t(), C.c_void_p(), C.c_size_t(), C.c_void_p()
         try:
             while True:
-                r = self._chk(self.L.mrhbm_groups_next(it, C.byref(kp), C.byref(kl), C.byref(vp), C.byref(vn)))
+                if self.byte_values:
+                    r = self._chk(self.L.mrhbm_groups_next_values(it, C.byref(kp), C.byref(kl), C.byref(vp), C.byref(op),
+                                                                  C.byref(vn)))
+                else:
+                    r = self._chk(self.L.mrhbm_groups_next(it, C.byref(kp), C.byref(kl), C.byref(vp), C.byref(vn)))
                 if r == 0:
                     return
                 key = C.string_at(kp, kl.value) if kl.value else b""
-                yield key, list((C.c_uint64 * vn.value).from_address(vp.value))
+                if self.byte_values:
+                    off = (C.c_uint64 * (vn.value + 1)).from_address(op.value)
+                    blob = C.string_at(vp, off[vn.value]) if off[vn.value] else b""
+                    yield key, [blob[off[j]:off[j + 1]] for j in range(vn.value)]
+                else:
+                    yield key, list((C.c_uint64 * vn.value).from_address(vp.value))
         finally:
             self.L.mrhbm_groups_close(it)
 
@@ -322,11 +363,18 @@ class Ctx:
         return info
 
     def result_copy(self, keys=None, sums=None):
-        """(keys, sums, part_off): all groups of this rank, partition-major."""
+        """(keys, sums, part_off): all groups of this rank, partition-major (F_BYTE_VALUES: sums is None, see
+        result_values)."""
         info = self.result_info()
         g = info.groups
         if keys is None:
             keys = np.empty(max(g, 1), dtype=np.uint64 if self.key_kind == KEY_U64 else "S%d" % info.key_bytes)
+        if self.byte_values:  # rows carry value ids, their bytes come from result_values
+            if keys.shape[0] < g:
+                raise MrhbmError(-1, "result_copy: the key array holds %d groups, %d needed" % (keys.shape[0], g))
+            po = np.empty(self.num_partitions + 1, dtype=np.uint64)
+            self._chk(self.L.mrhbm_result_copy(self.h, keys.ctypes.data, None, po.ctypes.data))
+            return keys[:g], None, po
         if sums is None:
             sums = np.empty(max(g, 1), dtype=np.uint64)
         if keys.shape[0] < g or sums.shape[0] < g:
@@ -334,6 +382,16 @@ class Ctx:
         po = np.empty(self.num_partitions + 1, dtype=np.uint64)
         self._chk(self.L.mrhbm_result_copy(self.h, keys.ctypes.data, sums.ctypes.data, po.ctypes.data))
         return keys[:g], sums[:g], po
+
+    def result_values(self):
+        """F_BYTE_VALUES: (uint8 blob, uint64 row_off) -- row r's value is blob[row_off[r]:row_off[r+1]], rows in
+        result_copy order."""
+        need = C.c_size_t()
+        self._chk(self.L.mrhbm_result_values(self.h, None, 0, None, C.byref(need)))
+        blob = np.empty(max(need.value, 1), dtype=np.uint8)
+        row_off = np.empty(self.result_info().groups + 1, dtype=np.uint64)
+        self._chk(self.L.mrhbm_result_values(self.h, blob.ctypes.data, blob.nbytes, row_off.ctypes.data, C.byref(need)))
+        return blob[:need.value], row_off
 
     def checksum_input(self):
         a = (C.c_uint64 * 4)()
