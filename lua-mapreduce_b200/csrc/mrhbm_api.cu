@@ -19,11 +19,11 @@
 #include "mrhbm_kernels.h"
 #include "mrhbm_dev.cuh"  // splitmix64
 #include "mrhbm_keys.h"
+#include "mrhbm_pool.h"
 
 using namespace mrhbm;
 
 namespace {
-enum { R_OPEN = 0, R_COMMITTED = 1, R_DEAD = 2 };
 constexpr uint32_t kErrfLongKeys = 0x80000000u;  // rides on the error-flag all-gather of a multi-GPU shuffle: this rank holds long keys
 constexpr size_t kMaxLongKey = 1u << 20;  // bytes; longer keys are refused (MRHBM_E_KEY)
 struct LongPair {
@@ -36,13 +36,6 @@ struct LongGroup {
   std::vector<uint64_t> values;  // built-in sum: one element
 };
 
-struct Range {
-  uint64_t off, cnt;
-  std::string job;
-  int state;
-  uint64_t owner;  // map handle serial
-  uint64_t aoff;   // MRHBM_F_BYTE_VALUES: the arena offset of the range's first value (its bytes follow in pool order)
-};
 constexpr size_t kStageRecs = 1 << 16;
 constexpr size_t kStageValBytes = 4u << 20;       // value bytes staged next to the records; a longer value goes alone
 constexpr uint64_t kMaxValue = 1ull << 30;        // bytes; longer values are refused (MRHBM_E_INVAL)
@@ -54,17 +47,15 @@ struct mrhbm_ctx {
   mrhbm_config cfg{};
   int dev = 0, rb = 16, kb = 8, sm_count = 132;
   cudaStream_t stream = nullptr;
-  // HBM emit pool: committed + open map output, record granularity
+  // HBM emit pool: committed + open map output, record granularity; led says what is in use and whose it is
   void* pool = nullptr;
-  uint64_t pool_cap = 0, pool_used = 0;
-  std::vector<Range> ranges;
-  uint64_t map_serial = 0;
+  uint64_t pool_cap = 0;
+  PoolLedger led;
   // MRHBM_F_BYTE_VALUES: a pair's value field holds its pool index (value id); value id i has the bytes
-  // arena[voff[i] .. voff[i+1]).  Values are appended in pool order, so voff[pool_used] == arena_used always; abort
-  // takes back the arena with the pool, dead ranges keep their bytes until mrhbm_reset.
+  // arena[voff[i] .. voff[i+1])
   bool bytevals = false;
   unsigned char* arena = nullptr;
-  uint64_t arena_cap = 0, arena_used = 0;
+  uint64_t arena_cap = 0;
   uint64_t* voff = nullptr;  // pool_cap + 1 entries
   // after the compaction: row r's value at cvals[row_off[r] .. row_off[r+1])
   unsigned char* cvals = nullptr;
@@ -240,82 +231,84 @@ int regrow(mrhbm_ctx* c, void** p, uint64_t want, uint64_t keep, size_t elem) {
   return 0;
 }
 
-int pool_reserve(mrhbm_ctx* c, uint64_t n, uint64_t* off) {
-  if (c->bytevals && c->pool_used + n >= 0xffffffffull)  // (value ids are u32 in string records)
-    return fail(c, MRHBM_E_INVAL, "byte values: 2^32 pairs emitted since the last reset");
-  if (c->pool_used + n > c->pool_cap) {
-    uint64_t want = std::max<uint64_t>(c->pool_used + n, c->pool_cap * 2);
+// Room at the tail of the pool (and of the arena) between the moment it is taken and the moment it becomes a range of
+// a map's output.  If its owner returns before add() -- a copy or a launch failed -- the ledger is rewound and the
+// room is free again.
+struct Reservation {
+  PoolLedger* led = nullptr;  // set while the room is held
+  PoolLedger::Mark mk{};
+  uint64_t off = 0, aoff = 0, n = 0;
+  ~Reservation() {
+    if (led) led->rewind(mk);
+  }
+  void add(const mrhbm_map* m) {
+    led->add(m->serial, m->job, off, n, aoff);
+    led = nullptr;
+  }
+};
+
+int stage_flush(mrhbm_map* m);
+
+// r: room for n records straight in the pool and, with byte values, for the `bytes` bytes of their values in the arena
+// (values follow pool order).  With `behind`, the room lies behind what that map has staged (emission order).  The
+// caller fills the room and then adds it.
+int reserve(mrhbm_ctx* c, mrhbm_map* behind, uint64_t n, uint64_t bytes, Reservation& r) {
+  int rc = behind ? stage_flush(behind) : 0;
+  if (rc) return rc;
+  PoolLedger& led = c->led;
+  if (!led.fits(n)) return fail(c, MRHBM_E_INVAL, "byte values: 2^32 pairs emitted since the last reset");
+  if (led.used() + n > c->pool_cap) {
+    uint64_t want = std::max<uint64_t>(led.used() + n, c->pool_cap * 2);
     want = std::max<uint64_t>(want, 1 << 16);
-    int rc = regrow(c, &c->pool, want, c->pool_used, (size_t)c->rb);
-    if (!rc && c->bytevals) rc = regrow(c, (void**)&c->voff, want + 1, c->voff ? c->pool_used + 1 : 0, sizeof(uint64_t));
+    rc = regrow(c, &c->pool, want, led.used(), (size_t)c->rb);
+    if (!rc && c->bytevals) rc = regrow(c, (void**)&c->voff, want + 1, c->voff ? led.used() + 1 : 0, sizeof(uint64_t));
     if (rc) return rc;
     c->pool_cap = want;
   }
-  *off = c->pool_used;
-  c->pool_used += n;
-  return 0;
-}
-
-// MRHBM_F_BYTE_VALUES: room for `bytes` value bytes at the end of the arena, *aoff the first.  Called right after the
-// pool_reserve of the pairs they belong to (values follow pool order).
-int arena_reserve(mrhbm_ctx* c, uint64_t bytes, uint64_t* aoff) {
-  if (c->arena_used + bytes > c->arena_cap) {
-    uint64_t want = std::max<uint64_t>(c->arena_used + bytes, c->arena_cap * 2);
+  if (led.arena_used() + bytes > c->arena_cap) {
+    uint64_t want = std::max<uint64_t>(led.arena_used() + bytes, c->arena_cap * 2);
     want = std::max<uint64_t>(want, 1 << 20);
-    int rc = regrow(c, (void**)&c->arena, want, c->arena_used, 1);
+    rc = regrow(c, (void**)&c->arena, want, led.arena_used(), 1);
     if (rc) return rc;
     c->arena_cap = want;
   }
-  *aoff = c->arena_used;
-  c->arena_used += bytes;
+  r.mk = led.mark();
+  const PoolLedger::Room room = led.take(n, bytes);
+  r.led = &led;
+  r.off = room.off;
+  r.aoff = room.aoff;
+  r.n = n;
   return 0;
 }
 
-// aoff: the arena offset of the first pair's value (byte values; else 0)
-void add_range(mrhbm_map* m, uint64_t off, uint64_t cnt, uint64_t aoff = 0) {
-  mrhbm_ctx* c = m->ctx;
-  if (!c->ranges.empty()) {
-    Range& r = c->ranges.back();
-    if (r.owner == m->serial && r.state == R_OPEN && r.off + r.cnt == off) {
-      r.cnt += cnt;
-      return;
-    }
+// MRHBM_F_BYTE_VALUES: the value id into a record
+void put_value_id(unsigned char* rec, int rb, int kb, uint64_t id) {
+  if (rb == 16)
+    memcpy(rec + 8, &id, 8);
+  else {
+    const uint32_t id32 = (uint32_t)id;
+    memcpy(rec + kb, &id32, 4);
   }
-  c->ranges.push_back(Range{off, cnt, m->job, R_OPEN, m->serial, aoff});
 }
 
 int stage_flush(mrhbm_map* m) {
   mrhbm_ctx* c = m->ctx;
   if (!m->fill) return 0;
-  uint64_t off, aoff = 0;
-  int rc = pool_reserve(c, m->fill, &off);
+  const uint64_t bytes = c->bytevals ? m->vrel[m->cur][m->fill] : 0;
+  Reservation r;
+  int rc = reserve(c, nullptr, m->fill, bytes, r);
   if (rc) return rc;
   if (c->bytevals) {
     // the staged records get their value ids, the staged offsets become arena offsets
-    const uint64_t bytes = m->vrel[m->cur][m->fill];
-    rc = arena_reserve(c, bytes, &aoff);
-    if (rc) {
-      c->pool_used = off;
-      return rc;
-    }
-    unsigned char* st = m->stage[m->cur];
-    for (size_t i = 0; i < m->fill; i++) {
-      if (c->rb == 16) {
-        const uint64_t id = off + i;
-        memcpy(st + i * 16 + 8, &id, 8);
-      } else {
-        const uint32_t id = (uint32_t)(off + i);
-        memcpy(st + i * c->rb + c->kb, &id, 4);
-      }
-    }
-    for (size_t i = 0; i <= m->fill; i++) m->vrel[m->cur][i] += aoff;
-    if (bytes) CU(c, cudaMemcpyAsync(c->arena + aoff, m->vstage[m->cur], bytes, cudaMemcpyHostToDevice, c->stream));
-    CU(c, cudaMemcpyAsync(c->voff + off, m->vrel[m->cur], (m->fill + 1) * 8, cudaMemcpyHostToDevice, c->stream));
+    for (size_t i = 0; i < m->fill; i++) put_value_id(m->stage[m->cur] + i * c->rb, c->rb, c->kb, r.off + i);
+    for (size_t i = 0; i <= m->fill; i++) m->vrel[m->cur][i] += r.aoff;
+    if (bytes) CU(c, cudaMemcpyAsync(c->arena + r.aoff, m->vstage[m->cur], bytes, cudaMemcpyHostToDevice, c->stream));
+    CU(c, cudaMemcpyAsync(c->voff + r.off, m->vrel[m->cur], (m->fill + 1) * 8, cudaMemcpyHostToDevice, c->stream));
   }
-  CU(c, cudaMemcpyAsync((char*)c->pool + off * c->rb, m->stage[m->cur], m->fill * c->rb, cudaMemcpyHostToDevice, c->stream));
+  CU(c, cudaMemcpyAsync((char*)c->pool + r.off * c->rb, m->stage[m->cur], m->fill * c->rb, cudaMemcpyHostToDevice, c->stream));
   CU(c, cudaEventRecord(m->stage_ev[m->cur], c->stream));
   m->stage_busy[m->cur] = true;
-  add_range(m, off, m->fill, aoff);
+  r.add(m);
   m->fill = 0;
   m->cur ^= 1;
   if (m->stage_busy[m->cur]) {
@@ -346,45 +339,40 @@ int stage_slot(mrhbm_map* m, unsigned char** slot) {
   return 0;
 }
 
+int check_value(mrhbm_ctx* c, const void* val, size_t vlen) {
+  if (vlen > kMaxValue) return fail(c, MRHBM_E_INVAL, "value of %zu bytes (limit %llu)", vlen, (unsigned long long)kMaxValue);
+  if (vlen && !val) return fail(c, MRHBM_E_INVAL, "null value");
+  return 0;
+}
+
 // MRHBM_F_BYTE_VALUES: one pair, its key written into the record slot by key_to_slot, its value staged next to it.  A
 // value larger than the value stage goes to the device on its own, behind what is staged.
 template <class F>
 int stage_value_pair(mrhbm_map* m, const void* val, size_t vlen, F key_to_slot) {
   mrhbm_ctx* c = m->ctx;
-  if (vlen > kMaxValue) return fail(c, MRHBM_E_INVAL, "value of %zu bytes (limit %llu)", vlen, (unsigned long long)kMaxValue);
-  if (vlen && !val) return fail(c, MRHBM_E_INVAL, "null value");
+  int rc = check_value(c, val, vlen);
+  if (rc) return rc;
   if (vlen > kStageValBytes) {
-    int rc = stage_flush(m);
-    uint64_t off = 0, aoff = 0;
-    if (!rc) rc = pool_reserve(c, 1, &off);
+    Reservation r;
+    rc = reserve(c, m, 1, vlen, r);
     if (rc) return rc;
-    rc = arena_reserve(c, vlen, &aoff);
-    if (rc) {
-      c->pool_used = off;
-      return rc;
-    }
     unsigned char rec[128];
     key_to_slot(rec);
-    if (c->rb == 16)
-      memcpy(rec + 8, &off, 8);
-    else {
-      const uint32_t id = (uint32_t)off;
-      memcpy(rec + c->kb, &id, 4);
-    }
-    const uint64_t vo[2] = {aoff, aoff + vlen};
-    CU(c, cudaMemcpyAsync(c->arena + aoff, val, vlen, cudaMemcpyHostToDevice, c->stream));
-    CU(c, cudaMemcpyAsync(c->voff + off, vo, sizeof vo, cudaMemcpyHostToDevice, c->stream));
-    CU(c, cudaMemcpyAsync((char*)c->pool + off * c->rb, rec, c->rb, cudaMemcpyHostToDevice, c->stream));
+    put_value_id(rec, c->rb, c->kb, r.off);
+    const uint64_t vo[2] = {r.aoff, r.aoff + vlen};
+    CU(c, cudaMemcpyAsync(c->arena + r.aoff, val, vlen, cudaMemcpyHostToDevice, c->stream));
+    CU(c, cudaMemcpyAsync(c->voff + r.off, vo, sizeof vo, cudaMemcpyHostToDevice, c->stream));
+    CU(c, cudaMemcpyAsync((char*)c->pool + r.off * c->rb, rec, c->rb, cudaMemcpyHostToDevice, c->stream));
     CU(c, cudaStreamSynchronize(c->stream));  // (the caller's value may be pinned memory: copied before return)
-    add_range(m, off, 1, aoff);
+    r.add(m);
     return MRHBM_OK;
   }
   if (m->stage[0] && m->fill && m->vrel[m->cur][m->fill] + vlen > kStageValBytes) {
-    int rc = stage_flush(m);
+    rc = stage_flush(m);
     if (rc) return rc;
   }
   unsigned char* slot;
-  int rc = stage_slot(m, &slot);
+  rc = stage_slot(m, &slot);
   if (rc) return rc;
   const size_t i = m->fill - 1;
   if (i == 0) m->vrel[m->cur][0] = 0;
@@ -401,11 +389,28 @@ int refuse_byte_values(mrhbm_ctx* c) {
   return fail(c, MRHBM_E_INVAL, "byte values need a ctx with MRHBM_F_BYTE_VALUES");
 }
 
-// room for n records of the map's output straight in the pool, behind what it has staged (emission order): *off is
-// the first of them.  The caller fills them and then adds the range.
-int pool_take(mrhbm_map* m, uint64_t n, uint64_t* off) {
-  int rc = stage_flush(m);
-  return rc ? rc : pool_reserve(m->ctx, n, off);
+// A key whose escaped form (elen bytes) does not fit a record slot stays on the host, escaped like a slot would hold
+// it, with its value or value bytes (see mrhbm_ctx::long_jobs).
+int long_pair(mrhbm_map* m, const unsigned char* k, size_t klen, size_t elen, uint64_t value, const void* val, size_t vlen) {
+  mrhbm_ctx* c = m->ctx;
+  if (klen > kMaxLongKey) return fail(c, MRHBM_E_KEY, "key of %zu bytes (limit %zu)", klen, (size_t)kMaxLongKey);
+  int rc = check_value(c, val, vlen);
+  if (rc) return rc;
+  LongPair lp;
+  lp.esc.resize(elen);
+  escape(k, klen, (unsigned char*)&lp.esc[0]);
+  lp.value = value;
+  if (vlen) lp.bytes.assign((const char*)val, vlen);
+  m->long_pairs.push_back(std::move(lp));
+  return MRHBM_OK;
+}
+
+// a host pointer that the copy engine reads in place: a copy from it is still running when the call returns
+bool is_pinned(const void* p) {
+  cudaPointerAttributes at{};
+  const bool pinned = p && cudaPointerGetAttributes(&at, p) == cudaSuccess && at.type == cudaMemoryTypeHost;
+  cudaGetLastError();
+  return pinned;
 }
 
 void map_release(mrhbm_map* m) {
@@ -473,19 +478,6 @@ int ensure_buffers(mrhbm_ctx* c, uint64_t B, uint64_t N) {
   int rc = ensure_small_arrays(c, B);
   if (!rc) rc = ensure_records(c, &c->sb.mid, &c->mid_cap, N);
   return rc ? rc : ensure_out(c, N);
-}
-
-// committed ranges, adjacent ones merged
-std::vector<std::pair<uint64_t, uint64_t>> live_ranges(const mrhbm_ctx* c) {
-  std::vector<std::pair<uint64_t, uint64_t>> v;
-  for (const Range& r : c->ranges) {
-    if (r.state != R_COMMITTED || !r.cnt) continue;
-    if (!v.empty() && v.back().first + v.back().second == r.off)
-      v.back().second += r.cnt;
-    else
-      v.emplace_back(r.off, r.cnt);
-  }
-  return v;
 }
 
 int ensure_compact(mrhbm_ctx* c) {
@@ -582,7 +574,7 @@ int mrhbm_init(const mrhbm_config* cfg, mrhbm_ctx** out) {
   if (cfg->reducer == MRHBM_RED_NONE && cfg->combiner) return fail(c, MRHBM_E_INVAL, "a general reducer cannot be combined on the device (combiner must be 0)");
   if ((cfg->flags & MRHBM_F_BYTE_VALUES) && (cfg->reducer != MRHBM_RED_NONE || cfg->combiner))
     return fail(c, MRHBM_E_INVAL, "byte values (MRHBM_F_BYTE_VALUES) need reducer MRHBM_RED_NONE and combiner 0");
-  c->bytevals = (cfg->flags & MRHBM_F_BYTE_VALUES) != 0;
+  c->bytevals = c->led.byte_values = (cfg->flags & MRHBM_F_BYTE_VALUES) != 0;
   c->sb.no_reduce = cfg->reducer == MRHBM_RED_NONE;
   CU(c, cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
   if (cfg->partitioner == MRHBM_PART_RANGE && cfg->num_partitions == 1) {  // one key range, no splitters: its table now
@@ -601,11 +593,10 @@ int mrhbm_init(const mrhbm_config* cfg, mrhbm_ctx** out) {
   c->cap = (cfg->flags & MRHBM_F_SMALL_BINS) ? 96 : cap_records(c->rb);
   CU(c, cudaMalloc((void**)&c->d_sample, 256 * sizeof(uint32_t)));
   CU(c, cudaHostAlloc((void**)&c->h_sample, 256 * sizeof(uint32_t), cudaHostAllocDefault));
-  if (cfg->reserve_pairs) {
-    uint64_t off;
-    int rc = pool_reserve(c, cfg->reserve_pairs, &off);
+  if (cfg->reserve_pairs) {  // capacity only: the room goes straight back
+    Reservation r;
+    int rc = reserve(c, nullptr, cfg->reserve_pairs, 0, r);
     if (rc) return rc;
-    c->pool_used = 0;
   }
   return MRHBM_OK;
 }
@@ -672,7 +663,7 @@ int mrhbm_map_begin(mrhbm_ctx* c, const char* job, mrhbm_map** out) {
   mrhbm_map* m = new mrhbm_map();
   m->ctx = c;
   m->job = job;
-  m->serial = ++c->map_serial;
+  m->serial = c->led.new_owner();
   *out = m;
   return MRHBM_OK;
 }
@@ -686,15 +677,7 @@ int mrhbm_emit_str(mrhbm_map* m, const void* key, size_t klen, uint32_t value) {
   // (keys are stored escaped, see escape)
   const unsigned char* k = (const unsigned char*)key;
   const size_t elen = esc_size(k, klen);
-  if (elen >= (size_t)c->kb) {  // longer than a record slot: kept on the host (escaped like a slot would hold it)
-    if (klen > kMaxLongKey) return fail(c, MRHBM_E_KEY, "key of %zu bytes (limit %zu)", klen, (size_t)kMaxLongKey);
-    LongPair lp;
-    lp.esc.resize(elen);
-    escape(k, klen, (unsigned char*)&lp.esc[0]);
-    lp.value = value;
-    m->long_pairs.push_back(std::move(lp));
-    return MRHBM_OK;
-  }
+  if (elen >= (size_t)c->kb) return long_pair(m, k, klen, elen, value, nullptr, 0);
   unsigned char* slot;
   int rc = stage_slot(m, &slot);
   if (rc) return rc;
@@ -726,18 +709,7 @@ int mrhbm_emit_str_value(mrhbm_map* m, const void* key, size_t klen, const void*
   if (c->cfg.key_kind != MRHBM_KEY_STR) return fail(c, MRHBM_E_INVAL, "ctx holds u64 keys");
   const unsigned char* k = (const unsigned char*)key;
   const size_t elen = esc_size(k, klen);
-  if (elen >= (size_t)c->kb) {  // longer than a record slot: on the host with its value (see mrhbm_emit_str)
-    if (klen > kMaxLongKey) return fail(c, MRHBM_E_KEY, "key of %zu bytes (limit %zu)", klen, (size_t)kMaxLongKey);
-    if (vlen > kMaxValue) return fail(c, MRHBM_E_INVAL, "value of %zu bytes (limit %llu)", vlen, (unsigned long long)kMaxValue);
-    if (vlen && !val) return fail(c, MRHBM_E_INVAL, "null value");
-    LongPair lp;
-    lp.esc.resize(elen);
-    escape(k, klen, (unsigned char*)&lp.esc[0]);
-    lp.value = 0;
-    lp.bytes.assign((const char*)val, vlen);
-    m->long_pairs.push_back(std::move(lp));
-    return MRHBM_OK;
-  }
+  if (elen >= (size_t)c->kb) return long_pair(m, k, klen, elen, 0, val, vlen);
   return stage_value_pair(m, val, vlen, [&](unsigned char* slot) {
     escape(k, klen, slot);
     memset(slot + elen, 0, c->kb - elen);
@@ -765,27 +737,17 @@ int mrhbm_emit_batch_values(mrhbm_map* m, const void* recs, size_t n, const void
                   (unsigned long long)voff[i], (unsigned long long)voff[i + 1], (unsigned long long)kMaxValue);
   const uint64_t bytes = voff[n] - voff[0];
   if (bytes && !vals) return fail(c, MRHBM_E_INVAL, "null values");
-  uint64_t off, aoff;
-  int rc = pool_take(m, n, &off);
+  Reservation r;
+  int rc = reserve(c, m, n, bytes, r);
   if (rc) return rc;
-  rc = arena_reserve(c, bytes, &aoff);
-  if (rc) {
-    c->pool_used = off;
-    return rc;
-  }
-  bool pinned = false;
-  for (const void* p : {recs, vals, (const void*)voff}) {
-    cudaPointerAttributes at{};
-    if (p && cudaPointerGetAttributes(&at, p) == cudaSuccess && at.type == cudaMemoryTypeHost) pinned = true;
-    cudaGetLastError();
-  }
-  CU(c, cudaMemcpyAsync((char*)c->pool + off * c->rb, recs, n * c->rb, cudaMemcpyHostToDevice, c->stream));
-  if (bytes) CU(c, cudaMemcpyAsync(c->arena + aoff, (const char*)vals + voff[0], bytes, cudaMemcpyHostToDevice, c->stream));
-  CU(c, cudaMemcpyAsync(c->voff + off, voff, (n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, c->stream));
-  launch_value_stamp(c->rb, (char*)c->pool + off * c->rb, n, off, c->voff + off, voff[0], aoff, c->stream);
+  const bool pinned = is_pinned(recs) || is_pinned(vals) || is_pinned(voff);
+  CU(c, cudaMemcpyAsync((char*)c->pool + r.off * c->rb, recs, n * c->rb, cudaMemcpyHostToDevice, c->stream));
+  if (bytes) CU(c, cudaMemcpyAsync(c->arena + r.aoff, (const char*)vals + voff[0], bytes, cudaMemcpyHostToDevice, c->stream));
+  CU(c, cudaMemcpyAsync(c->voff + r.off, voff, (n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, c->stream));
+  launch_value_stamp(c->rb, (char*)c->pool + r.off * c->rb, n, r.off, c->voff + r.off, voff[0], r.aoff, c->stream);
   CU(c, cudaGetLastError());
   if (pinned) m->async_reads = true;  // pageable sources are fully staged before the call returns
-  add_range(m, off, n, aoff);
+  r.add(m);
   return MRHBM_OK;
 }
 
@@ -795,15 +757,13 @@ int mrhbm_emit_batch(mrhbm_map* m, const void* recs, size_t n) {
   Entry g(c);
   if (c->bytevals) return refuse_int_values(c);
   if (!n) return MRHBM_OK;
-  uint64_t off;
-  int rc = pool_take(m, n, &off);
+  Reservation r;
+  int rc = reserve(c, m, n, 0, r);
   if (rc) return rc;
-  cudaPointerAttributes at{};
-  bool pinned = cudaPointerGetAttributes(&at, recs) == cudaSuccess && at.type == cudaMemoryTypeHost;
-  cudaGetLastError();
-  CU(c, cudaMemcpyAsync((char*)c->pool + off * c->rb, recs, n * c->rb, cudaMemcpyHostToDevice, c->stream));
+  const bool pinned = is_pinned(recs);
+  CU(c, cudaMemcpyAsync((char*)c->pool + r.off * c->rb, recs, n * c->rb, cudaMemcpyHostToDevice, c->stream));
   if (pinned) m->async_reads = true;  // pageable sources are fully staged before the call returns
-  add_range(m, off, n);
+  r.add(m);
   return MRHBM_OK;
 }
 
@@ -813,11 +773,11 @@ int mrhbm_emit_device(mrhbm_map* m, const void* drecs, size_t n) {
   Entry g(c);
   if (c->bytevals) return refuse_int_values(c);
   if (!n) return MRHBM_OK;
-  uint64_t off;
-  int rc = pool_take(m, n, &off);
+  Reservation r;
+  int rc = reserve(c, m, n, 0, r);
   if (rc) return rc;
-  CU(c, cudaMemcpyAsync((char*)c->pool + off * c->rb, drecs, n * c->rb, cudaMemcpyDeviceToDevice, c->stream));
-  add_range(m, off, n);
+  CU(c, cudaMemcpyAsync((char*)c->pool + r.off * c->rb, drecs, n * c->rb, cudaMemcpyDeviceToDevice, c->stream));
+  r.add(m);
   return MRHBM_OK;
 }
 
@@ -827,12 +787,12 @@ int mrhbm_map_gen_u64(mrhbm_map* m, uint64_t seed, uint64_t start, uint64_t n) {
   Entry g(c);
   if (c->rb != 16) return fail(c, MRHBM_E_INVAL, "gen_u64 needs a u64-key ctx");
   if (c->bytevals) return refuse_int_values(c);
-  uint64_t off;
-  int rc = pool_take(m, n, &off);
+  Reservation r;
+  int rc = reserve(c, m, n, 0, r);
   if (rc) return rc;
-  launch_gen_u64((char*)c->pool + off * c->rb, seed, start, n, c->stream);
+  launch_gen_u64((char*)c->pool + r.off * c->rb, seed, start, n, c->stream);
   CU(c, cudaGetLastError());
-  add_range(m, off, n);
+  r.add(m);
   return MRHBM_OK;
 }
 
@@ -853,12 +813,12 @@ int mrhbm_map_gen_zipf(mrhbm_map* m, uint64_t seed, uint64_t start, uint64_t n, 
     c->d_table_first = table[0];
     c->d_table_last = table[V - 1];
   }
-  uint64_t off;
-  int rc = pool_take(m, n, &off);
+  Reservation r;
+  int rc = reserve(c, m, n, 0, r);
   if (rc) return rc;
-  launch_gen_zipf32((char*)c->pool + off * c->rb, seed, start, n, c->d_table, V, c->stream);
+  launch_gen_zipf32((char*)c->pool + r.off * c->rb, seed, start, n, c->d_table, V, c->stream);
   CU(c, cudaGetLastError());
-  add_range(m, off, n);
+  r.add(m);
   return MRHBM_OK;
 }
 
@@ -892,16 +852,8 @@ int mrhbm_map_wordcount(mrhbm_map* m, const void* text, size_t len, uint64_t* wo
     }
   }
   // undo information: a word that does not fit emits NOTHING of this call
-  const size_t nr0 = c->ranges.size();
-  const uint64_t last_cnt0 = nr0 ? c->ranges.back().cnt : 0, used0 = c->pool_used;
+  const PoolLedger::Mark mark0 = c->led.mark();
   const size_t long0 = m->long_pairs.size();
-  auto undo = [&]() {
-    c->ranges.resize(nr0);
-    if (nr0) c->ranges.back().cnt = last_cnt0;
-    c->pool_used = used0;
-    m->long_pairs.resize(long0);  // (words of a piece that was tokenised on the host)
-    m->fill = 0;                  // the staging buffer was empty when the call began (stage_flush above)
-  };
   auto piece_end = [&](size_t p) -> size_t {  // end of the piece that starts at p: <= kTokPiece bytes, cut after white space
     size_t e = std::min(len, p + kTokPiece);
     if (e < len) {
@@ -935,18 +887,22 @@ int mrhbm_map_wordcount(mrhbm_map* m, const void* text, size_t len, uint64_t* wo
     if ((e = cudaStreamSynchronize(c->stream)) != cudaSuccess) break;
     const uint64_t total = c->h_small[0];
     if (total) {
-      uint64_t off = 0;
-      rc = pool_reserve(c, total, &off);
-      if (rc) break;
-      if ((e = cudaMemsetAsync(flagw, 0, 4, c->stream)) != cudaSuccess) break;
-      launch_tok_emit(c->rb, d_text, n, c->d_tok_off, (char*)c->pool + off * c->rb, flagw, c->stream);
-      if ((e = cudaMemcpyAsync(c->h_small + 1, flagw, 4, cudaMemcpyDeviceToHost, c->stream)) != cudaSuccess) break;
-      if ((e = cudaStreamSynchronize(c->stream)) != cudaSuccess) break;
-      if (c->h_small[1] & ERRF_KEYLEN) {
+      bool fit = false;
+      {
+        Reservation r;
+        rc = reserve(c, nullptr, total, 0, r);
+        if (rc) break;
+        if ((e = cudaMemsetAsync(flagw, 0, 4, c->stream)) != cudaSuccess) break;
+        launch_tok_emit(c->rb, d_text, n, c->d_tok_off, (char*)c->pool + r.off * c->rb, flagw, c->stream);
+        if ((e = cudaMemcpyAsync(c->h_small + 1, flagw, 4, cudaMemcpyDeviceToHost, c->stream)) != cudaSuccess) break;
+        if ((e = cudaStreamSynchronize(c->stream)) != cudaSuccess) break;
+        fit = !(c->h_small[1] & ERRF_KEYLEN);
+        if (fit) r.add(m);
+      }
+      if (!fit) {
         // a word of this piece does not fit the key slot (a URL in a corpus): the piece's records are dropped again and
         // the piece is tokenised on the host -- words that fit are staged like emit_str pairs, the long ones go to the
         // host-side store of long keys.  Rare by assumption: 64 MB take a fraction of a second here.
-        c->pool_used = off;
         uint64_t words_here = 0;
         for (size_t a = p; a < pn && rc == 0;) {
           while (a < pn && is_space(t[a])) a++;
@@ -961,7 +917,6 @@ int mrhbm_map_wordcount(mrhbm_map* m, const void* text, size_t len, uint64_t* wo
         if (rc) break;
         total_words += words_here;
       } else {
-        add_range(m, off, total);
         total_words += total;
       }
     }
@@ -972,7 +927,9 @@ int mrhbm_map_wordcount(mrhbm_map* m, const void* text, size_t len, uint64_t* wo
   if (e != cudaSuccess || rc) {
     cudaStreamSynchronize(c->copy_stream);  // an upload may still be reading the caller's text
     cudaStreamSynchronize(c->stream);
-    undo();
+    c->led.rewind(mark0);
+    m->long_pairs.resize(long0);  // (words of a piece that was tokenised on the host)
+    m->fill = 0;                  // the staging buffer was empty when the call began (stage_flush above)
     if (e != cudaSuccess) {
       cudaGetLastError();
       return fail(c, MRHBM_E_CUDA, "wordcount: %s", cudaGetErrorString(e));
@@ -1057,7 +1014,7 @@ int mrhbm_pool_read(mrhbm_ctx* c, uint64_t first, uint64_t n, void* host_out) {
   if (!c || (!host_out && n)) return MRHBM_E_INVAL;
   Entry g(c);
   uint64_t skip = first, done = 0;
-  for (auto& r : live_ranges(c)) {
+  for (auto& r : c->led.live()) {
     if (done == n) break;
     if (skip >= r.second) {
       skip -= r.second;
@@ -1087,11 +1044,7 @@ int mrhbm_map_commit(mrhbm_map* m) {
     mrhbm_map_abort(m);
     return rc;
   }
-  for (Range& r : c->ranges) {
-    if (r.state == R_COMMITTED && r.job == m->job) r.state = R_DEAD;  // replace-by-job-id
-  }
-  for (Range& r : c->ranges)
-    if (r.owner == m->serial && r.state == R_OPEN) r.state = R_COMMITTED;
+  c->led.commit(m->serial, m->job);
   c->long_jobs.erase(m->job);  // replace-by-job-id on the host side too
   if (!m->long_pairs.empty()) c->long_jobs[m->job] = std::move(m->long_pairs);
   invalidate(c);
@@ -1103,24 +1056,15 @@ void mrhbm_map_abort(mrhbm_map* m) {
   if (!m) return;
   mrhbm_ctx* c = m->ctx;
   Entry g(c);
-  cudaStreamSynchronize(c->stream);
-  for (Range& r : c->ranges)
-    if (r.owner == m->serial && r.state == R_OPEN) r.state = R_DEAD;
-  while (!c->ranges.empty() && c->ranges.back().state == R_DEAD &&
-         c->ranges.back().off + c->ranges.back().cnt == c->pool_used) {
-    c->pool_used = c->ranges.back().off;
-    if (c->bytevals) c->arena_used = c->ranges.back().aoff;
-    c->ranges.pop_back();
-  }
+  cudaStreamSynchronize(c->stream);  // (copies into the room that goes back)
+  c->led.abort(m->serial);
   map_release(m);
 }
 
 int mrhbm_reset(mrhbm_ctx* c) {
   if (!c) return MRHBM_E_INVAL;
   Entry g(c);
-  c->ranges.clear();
-  c->pool_used = 0;
-  c->arena_used = 0;
+  c->led.reset();
   c->long_jobs.clear();
   invalidate(c);
   return MRHBM_OK;
@@ -1292,7 +1236,7 @@ constexpr uint32_t kGtabMaxExtra = 5;   // ... grown up to 32x (1 GB) when the k
 int collect_sources(mrhbm_ctx* c, std::vector<Src>& srcs, uint64_t* N, mrhbm_stats& st) {
   srcs.clear();
   uint64_t n = 0;
-  for (auto& r : live_ranges(c)) {
+  for (auto& r : c->led.live()) {
     srcs.push_back(Src{(const char*)c->pool + r.first * c->rb, r.second});
     n += r.second;
   }
@@ -2035,11 +1979,10 @@ extern "C" {
 int mrhbm_shuffle(mrhbm_ctx* c) {
   if (!c || !c->stream) return MRHBM_E_INVAL;
   Entry g(c);
-  for (const Range& r : c->ranges)
-    if (r.state == R_OPEN) return fail(c, MRHBM_E_INVAL, "map job '%s' is still open", r.job.c_str());
+  if (const std::string* job = c->led.open_job()) return fail(c, MRHBM_E_INVAL, "map job '%s' is still open", job->c_str());
   invalidate(c);
   uint64_t N_in = 0, N = 0;
-  for (auto& r : live_ranges(c)) N_in += r.second;
+  for (auto& r : c->led.live()) N_in += r.second;
   if (N_in >= 0xfffffff0ull) return fail(c, MRHBM_E_INVAL, "more than 2^32 pairs on one GPU (%llu)", (unsigned long long)N_in);
   if (c->cfg.partitioner == MRHBM_PART_RANGE && c->world == 1 && !c->spl_set)  // (several GPUs: at the first all-gather)
     return fail(c, MRHBM_E_INVAL, "MRHBM_PART_RANGE needs splitters: call mrhbm_set_splitters or mrhbm_sample_splitters");
@@ -2078,7 +2021,7 @@ int mrhbm_sample_splitters(mrhbm_ctx* c, void* keys, size_t cap, uint64_t* off, 
   if (c->cfg.partitioner != MRHBM_PART_RANGE) return fail(c, MRHBM_E_INVAL, "splitters need partitioner MRHBM_PART_RANGE");
   const int G = c->world, me = c->rank;
   const uint32_t P = c->cfg.num_partitions, KW = (uint32_t)c->kb / 4;
-  const auto live = live_ranges(c);
+  const auto live = c->led.live();
   uint64_t N = 0;
   for (auto& r : live) N += r.second;
   // every rank's share of the sample follows its committed pairs (the same arithmetic on every rank)
@@ -2237,7 +2180,7 @@ int mrhbm_checksum_input(mrhbm_ctx* c, uint64_t in[4]) {
   if (!c || !in) return MRHBM_E_INVAL;
   Entry g(c);
   CU(c, cudaMemsetAsync(c->d_acc, 0, 8 * sizeof(uint64_t), c->stream));
-  for (auto& r : live_ranges(c)) launch_checksum_in(c->rb, (char*)c->pool + r.first * c->rb, r.second, c->d_acc, c->stream);
+  for (auto& r : c->led.live()) launch_checksum_in(c->rb, (char*)c->pool + r.first * c->rb, r.second, c->d_acc, c->stream);
   CU(c, cudaGetLastError());
   CU(c, cudaMemcpyAsync(c->h_acc, c->d_acc, 8 * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream));
   CU(c, cudaStreamSynchronize(c->stream));

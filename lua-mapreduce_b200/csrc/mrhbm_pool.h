@@ -1,0 +1,124 @@
+// mrhbm_pool.h -- the ledger of the HBM emit pool: which records belong to which map job, and how much of the pool
+// and of the value arena is in use (no CUDA runtime calls, no ctx; the memory itself and its growth are the ctx's).
+//
+// The pool is filled from its tail.  A map handle (an owner) takes room, fills it and adds it as an open range of its
+// job.  Commit makes the owner's open ranges the job's output and kills what an earlier commit of the same job id left
+// (replace-by-job-id, mapreduce/job.lua:217-221); abort kills the owner's open ranges (worker.lua:120-127).  What the
+// ledger keeps:
+//   - ranges are in pool order and never overlap; every record below used() that no range covers is lost room, so
+//     room that is taken is either added or rewound;
+//   - MRHBM_F_BYTE_VALUES: a pair's value id is its pool index and values are appended to the arena in pool order,
+//     so room in both is taken together (voff[used()] == arena_used() always) and goes back together: a range
+//     remembers the arena offset of its first value;
+//   - dead ranges at the tail give their room back when an abort finds them there; dead ranges with live or open
+//     records behind them keep their room (records and value bytes) until reset().
+#pragma once
+#include <cassert>
+#include <cstdint>
+#include <string>
+#include <utility>
+#include <vector>
+
+namespace mrhbm {
+
+class PoolLedger {
+ public:
+  struct Mark {
+    size_t ranges;
+    uint64_t last_cnt, used, arena_used;
+  };
+  struct Room {
+    uint64_t off, aoff;  // the first record, the first value byte
+  };
+
+  bool byte_values = false;  // value ids are u32 in string records: fewer than 2^32 - 1 pairs between resets
+
+  uint64_t used() const { return used_; }
+  uint64_t arena_used() const { return arena_used_; }
+  uint64_t new_owner() { return ++owners_; }
+
+  // rewind(mark()) undoes every take and add since the mark (no commit, abort or reset may lie between)
+  Mark mark() const { return Mark{ranges_.size(), ranges_.empty() ? 0 : ranges_.back().cnt, used_, arena_used_}; }
+  void rewind(const Mark& mk) {
+    assert(mk.ranges <= ranges_.size() && mk.used <= used_ && mk.arena_used <= arena_used_);
+    ranges_.erase(ranges_.begin() + (ptrdiff_t)mk.ranges, ranges_.end());
+    if (mk.ranges) ranges_.back().cnt = mk.last_cnt;
+    used_ = mk.used;
+    arena_used_ = mk.arena_used;
+  }
+
+  bool fits(uint64_t n) const { return !byte_values || used_ + n < 0xffffffffull; }
+  // n records and `bytes` value bytes at the tail; needs fits(n)
+  Room take(uint64_t n, uint64_t bytes) {
+    assert(fits(n));
+    const Room r{used_, arena_used_};
+    used_ += n;
+    arena_used_ += bytes;
+    return r;
+  }
+  // taken room becomes an open range of the owner's, one with the range it continues
+  void add(uint64_t owner, const std::string& job, uint64_t off, uint64_t cnt, uint64_t aoff) {
+    if (!ranges_.empty()) {
+      Range& r = ranges_.back();
+      if (r.owner == owner && r.state == OPEN && r.off + r.cnt == off) {
+        r.cnt += cnt;
+        return;
+      }
+    }
+    ranges_.push_back(Range{off, cnt, job, OPEN, owner, aoff});
+  }
+
+  void commit(uint64_t owner, const std::string& job) {
+    for (Range& r : ranges_)
+      if (r.state == COMMITTED && r.job == job) r.state = DEAD;  // replace-by-job-id
+    for (Range& r : ranges_)
+      if (r.owner == owner && r.state == OPEN) r.state = COMMITTED;
+  }
+  // (the caller has waited for the copies into the owner's ranges: their room may be handed out again)
+  void abort(uint64_t owner) {
+    for (Range& r : ranges_)
+      if (r.owner == owner && r.state == OPEN) r.state = DEAD;
+    while (!ranges_.empty() && ranges_.back().state == DEAD && ranges_.back().off + ranges_.back().cnt == used_) {
+      used_ = ranges_.back().off;
+      arena_used_ = ranges_.back().aoff;
+      ranges_.pop_back();
+    }
+  }
+  void reset() {
+    ranges_.clear();
+    used_ = arena_used_ = 0;
+  }
+
+  // committed records as (first, count), adjacent ranges merged
+  std::vector<std::pair<uint64_t, uint64_t>> live() const {
+    std::vector<std::pair<uint64_t, uint64_t>> v;
+    for (const Range& r : ranges_) {
+      if (r.state != COMMITTED || !r.cnt) continue;
+      if (!v.empty() && v.back().first + v.back().second == r.off)
+        v.back().second += r.cnt;
+      else
+        v.emplace_back(r.off, r.cnt);
+    }
+    return v;
+  }
+  // the job of some range that is still open, or null
+  const std::string* open_job() const {
+    for (const Range& r : ranges_)
+      if (r.state == OPEN) return &r.job;
+    return nullptr;
+  }
+
+ private:
+  enum { OPEN, COMMITTED, DEAD };
+  struct Range {
+    uint64_t off, cnt;
+    std::string job;
+    int state;
+    uint64_t owner;  // map handle serial
+    uint64_t aoff;   // the arena offset of the range's first value (its bytes follow in pool order)
+  };
+  std::vector<Range> ranges_;
+  uint64_t used_ = 0, arena_used_ = 0, owners_ = 0;
+};
+
+}  // namespace mrhbm
