@@ -96,11 +96,13 @@ typedef struct mrhbm_config {
 /* Byte-string values (lua-mapreduce's emit(key, value) takes any Lua string or number, utils.lua:100-120): a value is
  * opaque bytes, 0 to 1 GiB long, carried through group-only mode.  Needs reducer = MRHBM_RED_NONE and combiner = 0
  * (else mrhbm_init fails with MRHBM_E_INVAL) and one GPU (mrhbm_comm_init with world > 1 fails).  On such a ctx:
- *   - pairs are emitted with mrhbm_emit_str_value / mrhbm_emit_u64_value / mrhbm_emit_batch_values; the integer-valued
- *     emits (emit_str, emit_u64, emit_batch, emit_device, map_gen_*, map_wordcount) fail with MRHBM_E_INVAL;
+ *   - pairs are emitted with mrhbm_emit_str_value / mrhbm_emit_u64_value / mrhbm_emit_batch_values /
+ *     mrhbm_map_words_value; the integer-valued emits (emit_str, emit_u64, emit_batch, emit_device, map_gen_*,
+ *     map_wordcount) fail with MRHBM_E_INVAL;
  *   - groups are read with mrhbm_groups_next_values (mrhbm_groups_next fails) and rows with mrhbm_result_values;
  *     mrhbm_result_copy needs sums = NULL;
- *   - the value field of a record (pool_read, result_copy) holds the pair's value id, its index in the emit pool;
+ *   - the value field of a record (pool_read, result_copy) holds the pair's value id, its index in the emit pool,
+ *     except that the pairs of one device piece of mrhbm_map_words_value share the id of the piece's first pair;
  *     fewer than 2^32 pairs may be emitted between mrhbm_reset calls, those of aborted and replaced jobs included.
  * The order of a key's values is unspecified, as for MRHBM_RED_NONE.  The new calls fail with MRHBM_E_INVAL on a ctx
  * without the flag. */
@@ -174,6 +176,12 @@ int mrhbm_emit_u64_value(mrhbm_map *, uint64_t key, const void *val, size_t vlen
  * vals[voff[i] .. voff[i+1]) (voff has n + 1 non-decreasing entries).  Pinned and pageable memory as for
  * mrhbm_emit_batch: all three buffers are pinned-or-pageable independently. */
 int mrhbm_emit_batch_values(mrhbm_map *, const void *records, size_t n, const void *vals, const uint64_t *voff);
+/* MRHBM_F_BYTE_VALUES: the device tokeniser of mrhbm_map_wordcount (same word rule, same pieces, same host fall-back
+ * for words longer than the record class, same "nothing of a failed call is emitted"), emitting (word, val[0 .. vlen))
+ * for every word instead of (word, 1): an inverted index's map job (examples/WordCount/mapfn.lua:3-9 with the file
+ * name as the value).  val is copied before return (vlen <= 1 GiB, 0 allowed).  *words (optional) receives the token
+ * count.  String-key ctx only. */
+int mrhbm_map_words_value(mrhbm_map *, const void *text, size_t len, const void *val, size_t vlen, uint64_t *words);
 
 /* ---- barrier between MAP and REDUCE (server.lua:279-329) ---- */
 /* hash-partition [+ NCCL all-to-all] + sort + segmented reduce of everything committed */

@@ -822,13 +822,17 @@ int mrhbm_map_gen_zipf(mrhbm_map* m, uint64_t seed, uint64_t start, uint64_t n, 
   return MRHBM_OK;
 }
 
-int mrhbm_map_wordcount(mrhbm_map* m, const void* text, size_t len, uint64_t* words) {
-  if (!m || (!text && len)) return MRHBM_E_INVAL;
+}  // extern "C"
+
+namespace {
+
+// The device tokeniser of mrhbm_map_wordcount and mrhbm_map_words_value (the caller has checked the ctx and the
+// arguments): every maximal run of non-space bytes of the text becomes the pair (word, 1), or on a byte-values ctx
+// (word, val[0 .. vlen)).  With byte values the value bytes go to the arena once per device piece and every pair of
+// the piece carries the value id of the piece's first pair (see PoolLedger).
+int map_words(mrhbm_map* m, const unsigned char* t, size_t len, const void* val, size_t vlen, uint64_t* words) {
   mrhbm_ctx* c = m->ctx;
-  Entry g(c);
-  if (words) *words = 0;
-  if (c->cfg.key_kind != MRHBM_KEY_STR) return fail(c, MRHBM_E_INVAL, "wordcount needs a string-key ctx");
-  if (c->bytevals) return refuse_int_values(c);
+  const char* what = c->bytevals ? "words_value" : "wordcount";
   if (!len) return MRHBM_OK;
   int rc = stage_flush(m);
   if (rc) return rc;
@@ -836,7 +840,6 @@ int mrhbm_map_wordcount(mrhbm_map* m, const void* text, size_t len, uint64_t* wo
   // upload of piece k+1 (copy stream) runs while piece k is counted, scanned and emitted (ctx stream).  The scratch
   // (text x 2, per-256-byte-block word counts and offsets) lives with the ctx.
   constexpr size_t kTokPiece = 64u << 20;
-  const unsigned char* t = (const unsigned char*)text;
   auto is_space = [](unsigned char ch) { return ch == ' ' || (ch >= 9 && ch <= 13); };
   if (!c->d_tok_text[0]) {
     const uint64_t tcap = kTokPiece + 4096, bcap = tok_blocks(tcap) + 1;
@@ -848,7 +851,7 @@ int mrhbm_map_wordcount(mrhbm_map* m, const void* text, size_t len, uint64_t* wo
     for (int i = 0; i < 2 && ea == cudaSuccess; i++) ea = cudaEventCreateWithFlags(&c->tok_ev[i], cudaEventDisableTiming);
     if (ea != cudaSuccess) {
       cudaGetLastError();
-      return fail(c, MRHBM_E_NOMEM, "wordcount: %s", cudaGetErrorString(ea));
+      return fail(c, MRHBM_E_NOMEM, "%s: %s", what, cudaGetErrorString(ea));
     }
   }
   // undo information: a word that does not fit emits NOTHING of this call
@@ -890,10 +893,17 @@ int mrhbm_map_wordcount(mrhbm_map* m, const void* text, size_t len, uint64_t* wo
       bool fit = false;
       {
         Reservation r;
-        rc = reserve(c, nullptr, total, 0, r);
+        rc = reserve(c, nullptr, total, c->bytevals ? vlen : 0, r);
         if (rc) break;
+        uint32_t value = 1;
+        if (c->bytevals) {  // one copy of the value; ids r.off + 1 .. r.off + total - 1 get empty values
+          if (vlen && (e = cudaMemcpyAsync(c->arena + r.aoff, val, vlen, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess)
+            break;
+          launch_value_stamp(c->rb, nullptr, total, 0, c->voff + r.off, vlen, r.aoff, c->stream);
+          value = (uint32_t)r.off;
+        }
         if ((e = cudaMemsetAsync(flagw, 0, 4, c->stream)) != cudaSuccess) break;
-        launch_tok_emit(c->rb, d_text, n, c->d_tok_off, (char*)c->pool + r.off * c->rb, flagw, c->stream);
+        launch_tok_emit(c->rb, d_text, n, c->d_tok_off, (char*)c->pool + r.off * c->rb, value, flagw, c->stream);
         if ((e = cudaMemcpyAsync(c->h_small + 1, flagw, 4, cudaMemcpyDeviceToHost, c->stream)) != cudaSuccess) break;
         if ((e = cudaStreamSynchronize(c->stream)) != cudaSuccess) break;
         fit = !(c->h_small[1] & ERRF_KEYLEN);
@@ -901,15 +911,15 @@ int mrhbm_map_wordcount(mrhbm_map* m, const void* text, size_t len, uint64_t* wo
       }
       if (!fit) {
         // a word of this piece does not fit the key slot (a URL in a corpus): the piece's records are dropped again and
-        // the piece is tokenised on the host -- words that fit are staged like emit_str pairs, the long ones go to the
-        // host-side store of long keys.  Rare by assumption: 64 MB take a fraction of a second here.
+        // the piece is tokenised on the host -- words that fit are staged like emit_str / emit_str_value pairs, the
+        // long ones go to the host-side store of long keys.  Rare by assumption: 64 MB take a fraction of a second here.
         uint64_t words_here = 0;
         for (size_t a = p; a < pn && rc == 0;) {
           while (a < pn && is_space(t[a])) a++;
           size_t b = a;
           while (b < pn && !is_space(t[b])) b++;
           if (b > a) {
-            rc = mrhbm_emit_str(m, t + a, b - a, 1u);
+            rc = c->bytevals ? mrhbm_emit_str_value(m, t + a, b - a, val, vlen) : mrhbm_emit_str(m, t + a, b - a, 1u);
             words_here++;
           }
           a = b;
@@ -932,12 +942,38 @@ int mrhbm_map_wordcount(mrhbm_map* m, const void* text, size_t len, uint64_t* wo
     m->fill = 0;                  // the staging buffer was empty when the call began (stage_flush above)
     if (e != cudaSuccess) {
       cudaGetLastError();
-      return fail(c, MRHBM_E_CUDA, "wordcount: %s", cudaGetErrorString(e));
+      return fail(c, MRHBM_E_CUDA, "%s: %s", what, cudaGetErrorString(e));
     }
     return rc;
   }
   if (words) *words = total_words;
   return MRHBM_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int mrhbm_map_wordcount(mrhbm_map* m, const void* text, size_t len, uint64_t* words) {
+  if (!m || (!text && len)) return MRHBM_E_INVAL;
+  mrhbm_ctx* c = m->ctx;
+  Entry g(c);
+  if (words) *words = 0;
+  if (c->cfg.key_kind != MRHBM_KEY_STR) return fail(c, MRHBM_E_INVAL, "wordcount needs a string-key ctx");
+  if (c->bytevals) return refuse_int_values(c);
+  return map_words(m, (const unsigned char*)text, len, nullptr, 0, words);
+}
+
+int mrhbm_map_words_value(mrhbm_map* m, const void* text, size_t len, const void* val, size_t vlen, uint64_t* words) {
+  if (!m || (!text && len)) return MRHBM_E_INVAL;
+  mrhbm_ctx* c = m->ctx;
+  Entry g(c);
+  if (words) *words = 0;
+  if (!c->bytevals) return refuse_byte_values(c);
+  if (c->cfg.key_kind != MRHBM_KEY_STR) return fail(c, MRHBM_E_INVAL, "words_value needs a string-key ctx");
+  int rc = check_value(c, val, vlen);
+  if (rc) return rc;
+  return map_words(m, (const unsigned char*)text, len, val, vlen, words);
 }
 
 // ---- synthetic word-count text (SURVEY App. B), host side: the input of the end-to-end word-count measurements

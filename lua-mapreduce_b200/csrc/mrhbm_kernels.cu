@@ -99,7 +99,7 @@ __global__ void __launch_bounds__(256) k_tok_count(const unsigned char* __restri
 template <int RB>
 __global__ void __launch_bounds__(256) k_tok_emit(const unsigned char* __restrict__ t, uint64_t len,
                                                   const uint32_t* __restrict__ block_off, uint4* __restrict__ recs,
-                                                  uint32_t* __restrict__ flags) {
+                                                  uint32_t value, uint32_t* __restrict__ flags) {
   constexpr int KB = Rec<RB>::kKeyBytes;
   __shared__ uint32_t wcount[8];
   uint64_t nb = (len + 255) / 256;
@@ -138,8 +138,7 @@ __global__ void __launch_bounds__(256) k_tok_emit(const unsigned char* __restric
       l = KB - 1;
       rec.b[KB - 1] = 0;
     }
-    uint32_t one = 1u;
-    rec.b[KB] = (unsigned char)one;  // little-endian u32 value 1 (remaining value bytes are zero)
+    rec.v[RB / 16 - 1].w = value;  // the u32 value field, bytes KB .. RB - 1
     uint4* d = recs + ((uint64_t)block_off[blk] + before) * (RB / 16);
 #pragma unroll
     for (int v = 0; v < RB / 16; v++) d[v] = rec.v[v];
@@ -1451,14 +1450,14 @@ int launch_tok_count(const unsigned char* text, uint64_t len, uint32_t* block_co
   return 1;
 }
 int launch_tok_emit(int rb, const unsigned char* text, uint64_t len, const uint32_t* block_off, void* recs,
-                    uint32_t* flags, cudaStream_t s) {
+                    uint32_t value, uint32_t* flags, cudaStream_t s) {
   if (!len || rb == 16) return 0;
   uint64_t nb = (len + 255) / 256;
   int grid = (int)std::min<uint64_t>(nb, (uint64_t)g_sm_count * 16);
   switch (rb) {
-    case 32: k_tok_emit<32><<<grid, 256, 0, s>>>(text, len, block_off, (uint4*)recs, flags); break;
-    case 64: k_tok_emit<64><<<grid, 256, 0, s>>>(text, len, block_off, (uint4*)recs, flags); break;
-    default: k_tok_emit<128><<<grid, 256, 0, s>>>(text, len, block_off, (uint4*)recs, flags); break;
+    case 32: k_tok_emit<32><<<grid, 256, 0, s>>>(text, len, block_off, (uint4*)recs, value, flags); break;
+    case 64: k_tok_emit<64><<<grid, 256, 0, s>>>(text, len, block_off, (uint4*)recs, value, flags); break;
+    default: k_tok_emit<128><<<grid, 256, 0, s>>>(text, len, block_off, (uint4*)recs, value, flags); break;
   }
   return 1;
 }

@@ -117,10 +117,10 @@ int launch_sample_keys(int rb, const void* recs, uint64_t n, uint32_t nsample, u
 int launch_scatter(int rb, const void* recs, uint64_t n, const RangeBinParams& bp, uint32_t* cursor, void* mid,
                    cudaStream_t s);
 // device-side tokeniser: word starts per 256-byte block, then (after an exclusive scan of the
-// block counts) one record per word; *flags gets ERRF_KEYLEN when a word exceeds the key slot
+// block counts) one record (word, value) per word; *flags gets ERRF_KEYLEN when a word exceeds the key slot
 int launch_tok_count(const unsigned char* text, uint64_t len, uint32_t* block_counts, cudaStream_t s);
 int launch_tok_emit(int rb, const unsigned char* text, uint64_t len, const uint32_t* block_off, void* recs,
-                    uint32_t* flags, cudaStream_t s);
+                    uint32_t value, uint32_t* flags, cudaStream_t s);
 inline uint64_t tok_blocks(uint64_t len) { return (len + 255) / 256; }
 // The map-side combiner's global table for records of rb bytes: 2^glog short entries of 16 bytes, then, for string
 // records only, 2^(glog-4) long entries of one record each.  The compaction emits at most one record per entry.
@@ -209,7 +209,8 @@ inline uint64_t val_tiles(uint64_t rows) { return (rows + (1u << kValTileLog) - 
 // most pieces of the values longer than kValChunk that `bytes` value bytes can hold
 inline uint64_t val_chunks_cap(uint64_t bytes) { return 2 * (bytes / kValChunk) + 1; }
 // records [0, n) of the rb-byte records at recs get value id first + i; dvoff[i] (i <= n, the caller's offsets as
-// copied) becomes dvoff[i] - v0 + aoff, an offset into the arena
+// copied) becomes dvoff[i] - v0 + aoff, an offset into the arena.  recs == nullptr: the n pairs of a tokeniser piece
+// share one value of v0 bytes at aoff: dvoff[0] = aoff and dvoff[1 .. n] = aoff + v0 (first is unused)
 int launch_value_stamp(int rb, void* recs, uint64_t n, uint64_t first, uint64_t* dvoff, uint64_t v0, uint64_t aoff,
                        cudaStream_t s);
 // row_off[r] for rows r < n whose value id is ids[r]: value bytes of the rows before r inside its scan tile;

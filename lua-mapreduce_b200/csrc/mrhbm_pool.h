@@ -9,7 +9,8 @@
 //     room that is taken is either added or rewound;
 //   - MRHBM_F_BYTE_VALUES: a pair's value id is its pool index and values are appended to the arena in pool order,
 //     so room in both is taken together (voff[used()] == arena_used() always) and goes back together: a range
-//     remembers the arena offset of its first value;
+//     remembers the arena offset of its first value.  The pairs of one tokeniser piece (mrhbm_map_words_value)
+//     share the id of the piece's first pair, which holds the value; the other ids of the piece hold empty values;
 //   - dead ranges at the tail give their room back when an abort finds them there; dead ranges with live or open
 //     records behind them keep their room (records and value bytes) until reset().
 #pragma once

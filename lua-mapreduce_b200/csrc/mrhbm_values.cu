@@ -1,6 +1,7 @@
-// mrhbm_values.cu -- byte values (MRHBM_F_BYTE_VALUES): the map-side stamp of value ids and, after the compaction of
-// a group-only result, the per-row value lengths, their u64 exclusive scan and the gather of the value bytes from the
-// arena into one buffer in row order.  The split, sort and compaction kernels carry the value id unchanged.
+// mrhbm_values.cu -- byte values (MRHBM_F_BYTE_VALUES): the map-side stamp of value ids (or of the offsets of a
+// tokeniser piece's shared value) and, after the compaction of a group-only result, the per-row value lengths, their
+// u64 exclusive scan and the gather of the value bytes from the arena into one buffer in row order.  The split, sort
+// and compaction kernels carry the value id unchanged.
 #include <cstdint>
 
 #include "mrhbm_dev.cuh"
@@ -26,6 +27,10 @@ __global__ void __launch_bounds__(256) k_value_stamp(unsigned char* __restrict__
                                                      uint64_t* __restrict__ dvoff, uint64_t v0, uint64_t aoff) {
   const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i <= n; i += stride) {
+    if (!recs) {  // one shared value (mrhbm_map_words_value), v0 its length
+      dvoff[i] = i ? aoff + v0 : aoff;
+      continue;
+    }
     dvoff[i] = dvoff[i] - v0 + aoff;
     if (i == n) continue;
     if (rb == 16)

@@ -250,7 +250,13 @@ function hbm.map_job(map_key)
   local finish = function(ok)
     if ok then assert(m:commit()) else m:abort() end -- BROKEN jobs publish nothing
   end
-  return emit, finish
+  -- a mapfn module declaring hbm_mapfn = "words_file" (value_kind = "bytes"): the device tokenises the file's bytes
+  -- and pairs every word with the job value, the file name -- emit(word, value) per token, as an inverted index does
+  local words = function(text, value)
+    assert(byte_values, "hbm_mapfn = 'words_file' needs value_kind = 'bytes'")
+    return assert(m:words_value(text, hbm.encode_value(value)))
+  end
+  return emit, finish, words
 end
 
 -- server_prepare_reduce (server.lua:279-329)

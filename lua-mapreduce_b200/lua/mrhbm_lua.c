@@ -179,6 +179,18 @@ static int map_wordcount(lua_State *L) {
   lua_pushnumber(L, (lua_Number)n);
   return 1;
 }
+/* map:words_value(text, value) -> number of words, with values = "bytes": the same tokeniser emitting (word, value)
+ * for every word (an inverted index's mapfn), value is a Lua string (copied before return) */
+static int map_words_value(lua_State *L) {
+  lmap *m = (lmap *)luaL_checkudata(L, 1, MAP_MT);
+  size_t len, vlen;
+  const char *t = luaL_checklstring(L, 2, &len);
+  const char *v = luaL_checklstring(L, 3, &vlen);
+  uint64_t n = 0;
+  if (!m->h || mrhbm_map_words_value(m->h, t, len, v, vlen, &n) != MRHBM_OK) return fail(L, m->ctx);
+  lua_pushnumber(L, (lua_Number)n);
+  return 1;
+}
 static int map_commit(lua_State *L) { /* job.lua:217-221: remove_file + build */
   lmap *m = (lmap *)luaL_checkudata(L, 1, MAP_MT);
   mrhbm_map *h = m->h;
@@ -306,7 +318,8 @@ static const luaL_Reg ctx_methods[] = {{"map_begin", ctx_map_begin}, {"shuffle",
                                        {"partitions", ctx_partitions}, {"groups", ctx_groups},
                                        {"reset", ctx_reset}, {"set_splitters", ctx_set_splitters},
                                        {"sample_splitters", ctx_sample_splitters}, {"__gc", ctx_gc}, {NULL, NULL}};
-static const luaL_Reg map_methods[] = {{"emit", map_emit}, {"wordcount", map_wordcount}, {"commit", map_commit},
+static const luaL_Reg map_methods[] = {{"emit", map_emit}, {"wordcount", map_wordcount},
+                                       {"words_value", map_words_value}, {"commit", map_commit},
                                        {"abort", map_abort}, {"__gc", map_abort}, {NULL, NULL}};
 static const luaL_Reg mod_funcs[] = {{"new", l_new}, {NULL, NULL}};
 

@@ -57,11 +57,17 @@ class Job:
         mapfn = mod.mapfn
         m = ctx.map_begin(self.get_id())
         try:
-            if getattr(mod, "hbm_mapfn", None) == "wordcount_file" and hasattr(m, "wordcount"):
+            hbm_mapfn = getattr(mod, "hbm_mapfn", None)
+            if hbm_mapfn == "wordcount_file" and hasattr(m, "wordcount"):
                 # declared built-in (same opt-in pattern as hbm_reducefn): the job value is a file
                 # path, the device tokenises its bytes exactly like examples/WordCount/mapfn.lua:3-9
                 with open(self.doc["value"], "rb") as fh:
                     m.wordcount(fh.read())
+                mapfn = None
+            elif hbm_mapfn == "words_file" and hasattr(m, "words_value"):
+                # the same tokeniser pairing every word with the job value (the file path): an inverted index
+                with open(self.doc["value"], "rb") as fh:
+                    m.words_value(fh.read(), tuple_keys.encode_value(self.doc["value"]))
                 mapfn = None
             kind = cfg["hbm"]["key_kind"]
             if kind == "u64":

@@ -106,6 +106,9 @@ class server:
         if hbm["value_kind"] == "bytes" and builtin_red is not None:
             raise ValueError("hbm value_kind = 'bytes' hands string and number values to a general reducefn: "
                              "the reducefn module must not declare hbm_reducefn (it declares %r)" % (builtin_red,))
+        if getattr(mods["mapfn"], "hbm_mapfn", None) == "words_file" and hbm["value_kind"] != "bytes":
+            raise ValueError("hbm_mapfn = 'words_file' pairs every word with the file name, a string value: "
+                             "configure hbm = {'value_kind': 'bytes'}")
         hbm.update(partitioner=_BUILTIN_PART[pname], num_partitions=nparts, combiner=device_combiner,
                    reducer=0 if builtin_red == "sum" else 1,
                    splitters=range_splitters(part, nparts, hbm["key_kind"]) if pname == "range" else None)

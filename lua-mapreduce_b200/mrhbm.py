@@ -57,7 +57,7 @@ EXPORTS = [
     "mrhbm_groups_close", "mrhbm_result_info_get", "mrhbm_result_copy", "mrhbm_checksum_input",
     "mrhbm_checksum_result", "mrhbm_stats_get", "mrhbm_reset", "mrhbm_comm_unique_id", "mrhbm_comm_init",
     "mrhbm_set_splitters", "mrhbm_sample_splitters", "mrhbm_emit_str_value", "mrhbm_emit_u64_value",
-    "mrhbm_emit_batch_values", "mrhbm_groups_next_values", "mrhbm_result_values",
+    "mrhbm_emit_batch_values", "mrhbm_groups_next_values", "mrhbm_result_values", "mrhbm_map_words_value",
 ]
 
 _lib = None
@@ -124,6 +124,7 @@ def load(build_if_missing=True):
     sig("mrhbm_emit_batch_values", i, vp, vp, sz, vp, vp)
     sig("mrhbm_groups_next_values", i, vp, C.POINTER(vp), C.POINTER(sz), C.POINTER(vp), C.POINTER(vp), C.POINTER(sz))
     sig("mrhbm_result_values", i, vp, vp, sz, vp, C.POINTER(sz))
+    sig("mrhbm_map_words_value", i, vp, vp, sz, C.c_char_p, sz, C.POINTER(u64))
     _lib = L
     return L
 
@@ -223,18 +224,33 @@ class Map:
         t = np.ascontiguousarray(table, dtype=np.uint64)
         self.ctx._chk(self.ctx.L.mrhbm_map_gen_zipf(self.h, seed, start, n, t.ctypes.data, t.size))
 
+    @staticmethod
+    def _text(text, nbytes):
+        """(address, bytes, object that keeps the memory alive) of a text buffer"""
+        if isinstance(text, (bytes, bytearray)):
+            keep = C.create_string_buffer(bytes(text), len(text)) if isinstance(text, bytearray) else text
+            return C.cast(C.c_char_p(keep), C.c_void_p), len(text), keep
+        if isinstance(text, np.ndarray):
+            return C.c_void_p(text.ctypes.data), text.nbytes, text
+        return C.c_void_p(int(text)), nbytes, None
+
     def wordcount(self, text, nbytes=None):
         """device-side WordCount mapfn over a text buffer (bytes, a uint8 numpy array, or an address with
         nbytes); returns the number of words emitted"""
         n = C.c_uint64()
-        if isinstance(text, (bytes, bytearray)):
-            keep = C.create_string_buffer(bytes(text), len(text)) if isinstance(text, bytearray) else text
-            ptr, nbytes = C.cast(C.c_char_p(keep), C.c_void_p), len(text)
-        elif isinstance(text, np.ndarray):
-            ptr, nbytes = C.c_void_p(text.ctypes.data), text.nbytes
-        else:
-            ptr = C.c_void_p(int(text))
+        ptr, nbytes, keep = self._text(text, nbytes)
         self.ctx._chk(self.ctx.L.mrhbm_map_wordcount(self.h, ptr, nbytes, C.byref(n)))
+        return n.value
+
+    def words_value(self, text, value, nbytes=None):
+        """F_BYTE_VALUES: the device tokeniser of wordcount emitting (word, value) for every word of the text (text
+        as for wordcount, value bytes); returns the number of words emitted"""
+        if not isinstance(value, (bytes, bytearray)):
+            raise MrhbmError(-1, "words_value takes a bytes value, got %r" % type(value).__name__)
+        v = bytes(value)
+        n = C.c_uint64()
+        ptr, nbytes, keep = self._text(text, nbytes)
+        self.ctx._chk(self.ctx.L.mrhbm_map_words_value(self.h, ptr, nbytes, v, len(v), C.byref(n)))
         return n.value
 
     def commit(self):
