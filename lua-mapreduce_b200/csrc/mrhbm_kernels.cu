@@ -710,7 +710,21 @@ __global__ void __launch_bounds__(1024) k_exscan_rows(const uint32_t* __restrict
 // the combiner; a u32 sum about to wrap raises ERRF_OVERFLOW (string records carry u32 values), and the host then
 // hands the raw pairs on, whose sums the sort / reduce stages keep in u64.
 constexpr int kCombineThreads = 1024;
-constexpr int kCombineSmem = 188 * 1024;  // (+ 38 KB of per-warp miss queues = 226 of the 227 KB)
+// Warp roles (see k_combine): the first kCombineStreamWarps warps stream the pairs, the last kCombineTableWarps
+// warps alone talk to the global table.
+constexpr int kCombineTableWarps = 8;
+constexpr int kCombineStreamWarps = kCombineThreads / 32 - kCombineTableWarps;
+constexpr uint32_t kCombineStreamThreads = 32u * kCombineStreamWarps;
+constexpr uint32_t kHandoffSlots = 128;  // entries of one table warp's handoff queue
+// Who walks the keys longer than 12 bytes: the stream warp that read them (true) or a table warp (false).
+// Measured per record size (DESIGN §4.4): with 64-byte records long pairs can arrive faster than 8 table warps walk
+// them (a stream of long keys only took 5.1 ms per 4·10^7 pairs that way, 4.1 with the stream warps walking);
+// with 32- and 128-byte records the table warps walk them faster than the stream warps would.
+template <int RB>
+constexpr bool kStreamWalksLong = RB == 64;
+// the shared table; the rest of the 227 KB holds the handoff queues (8 x 128 x 20 bytes) and the table warps'
+// probe rings (8 x 1.2 KB): 188 + 30 = 218 KB
+constexpr int kCombineSmem = 188 * 1024;
 
 // cheap 32-bit hash of KW key words (one IMAD per word); the shared table (over the words of a key of up to 12
 // bytes) and the long entries of the global table (over all key words) take its top bits
@@ -755,7 +769,7 @@ __device__ __forceinline__ void bulk_prefetch_l2(const void* p, uint32_t bytes, 
 // trips: 17.3 / 17.1 / 17.7 / 19.0).  Records of 64 and 128 bytes keep the 2 trips; they were not swept.
 template <int RB>
 constexpr uint32_t kPrefetchTrips = RB <= 32 ? 0u : 2u;
-constexpr uint32_t kEpochTrips = 256;  // shared-table clean-up period: 256 trips = 262,144 pairs per CTA
+constexpr uint32_t kEpochTrips = 256;  // shared-table clean-up period: 256 trips = 196,608 pairs per CTA
 __device__ __forceinline__ uint32_t ldv_u32(const uint32_t* p, uint64_t pol) {
   uint32_t v;
   asm volatile("ld.relaxed.gpu.global.L2::cache_hint.u32 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(pol) : "memory");
@@ -830,7 +844,8 @@ struct GtabEntry {
 
 // The update protocol of an entry's state word.  An entry is claimed with a CAS of its state from 0 to the lock,
 // written (key + lock) with vector stores and published with an exchange of the state after a fence: a reader
-// that sees a published state sees its key.
+// that sees a published state sees its key.  (A release store in place of fence + exchange measured the same on
+// config 3, before and after the warp split of k_combine -- DESIGN §4.4 -- so the plain form stays.)
 template <typename State>
 __device__ __forceinline__ bool gtab_claim(State* st) {
   return atomicCAS(st, State(0), kGtabLock<State>) == State(0);
@@ -930,53 +945,59 @@ __device__ __forceinline__ void gtab_add_long(bool active, uint32_t* __restrict_
   if (!ldone) atomicOr(flags, (uint32_t)ERRF_SKEW);
 }
 
-// flags[0] |= ERRF_*, flags[2] = max over the values seen (saturated to u32).
-// vcap: largest value the shared table accepts -- chosen by the host so that one CTA's sum of such values cannot
-// wrap 32 bits (pairs per CTA x vcap < 2^32), which keeps saturation tests out of the per-pair path.
+// The handoff from the stream warps to the table warps: one queue per table warp t, fed by the stream warps w with
+// w % kCombineTableWarps == t.  A stream warp claims as many consecutive positions as it has entries with ONE shared
+// atomic on the queue's tail, waits while they are not free yet (backpressure: the table warp has not yet taken what
+// was there one lap ago -- nothing is ever dropped), writes the 16-byte entries and publishes each slot with its
+// sequence word ((position + 1) << 1 | long key).  The table warp takes the published prefix at its head, up to 32
+// slots at a time, and frees them by moving the head.  A pair with a key longer than 12 bytes travels as {its index,
+// 0, 0, 0}: the table warp reloads the record for its walk.
+struct CombineHandoff {
+  uint4 e[kCombineTableWarps][kHandoffSlots];
+  uint32_t seq[kCombineTableWarps][kHandoffSlots];
+  uint32_t tail[kCombineTableWarps], head[kCombineTableWarps];
+  uint32_t streams_done;  // stream warps that have handed off their last entry
+};
+
+// WARP-COLLECTIVE: the pairs lq[0 .. nl) (indices, nl <= 32) have keys longer than 12 bytes; each lane reloads
+// its record and the warp walks the long entries of the global table for all of them at once
 template <int RB, bool CHECKED>
-__global__ void __launch_bounds__(kCombineThreads, 1)
-    k_combine(const uint4* __restrict__ recs, uint64_t n, uint32_t pf_trips, uint32_t vcap, uint32_t* __restrict__ gtab,
-              uint32_t glog, uint32_t* __restrict__ flags) {
-  extern __shared__ __align__(16) unsigned char smem_raw[];
+__device__ __forceinline__ void walk_long_keys(const uint32_t* lq, uint32_t nl, const uint4* __restrict__ recs,
+                                               uint32_t* __restrict__ gtab, uint32_t glog, uint32_t* __restrict__ flags,
+                                               const L2Policy& pol) {
   using R = Rec<RB>;
-  using G = GtabEntry<RB>;
-  static_assert(!(CHECKED && R::kU64), "u64 keys keep u64 sums: their adds are never checked");
-  constexpr int W = R::kWords, KW = R::kKeyWords;
-  constexpr int KC = KW < 3 ? KW : 3;  // key words of a shared-table entry: only keys of up to 12 bytes live there
-  // Shared table, ARRAY PER FIELD (32 lanes probing 32 random entries hit 32 random banks, not the four a record
-  // stride allows): tag[e] = 0 empty / 1 being written / the key's 32-bit hash with bit 1 set; val[e] = u32 partial
-  // sum; key[k][e] = key word k < KC.  A probe reads two neighbouring tags; only a tag hit touches the key words.
-  // Longer keys (rare in a word count) bypass it: 20 bytes per entry instead of 36 buys 1.8 times the entries.
-  // Every kEpochTrips trips the CTA stops at a barrier and evicts the entries that gathered less than two pairs
-  // since they were admitted (into the global table, like a miss): the table is filled first come first served,
-  // and without that the keys that happened to arrive first would keep out warmer keys that arrived later.
-  // (compile-time sizes: table addresses become immediates -- the kernel is short of registers)
-  constexpr uint32_t entries = (uint32_t)(kCombineSmem / (R::kU64 ? 16 : 20));  // tag + value + 2 (u64) or 3 key words
-  uint32_t* tag = (uint32_t*)smem_raw;
-  uint32_t* val = tag + entries;
-  uint32_t* key = val + entries;
-  // Pairs that found no place in the shared table queue up per warp as 16-byte compact entries (a ring of 64, with
-  // the number of the probe they are at).  When 32 are there the warp ISSUES their probes -- one 16-byte read per
-  // lane, into registers -- and goes on with the stream; it LOOKS at them when the next 32 are ready: a match is
-  // added to with a fire-and-forget red, an empty entry is claimed, anything else (another key: next probe; an
-  // entry being written: same probe) goes back into the ring.  Nothing ever waits for the table: the L2 round trip,
-  // microseconds with 32 warps per SM and nothing else to run, is spent on the stream (a synchronous walk waits for
-  // these reads and takes as long as its unluckiest lane).
-  __shared__ uint4 queue[kCombineThreads / 32][64];
-  __shared__ uint8_t queue_probe[kCombineThreads / 32][64];
-  __shared__ uint32_t long_queue[kCombineThreads / 32][32];  // indices of pairs with long keys, walked 32 at a time
-  const uint32_t tid = threadIdx.x, lane = tid & 31;
-  const L2Policy pol = l2_policies();
-  uint4* q = queue[tid >> 5];
-  uint8_t* qp = queue_probe[tid >> 5];
-  uint32_t* lq = long_queue[tid >> 5];
+  uint32_t w[R::kWords];
+#pragma unroll
+  for (int k = 0; k < R::kWords; k++) w[k] = 0;
+  const bool mine = (threadIdx.x & 31) < nl;
+  if (mine) load_rec_hint<RB>(recs + (size_t)lq[threadIdx.x & 31] * R::kVec, w, pol.stream);
+  gtab_add_long<RB, CHECKED>(mine, gtab, glog, w, (uint32_t)rec_value<RB>(w), flags, pol.keep);
+  __syncwarp();
+}
+
+// One TABLE warp: drains handoff queue t into the global table until every stream warp is done and the queue is
+// empty, then flushes what it still has in flight.
+// Its entries queue up as 16-byte compact entries in a ring of 64 (with the number of the probe they are at).  When
+// 32 are there the warp ISSUES their probes -- one 16-byte read per lane, into registers -- and takes the next
+// entries from the handoff queue; it LOOKS at them when the next 32 are ready (or the queue is idle): a match is
+// added to with a fire-and-forget red, an empty entry is claimed, anything else (another key: next probe; an entry
+// being written: same probe) goes back into the ring.  Long keys are collected by index and walked 32 at a time.
+template <int RB, bool CHECKED>
+__device__ __forceinline__ void combine_table_warp(CombineHandoff& hq, uint32_t t, const uint4* __restrict__ recs,
+                                                   uint32_t* __restrict__ gtab, uint32_t glog, uint32_t* __restrict__ flags,
+                                                   const L2Policy& pol) {
+  using R = Rec<RB>;
+  __shared__ uint4 queue[kCombineTableWarps][64];
+  __shared__ uint8_t queue_probe[kCombineTableWarps][64];
+  __shared__ uint32_t long_queue[kCombineTableWarps][32];
+  const uint32_t lane = threadIdx.x & 31;
+  uint4* q = queue[t];
+  uint8_t* qp = queue_probe[t];
+  uint32_t* lq = long_queue[t];
   uint32_t lq_n = 0;
   uint32_t q_tail = 0, q_pend = 0;  // ring: [.. in flight ..][.. q_pend pending ..] tail
   uint32_t fly_base = 0, fly_n = 0; // the batch in flight: fly_n entries from fly_base (0 = none)
   uint4 fx;                         // ... this lane's probed table entry
-  uint32_t vmax = 0;
-  for (uint32_t i = tid; i < entries * (KC + 2); i += blockDim.x) tag[i] = 0;
-  __syncthreads();
   const uint32_t gmask = GtabLayout{RB, glog}.nshort() - 1u;
   auto append = [&](bool p, const uint4& E, uint32_t probe) {  // collective: the entries of the lanes with p go to the tail
     const uint32_t m = __ballot_sync(0xffffffffu, p);
@@ -1031,53 +1052,155 @@ __global__ void __launch_bounds__(kCombineThreads, 1)
     }
   };
   auto long_walk = [&]() {  // collective
-    uint32_t w[W];
-#pragma unroll
-    for (int k = 0; k < W; k++) w[k] = 0;
-    const bool mine = lane < lq_n;
-    if (mine) load_rec_hint<RB>(recs + (size_t)lq[lane] * R::kVec, w, pol.stream);
-    gtab_add_long<RB, CHECKED>(mine, gtab, glog, w, (uint32_t)rec_value<RB>(w), flags, pol.keep);
+    walk_long_keys<RB, CHECKED>(lq, lq_n, recs, gtab, glog, flags, pol);
     lq_n = 0;
-    __syncwarp();
   };
-  // (between two barriers) entries with a sum below `below` leave the shared table for the global one
+  const volatile uint32_t* seq = hq.seq[t];
+  uint32_t head = 0;  // (hq.head[t] is this warp's to move)
+  for (;;) {
+    const bool last = *(volatile uint32_t*)&hq.streams_done == (uint32_t)kCombineStreamWarps;
+    __threadfence_block();  // (a stream warp counts itself done after its last slot is published)
+    const uint32_t at = head + lane, s = at % kHandoffSlots, sq = seq[s];
+    const uint32_t ready = __ballot_sync(0xffffffffu, (sq & ~1u) == (at + 1u) << 1);
+    const uint32_t k = ~ready ? __ffs(~ready) - 1u : 32u;  // the published prefix
+    if (!k) {
+      if (last) break;  // every stream warp is done and all it published is taken
+      if (fly_n) look();  // the queue is idle: move the ring on
+      else if (q_pend) issue();
+      else __nanosleep(100);
+      continue;
+    }
+    __threadfence_block();
+    const bool mine = lane < k, lng = mine && (sq & 1u);
+    const uint4 E = mine ? hq.e[t][s] : make_uint4(0, 0, 0, 0);
+    __syncwarp();
+    __threadfence_block();  // (the slots are read before they are freed)
+    head += k;
+    if (lane == 0) *(volatile uint32_t*)&hq.head[t] = head;
+    if (!R::kU64) {
+      const uint32_t ml = __ballot_sync(0xffffffffu, lng);
+      if (ml) {
+        if (lq_n + __popc(ml) > 32) long_walk();
+        if (lng) lq[lq_n + __popc(ml & ((1u << lane) - 1u))] = E.x;
+        lq_n += __popc(ml);
+        __syncwarp();
+      }
+    }
+    const bool p = mine && !lng;
+    if (__any_sync(0xffffffffu, p)) push(p, E);
+  }
+  if (!R::kU64 && lq_n) long_walk();
+  // drain: whatever is in flight or pending, batch by batch, until nothing comes back
+  while (fly_n || q_pend) {
+    if (fly_n) look();
+    if (q_pend) issue();
+  }
+}
+
+// flags[0] |= ERRF_*, flags[2] = max over the values seen (saturated to u32).
+// vcap: largest value the shared table accepts -- chosen by the host so that one CTA's sum of such values cannot
+// wrap 32 bits (pairs per CTA x vcap < 2^32), which keeps saturation tests out of the per-pair path.
+// WARP ROLES.  The first kCombineStreamWarps warps STREAM the pairs: they load them, probe and fill the shared
+// table and evict from it.  Every pair they cannot settle there, and every evicted entry, is handed off (see
+// CombineHandoff) to one of the kCombineTableWarps TABLE warps, which alone probe, claim and add to the global table
+// and walk the long keys.  So a stream warp never waits for an L2 round trip and its reads in flight are all
+// stream reads.
+template <int RB, bool CHECKED>
+__global__ void __launch_bounds__(kCombineThreads, 1)
+    k_combine(const uint4* __restrict__ recs, uint64_t n, uint32_t pf_trips, uint32_t vcap, uint32_t* __restrict__ gtab,
+              uint32_t glog, uint32_t* __restrict__ flags) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  using R = Rec<RB>;
+  using G = GtabEntry<RB>;
+  static_assert(!(CHECKED && R::kU64), "u64 keys keep u64 sums: their adds are never checked");
+  constexpr int W = R::kWords, KW = R::kKeyWords;
+  constexpr int KC = KW < 3 ? KW : 3;  // key words of a shared-table entry: only keys of up to 12 bytes live there
+  // Shared table, ARRAY PER FIELD (32 lanes probing 32 random entries hit 32 random banks, not the four a record
+  // stride allows): tag[e] = 0 empty / 1 being written / the key's 32-bit hash with bit 1 set; val[e] = u32 partial
+  // sum; key[k][e] = key word k < KC.  A probe reads two neighbouring tags; only a tag hit touches the key words.
+  // Longer keys (rare in a word count) bypass it: 20 bytes per entry instead of 36 buys 1.8 times the entries.
+  // Every kEpochTrips trips the CTA stops at a barrier and evicts the entries that gathered less than two pairs
+  // since they were admitted (into the global table, like a miss): the table is filled first come first served,
+  // and without that the keys that happened to arrive first would keep out warmer keys that arrived later.
+  // (compile-time sizes: table addresses become immediates -- the kernel is short of registers)
+  constexpr uint32_t entries = (uint32_t)(kCombineSmem / (R::kU64 ? 16 : 20));  // tag + value + 2 (u64) or 3 key words
+  uint32_t* tag = (uint32_t*)smem_raw;
+  uint32_t* val = tag + entries;
+  uint32_t* key = val + entries;
+  __shared__ CombineHandoff hq;
+  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const L2Policy pol = l2_policies();
+  for (uint32_t i = tid; i < entries * (KC + 2); i += blockDim.x) tag[i] = 0;
+  for (uint32_t i = tid; i < kCombineTableWarps * kHandoffSlots; i += blockDim.x) (&hq.seq[0][0])[i] = 0;
+  if (tid < kCombineTableWarps) hq.tail[tid] = hq.head[tid] = 0;
+  if (tid == 0) hq.streams_done = 0;
+  __syncthreads();  // (the last barrier of the whole CTA: from here on the stream warps sync among themselves)
+  if (warp >= (uint32_t)kCombineStreamWarps) {
+    combine_table_warp<RB, CHECKED>(hq, warp - kCombineStreamWarps, recs, gtab, glog, flags, pol);
+    return;
+  }
+  const uint32_t to = warp % kCombineTableWarps;  // the table warp this warp hands off to
+  // (kStreamWalksLong<RB>) the indices of this warp's pairs with long keys, walked 32 at a time by this warp
+  __shared__ uint32_t long_queue[kStreamWalksLong<RB> ? kCombineStreamWarps : 1][32];
+  uint32_t* lq = long_queue[kStreamWalksLong<RB> ? warp : 0];
+  uint32_t lq_n = 0;
+  auto stream_sync = []() { asm volatile("bar.sync 1, %0;" ::"r"(kCombineStreamThreads) : "memory"); };
+  auto handoff = [&](bool p, const uint4& E, bool lng) {  // collective: the entries of the lanes with p
+    const uint32_t m = __ballot_sync(0xffffffffu, p), k = __popc(m);
+    uint32_t base = 0;
+    if (lane == 0) {
+      base = atomicAdd(&hq.tail[to], k);
+      while (base + k - *(volatile uint32_t*)&hq.head[to] > kHandoffSlots) __nanosleep(32);  // backpressure
+    }
+    base = __shfl_sync(0xffffffffu, base, 0);
+    if (p) {
+      const uint32_t at = base + __popc(m & ((1u << lane) - 1u)), s = at % kHandoffSlots;
+      hq.e[to][s] = E;
+      __threadfence_block();
+      *(volatile uint32_t*)&hq.seq[to][s] = (at + 1u) << 1 | (uint32_t)lng;
+    }
+  };
+  uint32_t vmax = 0;
+  // (between two barriers of the stream warps) entries with a sum below `below` leave the shared table for the
+  // global one
   auto evict = [&](uint32_t below) {
     const uint32_t e_round = (entries + 31) / 32 * 32;
-    for (uint32_t e = tid; e < e_round; e += blockDim.x) {
+    for (uint32_t e = tid; e < e_round; e += kCombineStreamThreads) {
       const bool out = e < entries && tag[e] > 1u && val[e] < below;
       uint4 E = make_uint4(0, 0, 0, 0);
       if (out) {
         E = G::pack(key[e], key[entries + e], KC > 2 ? key[2u * entries + e] : 0u, val[e]);
         tag[e] = 0;
       }
-      if (__any_sync(0xffffffffu, out)) push(out, E);
+      if (__any_sync(0xffffffffu, out)) handoff(out, E, false);
     }
   };
-  // every CTA streams ONE contiguous slice of the pairs
+  // every CTA streams ONE contiguous slice of the pairs, kCombineStreamThreads pairs per trip
+  constexpr uint32_t T = kCombineStreamThreads;
   const uint64_t slice = ((n + gridDim.x - 1) / gridDim.x + 31) / 32 * 32;
   const uint64_t slice_lo = slice * blockIdx.x < n ? slice * blockIdx.x : n;
   const uint64_t slice_hi = slice_lo + slice < n ? slice_lo + slice : n;  // (this CTA's pairs: [slice_lo, slice_hi))
-  const uint32_t ntrips = (uint32_t)((slice_hi - slice_lo + blockDim.x - 1) / blockDim.x);  // (the same for every thread: barriers inside)
-  // the pair of the NEXT trip is requested before this one is processed.  Index arithmetic of the loop: running
-  // 64-bit pointers and 32-bit trip bounds (the per-trip 64-bit index, bounds checks and
-  // prefetch address were a visible share of its instructions)
+  const uint32_t ntrips = (uint32_t)((slice_hi - slice_lo + T - 1) / T);  // (the same for every stream thread: barriers inside)
+  // the pair of the NEXT trip is requested before this one is processed (two trips ahead measured the same on
+  // config 3).  Index arithmetic of the loop: running 64-bit pointers and 32-bit trip bounds (the per-trip 64-bit
+  // index, bounds checks and prefetch address were a visible share of its instructions)
   const uint32_t npairs = (uint32_t)(slice_hi - slice_lo);                                  // pairs of this CTA (< 2^32)
-  const uint32_t my_trips = tid < npairs ? (npairs - tid + blockDim.x - 1) / blockDim.x : 0u;  // trips in which this thread has a pair
+  const uint32_t my_trips = tid < npairs ? (npairs - tid + T - 1) / T : 0u;  // trips in which this thread has a pair
   // the warp's 32 pairs of trip t + pf_trips lie inside the slice for t < pf_ok
   const uint32_t wbase = (tid & ~31u) + 32u;
-  const uint32_t pf_full = npairs >= wbase ? (npairs - wbase) / blockDim.x + 1u : 0u;      // trips whose 32 pairs are all there
+  const uint32_t pf_full = npairs >= wbase ? (npairs - wbase) / T + 1u : 0u;      // trips whose 32 pairs are all there
   const uint32_t pf_ok = pf_trips && pf_full > pf_trips ? pf_full - pf_trips : 0u;
   const uint4* p_next = recs + (slice_lo + tid) * R::kVec;                                  // this thread's pair of the next trip
-  const uint4* p_pf = recs + (slice_lo + (tid & ~31u) + (uint64_t)pf_trips * blockDim.x) * R::kVec;  // the warp's prefetch target
-  const size_t p_step = (size_t)blockDim.x * R::kVec;
+  const uint4* p_pf = recs + (slice_lo + (tid & ~31u) + (uint64_t)pf_trips * T) * R::kVec;  // the warp's prefetch target
+  const size_t p_step = (size_t)T * R::kVec;
   uint32_t i32 = (uint32_t)slice_lo + tid;  // index of the pair in hand (all pairs of one shuffle: < 2^32)
   uint32_t wn[W];
   if (my_trips) load_rec_hint<RB>(p_next, wn, pol.stream);
-  for (uint32_t trip = 0; trip < ntrips; trip++, i32 += blockDim.x) {
+  for (uint32_t trip = 0; trip < ntrips; trip++, i32 += T) {
     if (trip % kEpochTrips == kEpochTrips - 1) {
-      __syncthreads();
+      stream_sync();
       evict(2u);
-      __syncthreads();
+      stream_sync();
     }
     uint32_t w[W];
 #pragma unroll
@@ -1127,32 +1250,33 @@ __global__ void __launch_bounds__(kCombineThreads, 1)
         }
       }
     }
-    // misses: long string keys (rare) are remembered by index and walk their table 32 at a time, all lanes busy;
-    // everything else queues up as a compact entry
-    if (!R::kU64) {
-      if (need && v > kMaxCombinedSum) {  // (this test also keeps such values out of the long table)
-        atomicOr(flags, (uint32_t)ERRF_OVERFLOW);
-        need = false;
-      }
+    // misses go to the table warps: a short key as its compact entry, a long string key by index (or, with
+    // kStreamWalksLong, into this warp's own walk)
+    if (!R::kU64 && need && v > kMaxCombinedSum) {  // (this test also keeps such values out of the long table)
+      atomicOr(flags, (uint32_t)ERRF_OVERFLOW);
+      need = false;
+    }
+    if constexpr (kStreamWalksLong<RB>) {
       const uint32_t ml = __ballot_sync(0xffffffffu, need && !is_short);
       if (ml) {
-        if (lq_n + __popc(ml) > 32) long_walk();
+        if (lq_n + __popc(ml) > 32) {
+          walk_long_keys<RB, CHECKED>(lq, lq_n, recs, gtab, glog, flags, pol);
+          lq_n = 0;
+        }
         if (need && !is_short) lq[lq_n + __popc(ml & ((1u << lane) - 1u))] = i32;
         lq_n += __popc(ml);
         __syncwarp();
+        need = need && is_short;
       }
     }
-    const bool p = need && is_short;
-    if (__any_sync(0xffffffffu, p)) push(p, G::pack(w[0], w[1], w[2], v));
+    if (__any_sync(0xffffffffu, need)) handoff(need, is_short ? G::pack(w[0], w[1], w[2], v) : make_uint4(i32, 0, 0, 0), !is_short);
   }
-  __syncthreads();
+  if (kStreamWalksLong<RB> && lq_n) walk_long_keys<RB, CHECKED>(lq, lq_n, recs, gtab, glog, flags, pol);
+  stream_sync();
   evict(0xffffffffu);  // the shared table's entries take the same road as the misses
-  if (!R::kU64 && lq_n) long_walk();
-  // drain: whatever is in flight or pending, batch by batch, until nothing comes back
-  while (fly_n || q_pend) {
-    if (fly_n) look();
-    if (q_pend) issue();
-  }
+  __syncwarp();
+  __threadfence_block();  // (this warp's slots are published before it counts itself done)
+  if (lane == 0) atomicAdd(&hq.streams_done, 1u);
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) vmax = max(vmax, __shfl_xor_sync(0xffffffffu, vmax, o));
   if (lane == 0 && vmax) atomicMax(flags + 2, vmax);
