@@ -72,6 +72,26 @@ enum {
   MRHBM_RED_NONE = 1
 };
 
+/* built-in combinerfn, run on the map side (job.lua:92-96,198-202: reducing the combined values must give what
+ * reducing the raw ones gives) */
+enum {
+  MRHBM_COMBINE_NONE = 0,
+  MRHBM_COMBINE_REDUCER = 1, /* the built-in reducer (MRHBM_RED_SUM), at the shuffle: one pair per key */
+  /* MRHBM_F_BYTE_VALUES only (any other combination fails mrhbm_init with MRHBM_E_INVAL): a combinerfn whose result
+   * depends only on the SET of a key's values, such as an inverted index's "distinct files of a word".  At
+   * mrhbm_map_commit the handle's pairs are reduced to their distinct (key, value) pairs: keys compare by their stored
+   * slot bytes (long keys, see mrhbm_emit_str, by their bytes, on the host), values by their bytes (not by their value
+   * id; the empty value is a value like any other).  The first copy in pool order (the handle's emission order)
+   * survives; survivors keep their
+   * relative order and their value ids.  Pairs of different map jobs are never merged (the host reducefn still sees
+   * one copy per job), and replace-by-job-id and abort are unchanged; a commit that fails leaves the job uncommitted.
+   * mrhbm_pool_read, mrhbm_checksum_input, mrhbm_result_info.pairs_in and everything after the commit see only the
+   * surviving pairs.  The room of the dropped pairs and of their value bytes is not reused before mrhbm_reset.  Device
+   * memory: a hash set of 16 bytes x (a power of two >= 2 x the job's pairs), kept across commits, plus 4 + record
+   * bytes per pair of the job. */
+  MRHBM_COMBINE_DISTINCT = 2
+};
+
 typedef struct mrhbm_ctx mrhbm_ctx;
 typedef struct mrhbm_map mrhbm_map;
 typedef struct mrhbm_iter mrhbm_iter;
@@ -84,8 +104,7 @@ typedef struct mrhbm_config {
   uint32_t num_partitions; /* P >= 1 (reduce jobs; server.lua:316-323) */
   uint32_t partitioner;    /* MRHBM_PART_* */
   uint32_t reducer;        /* MRHBM_RED_* */
-  uint32_t combiner;       /* 0 = none, 1 = combine with the reducer on the map side
-                              (job.lua:92-96,198-202) */
+  uint32_t combiner;       /* MRHBM_COMBINE_* (job.lua:92-96,198-202) */
   uint64_t reserve_pairs;  /* pre-size the HBM emit pool (0 = grow on demand) */
   uint32_t flags;          /* MRHBM_F_* */
   uint32_t reserved;
@@ -94,8 +113,8 @@ typedef struct mrhbm_config {
 #define MRHBM_F_SMALL_BINS 2u   /* test hook: tiny smem bins to exercise the overflow paths */
 #define MRHBM_F_NO_OPTIMISTIC 4u /* always run the exact two-pass (histogram) partition layout */
 /* Byte-string values (lua-mapreduce's emit(key, value) takes any Lua string or number, utils.lua:100-120): a value is
- * opaque bytes, 0 to 1 GiB long, carried through group-only mode.  Needs reducer = MRHBM_RED_NONE and combiner = 0
- * (else mrhbm_init fails with MRHBM_E_INVAL) and one GPU (mrhbm_comm_init with world > 1 fails).  On such a ctx:
+ * opaque bytes, 0 to 1 GiB long, carried through group-only mode.  Needs reducer = MRHBM_RED_NONE and combiner
+ * MRHBM_COMBINE_NONE or MRHBM_COMBINE_DISTINCT (else mrhbm_init fails with MRHBM_E_INVAL) and one GPU (mrhbm_comm_init with world > 1 fails).  On such a ctx:
  *   - pairs are emitted with mrhbm_emit_str_value / mrhbm_emit_u64_value / mrhbm_emit_batch_values /
  *     mrhbm_map_words_value; the integer-valued emits (emit_str, emit_u64, emit_batch, emit_device, map_gen_*,
  *     map_wordcount) fail with MRHBM_E_INVAL;

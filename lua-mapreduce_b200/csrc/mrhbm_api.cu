@@ -10,6 +10,7 @@
 #include <initializer_list>
 #include <map>
 #include <mutex>
+#include <set>
 #include <string>
 #include <thread>
 #include <vector>
@@ -119,6 +120,11 @@ struct mrhbm_ctx {
   uint32_t gtab_extra = 0;              // log2 growth of the table beyond its L2-resident size after it filled up once
   bool no_combine = false;              // sticky: more distinct keys than the largest table takes
   bool combine_checked = false;         // sticky: values large enough that u32 sums must be checked add by add
+  // MRHBM_COMBINE_DISTINCT at commit: the hash set (kept across commits, grown by doubling), the entry of every record
+  // of the job, the survivors before they are copied back, the job's ranges and its tile counts and offsets
+  void *dd_tab = nullptr, *dd_out = nullptr, *dd_rg = nullptr;
+  uint32_t *dd_slot = nullptr, *dd_tiles = nullptr;
+  uint64_t dd_tab_cap = 0, dd_rec_cap = 0, dd_rg_cap = 0, dd_tiles_cap = 0;  // entries, records, ranges, tiles
   uint64_t N = 0, groups = 0;
   bool shuffled = false;
   std::vector<uint32_t> h_bin_off, h_uoff;
@@ -513,6 +519,65 @@ int ensure_compact(mrhbm_ctx* c) {
   return 0;
 }
 
+// MRHBM_COMBINE_DISTINCT, at commit: the map's open ranges are reduced to their distinct (key slot, value bytes) pairs
+// in place, the first copy of each in pool order surviving (mrhbm_distinct.cu), and its long-key pairs to their
+// distinct (key, value bytes) pairs.  kept receives every open range as (first, survivors); the caller shrinks the
+// ranges in the ledger once the whole commit has succeeded.
+int distinct_pairs(mrhbm_map* m, std::vector<std::pair<uint64_t, uint64_t>>& kept) {
+  mrhbm_ctx* c = m->ctx;
+  cudaStream_t s = c->stream;
+  kept = c->led.open_ranges(m->serial);
+  std::vector<DistinctRange> rg;
+  uint64_t n = 0, nt = 0;
+  for (const auto& r : kept) {
+    rg.push_back(DistinctRange{r.first, n, (uint32_t)nt, 0});
+    n += r.second;
+    nt += (r.second + kDistinctTile - 1) / kDistinctTile;
+  }
+  rg.push_back(DistinctRange{0, n, (uint32_t)nt, 0});
+  const uint32_t nr = (uint32_t)rg.size() - 1;
+  if (n > (1ull << 31)) return fail(c, MRHBM_E_INVAL, "distinct combiner: a map job of %llu pairs (limit 2^31)", (unsigned long long)n);
+  if (n) {
+    uint64_t T = 1024;
+    while (T < 2 * n) T <<= 1;
+    int rc = grow(c, &c->dd_tab_cap, T, std::max(T, 2 * c->dd_tab_cap), {{&c->dd_tab, 16}});
+    if (!rc) rc = grow(c, &c->dd_rec_cap, n, n, {{(void**)&c->dd_slot, 4}, {&c->dd_out, (size_t)c->rb}});
+    if (!rc) rc = grow(c, &c->dd_rg_cap, nr + 1, nr + 1, {{&c->dd_rg, sizeof(DistinctRange)}});
+    if (!rc) rc = grow(c, &c->dd_tiles_cap, 2 * (nt + 1), 2 * (nt + 1), {{(void**)&c->dd_tiles, 4}});
+    if (rc) return rc;
+    uint32_t *tile_cnt = c->dd_tiles, *tile_off = c->dd_tiles + nt + 1;
+    const DistinctRange* drg = (const DistinctRange*)c->dd_rg;
+    CU(c, cudaMemsetAsync(c->dd_tab, 0xff, T * 16, s));
+    CU(c, cudaMemcpyAsync(c->dd_rg, rg.data(), rg.size() * sizeof(DistinctRange), cudaMemcpyHostToDevice, s));
+    launch_distinct_mark(c->rb, c->pool, drg, nr, (uint32_t)nt, c->arena, c->voff, c->dd_tab, T - 1, c->dd_slot, s);
+    launch_distinct_count(drg, nr, (uint32_t)nt, c->dd_tab, c->dd_slot, tile_cnt, s);
+    launch_exscan(tile_cnt, (uint32_t)nt, tile_off, nullptr, nullptr, 0xffffffffu, nullptr, nullptr, nullptr, 0, s,
+                  c->d_small + 64);
+    CU(c, cudaGetLastError());
+    std::vector<uint32_t> off(nt + 1);
+    CU(c, cudaMemcpyAsync(off.data(), tile_off, (nt + 1) * 4, cudaMemcpyDeviceToHost, s));
+    CU(c, cudaStreamSynchronize(s));
+    if (off[nt] < n) {
+      launch_distinct_scatter(c->rb, c->pool, drg, nr, (uint32_t)nt, c->dd_tab, c->dd_slot, tile_off, c->dd_out, s);
+      CU(c, cudaGetLastError());
+      for (size_t k = 0; k < kept.size(); k++) {
+        const uint64_t a = off[rg[k].tbase], b = off[rg[k + 1].tbase];
+        if (b - a < kept[k].second && b > a)
+          CU(c, cudaMemcpyAsync((char*)c->pool + kept[k].first * c->rb, (char*)c->dd_out + a * c->rb, (b - a) * c->rb,
+                                cudaMemcpyDeviceToDevice, s));
+        kept[k].second = b - a;
+      }
+      CU(c, cudaStreamSynchronize(s));
+    }
+  }
+  std::set<std::pair<std::string, std::string>> seen;
+  std::vector<LongPair> longs;
+  for (LongPair& lp : m->long_pairs)
+    if (seen.emplace(lp.esc, lp.bytes).second) longs.push_back(std::move(lp));
+  m->long_pairs.swap(longs);
+  return 0;
+}
+
 float ev_ms(mrhbm_ctx* c, int a, int b) {
   float ms = 0;
   if (cudaEventElapsedTime(&ms, c->ev[a], c->ev[b]) != cudaSuccess) {
@@ -571,9 +636,12 @@ int mrhbm_init(const mrhbm_config* cfg, mrhbm_ctx** out) {
   } else
     return fail(c, MRHBM_E_INVAL, "unknown key_kind %u", cfg->key_kind);
   if (cfg->reducer != MRHBM_RED_SUM && cfg->reducer != MRHBM_RED_NONE) return fail(c, MRHBM_E_INVAL, "unknown reducer %u", cfg->reducer);
-  if (cfg->reducer == MRHBM_RED_NONE && cfg->combiner) return fail(c, MRHBM_E_INVAL, "a general reducer cannot be combined on the device (combiner must be 0)");
-  if ((cfg->flags & MRHBM_F_BYTE_VALUES) && (cfg->reducer != MRHBM_RED_NONE || cfg->combiner))
-    return fail(c, MRHBM_E_INVAL, "byte values (MRHBM_F_BYTE_VALUES) need reducer MRHBM_RED_NONE and combiner 0");
+  if (cfg->combiner > MRHBM_COMBINE_DISTINCT) return fail(c, MRHBM_E_INVAL, "unknown combiner %u", cfg->combiner);
+  if (cfg->combiner == MRHBM_COMBINE_DISTINCT && !(cfg->flags & MRHBM_F_BYTE_VALUES))
+    return fail(c, MRHBM_E_INVAL, "combiner MRHBM_COMBINE_DISTINCT needs byte values (MRHBM_F_BYTE_VALUES)");
+  if (cfg->reducer == MRHBM_RED_NONE && cfg->combiner == MRHBM_COMBINE_REDUCER) return fail(c, MRHBM_E_INVAL, "a general reducer cannot be combined on the device (combiner must be 0)");
+  if ((cfg->flags & MRHBM_F_BYTE_VALUES) && (cfg->reducer != MRHBM_RED_NONE || cfg->combiner == MRHBM_COMBINE_REDUCER))
+    return fail(c, MRHBM_E_INVAL, "byte values (MRHBM_F_BYTE_VALUES) need reducer MRHBM_RED_NONE and combiner 0 or MRHBM_COMBINE_DISTINCT");
   c->bytevals = c->led.byte_values = (cfg->flags & MRHBM_F_BYTE_VALUES) != 0;
   c->sb.no_reduce = cfg->reducer == MRHBM_RED_NONE;
   CU(c, cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
@@ -619,7 +687,8 @@ void mrhbm_destroy(mrhbm_ctx* c) {
                    c->d_outoff,    c->d_segoff,    c->recvbuf,    c->bigbuf,      c->d_small,   c->comb,
                    c->gtab,        c->l1buf,       c->regions,    c->d_l1all,     c->d_sample,   c->d_tok_text[0],
                    c->d_tok_text[1], c->d_tok_cnt, c->d_tok_off, c->d_spl,     c->arena,       c->voff,
-                   c->cvals,       c->row_off,     c->val_tile,   c->val_pieces};
+                   c->cvals,       c->row_off,     c->val_tile,   c->val_pieces, c->dd_tab,     c->dd_out,
+                   c->dd_rg,       c->dd_slot,     c->dd_tiles};
   for (void* p : frees)
     if (p) cudaFree(p);
   if (c->h_counters) cudaFreeHost(c->h_counters);
@@ -1076,10 +1145,13 @@ int mrhbm_map_commit(mrhbm_map* m) {
     cudaError_t e = cudaStreamSynchronize(c->stream);  // caller may reuse its pinned buffers now
     if (e != cudaSuccess) rc = fail(c, MRHBM_E_CUDA, "commit: %s", cudaGetErrorString(e));
   }
+  std::vector<std::pair<uint64_t, uint64_t>> kept;
+  if (rc == 0 && c->cfg.combiner == MRHBM_COMBINE_DISTINCT) rc = distinct_pairs(m, kept);
   if (rc) {
     mrhbm_map_abort(m);
     return rc;
   }
+  for (const auto& r : kept) c->led.shrink(m->serial, r.first, r.second);
   c->led.commit(m->serial, m->job);
   c->long_jobs.erase(m->job);  // replace-by-job-id on the host side too
   if (!m->long_pairs.empty()) c->long_jobs[m->job] = std::move(m->long_pairs);
@@ -1277,7 +1349,7 @@ int collect_sources(mrhbm_ctx* c, std::vector<Src>& srcs, uint64_t* N, mrhbm_sta
     n += r.second;
   }
   *N = n;
-  if (!c->cfg.combiner || c->no_combine || n < (1u << 20)) return 0;
+  if (c->cfg.combiner != MRHBM_COMBINE_REDUCER || c->no_combine || n < (1u << 20)) return 0;
   cudaStream_t s = c->stream;
   bool checked = c->combine_checked;
   for (;;) {
@@ -1553,7 +1625,7 @@ int shuffle_fast(mrhbm_ctx* c, std::vector<Src>& live, uint64_t N, uint64_t N_in
     nonuniform |= all[k * r + 1];
   }
   if (Nglobal == 0) return 0;  // nothing to do here: the exact path handles the empty shuffle
-  const uint32_t S = pick_sub_bins(c, Nglobal, c->cfg.combiner && G > 1 ? (uint32_t)G : 1u);
+  const uint32_t S = pick_sub_bins(c, Nglobal, c->cfg.combiner == MRHBM_COMBINE_REDUCER && G > 1 ? (uint32_t)G : 1u);
   const uint64_t B = (uint64_t)P * S;
   if (B >= (1ull << 31)) return 0;
   const uint32_t ordered = (want_ordered && !nonuniform) || S == 1;

@@ -1,0 +1,222 @@
+// mrhbm_distinct.cu -- MRHBM_COMBINE_DISTINCT: at the commit of a map job on a byte-values ctx, the job's records are
+// reduced to their distinct (key slot, value bytes) pairs, the first copy of each in pool order surviving.
+//   k_distinct_mark     every record joins an open-addressing hash set of 16-byte entries {fingerprint, pool index of
+//                       the first copy}: it claims an empty entry, or finds the entry of an equal pair and lowers its
+//                       index to its own with atomicMin; it remembers the entry
+//   k_distinct_count    a record survives when it is its entry's minimum; survivors per tile of kTile records
+//   (launch_exscan of the tile counts)
+//   k_distinct_scatter  the survivors, whole records in pool order, to a scratch buffer at their tile's offset
+// The caller copies each range's survivors back to the range's start.  Records move as they are: value ids, voff and
+// the arena are not touched.
+#include <cstdint>
+
+#include "mrhbm_dev.cuh"
+
+namespace mrhbm {
+
+namespace {
+constexpr unsigned long long kEmpty = ~0ull;  // an entry's fingerprint and index before the claim (memset to 0xff)
+
+// tile t lies in the range k with rg[k].tbase <= t < rg[k + 1].tbase (no range is empty)
+__device__ __forceinline__ uint32_t range_of_tile(const DistinctRange* __restrict__ rg, uint32_t nr, uint32_t t) {
+  uint32_t lo = 0, hi = nr;
+  while (hi - lo > 1) {
+    const uint32_t mid = (lo + hi) >> 1;
+    if (rg[mid].tbase <= t) lo = mid;
+    else hi = mid;
+  }
+  return lo;
+}
+
+// this thread's record of tile blockIdx.x: its pool index p and its index g among the job's records; false past the
+// end of the range
+__device__ __forceinline__ bool tile_record(const DistinctRange* __restrict__ rg, uint32_t nr, uint64_t* p, uint64_t* g) {
+  const uint32_t t = blockIdx.x, k = range_of_tile(rg, nr, t);
+  const uint64_t j = (uint64_t)(t - rg[k].tbase) * kDistinctTile + threadIdx.x;
+  if (j >= rg[k + 1].vbase - rg[k].vbase) return false;
+  *p = rg[k].off + j;
+  *g = rg[k].vbase + j;
+  return true;
+}
+
+// A value's bytes as little-endian 32-bit words, whatever the alignment of its first byte in the arena: word i holds
+// bytes 4i .. 4i+3, zero past the end.  Only aligned words that hold a byte of the value are read.
+struct ValView {
+  const uint32_t* w;
+  uint32_t sh;
+  uint64_t len;
+};
+__device__ __forceinline__ ValView val_view(const unsigned char* __restrict__ arena, const uint64_t* __restrict__ voff,
+                                            uint64_t id) {
+  const uint64_t s = voff[id];
+  ValView v;
+  v.len = voff[id + 1] - s;
+  v.sh = (uint32_t)(s & 3);
+  v.w = (const uint32_t*)(arena + s - v.sh);
+  return v;
+}
+__device__ __forceinline__ uint32_t val_word(const ValView& v, uint64_t i) {
+  uint32_t x = __ldg(v.w + i);
+  if (v.sh) x = __funnelshift_r(x, 4 * (i + 1) < v.sh + v.len ? __ldg(v.w + i + 1) : 0u, 8 * v.sh);
+  const uint64_t rem = v.len - 4 * i;
+  return rem < 4 ? x & ((1u << (8 * rem)) - 1) : x;
+}
+
+__device__ __forceinline__ uint64_t fp_step(uint64_t h, uint64_t x) {
+  h = (h ^ x) * 0x9E3779B97F4A7C15ull;
+  return h ^ (h >> 29);
+}
+// 64-bit fingerprint of the key slot words and the value bytes (never kEmpty)
+template <int RB>
+__device__ __forceinline__ uint64_t fingerprint(const uint32_t* r, const ValView& v) {
+  uint64_t h = fp_step(0x5851F42D4C957F2Dull, v.len);
+#pragma unroll
+  for (int i = 0; i < Rec<RB>::kKeyWords; i += 2)
+    h = fp_step(h, (uint64_t)r[i] | (i + 1 < Rec<RB>::kKeyWords ? (uint64_t)r[i + 1] << 32 : 0ull));
+  const uint64_t nw = (v.len + 3) / 4;
+  for (uint64_t i = 0; i < nw; i += 2)
+    h = fp_step(h, (uint64_t)val_word(v, i) | (i + 1 < nw ? (uint64_t)val_word(v, i + 1) << 32 : 0ull));
+  h = mix64(h);
+  return h == kEmpty ? 0 : h;
+}
+
+// the record r (value id id, bytes v) against the record at q: equal key slots and equal value bytes
+template <int RB>
+__device__ __forceinline__ bool same_pair(const uint32_t* r, uint64_t id, const ValView& v, const uint32_t* __restrict__ q,
+                                          const unsigned char* __restrict__ arena, const uint64_t* __restrict__ voff) {
+  if (!key_eq<RB>(r, q)) return false;
+  const uint64_t qid = rec_value<RB>(q);
+  if (qid == id) return true;  // (the pairs of one tokeniser piece share their id)
+  const ValView u = val_view(arena, voff, qid);
+  if (u.len != v.len) return false;
+  const uint64_t nw = (v.len + 3) / 4;
+  for (uint64_t i = 0; i < nw; i++)
+    if (val_word(u, i) != val_word(v, i)) return false;
+  return true;
+}
+
+template <int RB>
+__device__ __forceinline__ void load_record(const unsigned char* __restrict__ pool, uint64_t p, uint32_t* r) {
+  const uint4* src = (const uint4*)(pool + p * RB);
+#pragma unroll
+  for (int i = 0; i < Rec<RB>::kVec; i++) {
+    const uint4 x = __ldg(src + i);
+    r[4 * i] = x.x;
+    r[4 * i + 1] = x.y;
+    r[4 * i + 2] = x.z;
+    r[4 * i + 3] = x.w;
+  }
+}
+
+__device__ __forceinline__ bool survives(const DistinctRange* __restrict__ rg, uint32_t nr,
+                                         const ulonglong2* __restrict__ tab, const uint32_t* __restrict__ slot_of,
+                                         uint64_t* p) {
+  uint64_t g;
+  return tile_record(rg, nr, p, &g) && tab[slot_of[g]].y == *p;
+}
+}  // namespace
+
+// Linear probing from fingerprint & mask.  An entry is claimed with atomicCAS on its fingerprint; its claimer stores
+// its index right after, and a thread that meets the fingerprint waits for that index to compare against the pair it
+// stands for.  A fingerprint shared by unequal pairs only costs a compare: the thread probes on.
+template <int RB>
+__global__ void __launch_bounds__(kDistinctTile) k_distinct_mark(const unsigned char* __restrict__ pool,
+                                                                 const DistinctRange* __restrict__ rg, uint32_t nr,
+                                                                 const unsigned char* __restrict__ arena,
+                                                                 const uint64_t* __restrict__ voff, ulonglong2* tab,
+                                                                 uint64_t mask, uint32_t* __restrict__ slot_of) {
+  uint64_t p, g;
+  if (!tile_record(rg, nr, &p, &g)) return;
+  uint32_t r[Rec<RB>::kWords];
+  load_record<RB>(pool, p, r);
+  const uint64_t id = rec_value<RB>(r);
+  const ValView v = val_view(arena, voff, id);
+  const uint64_t fp = fingerprint<RB>(r, v);
+  for (uint64_t s = fp & mask;; s = (s + 1) & mask) {
+    unsigned long long* e = (unsigned long long*)&tab[s];
+    unsigned long long f = *(volatile unsigned long long*)e;
+    if (f == kEmpty) {
+      f = atomicCAS(e, kEmpty, (unsigned long long)fp);
+      if (f == kEmpty) {
+        atomicMin(e + 1, (unsigned long long)p);
+        slot_of[g] = (uint32_t)s;
+        return;
+      }
+    }
+    if (f != fp) continue;
+    unsigned long long q;
+    while ((q = *(volatile unsigned long long*)(e + 1)) == kEmpty) {
+    }
+    if (same_pair<RB>(r, id, v, (const uint32_t*)(pool + q * RB), arena, voff)) {
+      if (p < q) atomicMin(e + 1, (unsigned long long)p);  // (the index only falls: p > q cannot be the minimum)
+      slot_of[g] = (uint32_t)s;
+      return;
+    }
+  }
+}
+
+__global__ void __launch_bounds__(kDistinctTile) k_distinct_count(const DistinctRange* __restrict__ rg, uint32_t nr,
+                                                                  const ulonglong2* __restrict__ tab,
+                                                                  const uint32_t* __restrict__ slot_of,
+                                                                  uint32_t* __restrict__ tile_cnt) {
+  uint64_t p;
+  const int n = __syncthreads_count(survives(rg, nr, tab, slot_of, &p));
+  if (threadIdx.x == 0) tile_cnt[blockIdx.x] = (uint32_t)n;
+}
+
+template <int RB>
+__global__ void __launch_bounds__(kDistinctTile) k_distinct_scatter(const unsigned char* __restrict__ pool,
+                                                                    const DistinctRange* __restrict__ rg, uint32_t nr,
+                                                                    const ulonglong2* __restrict__ tab,
+                                                                    const uint32_t* __restrict__ slot_of,
+                                                                    const uint32_t* __restrict__ tile_off,
+                                                                    unsigned char* __restrict__ out) {
+  uint64_t p = 0;
+  const bool keep = survives(rg, nr, tab, slot_of, &p);
+  const uint32_t rank = cta_exscan<kDistinctTile>(keep ? 1u : 0u).excl;
+  if (!keep) return;
+  const uint4* src = (const uint4*)(pool + p * RB);
+  uint4* dst = (uint4*)(out + ((uint64_t)tile_off[blockIdx.x] + rank) * RB);
+#pragma unroll
+  for (int i = 0; i < Rec<RB>::kVec; i++) dst[i] = __ldg(src + i);
+}
+
+int launch_distinct_mark(int rb, const void* pool, const DistinctRange* rg, uint32_t nr, uint32_t ntiles,
+                         const unsigned char* arena, const uint64_t* voff, void* tab, uint64_t mask, uint32_t* slot_of,
+                         cudaStream_t s) {
+  if (!ntiles) return 0;
+  const unsigned char* P = (const unsigned char*)pool;
+  ulonglong2* T = (ulonglong2*)tab;
+  switch (rb) {
+    case 16: k_distinct_mark<16><<<ntiles, kDistinctTile, 0, s>>>(P, rg, nr, arena, voff, T, mask, slot_of); break;
+    case 32: k_distinct_mark<32><<<ntiles, kDistinctTile, 0, s>>>(P, rg, nr, arena, voff, T, mask, slot_of); break;
+    case 64: k_distinct_mark<64><<<ntiles, kDistinctTile, 0, s>>>(P, rg, nr, arena, voff, T, mask, slot_of); break;
+    default: k_distinct_mark<128><<<ntiles, kDistinctTile, 0, s>>>(P, rg, nr, arena, voff, T, mask, slot_of); break;
+  }
+  return 1;
+}
+
+int launch_distinct_count(const DistinctRange* rg, uint32_t nr, uint32_t ntiles, const void* tab, const uint32_t* slot_of,
+                          uint32_t* tile_cnt, cudaStream_t s) {
+  if (!ntiles) return 0;
+  k_distinct_count<<<ntiles, kDistinctTile, 0, s>>>(rg, nr, (const ulonglong2*)tab, slot_of, tile_cnt);
+  return 1;
+}
+
+int launch_distinct_scatter(int rb, const void* pool, const DistinctRange* rg, uint32_t nr, uint32_t ntiles,
+                            const void* tab, const uint32_t* slot_of, const uint32_t* tile_off, void* out,
+                            cudaStream_t s) {
+  if (!ntiles) return 0;
+  const unsigned char* P = (const unsigned char*)pool;
+  const ulonglong2* T = (const ulonglong2*)tab;
+  unsigned char* O = (unsigned char*)out;
+  switch (rb) {
+    case 16: k_distinct_scatter<16><<<ntiles, kDistinctTile, 0, s>>>(P, rg, nr, T, slot_of, tile_off, O); break;
+    case 32: k_distinct_scatter<32><<<ntiles, kDistinctTile, 0, s>>>(P, rg, nr, T, slot_of, tile_off, O); break;
+    case 64: k_distinct_scatter<64><<<ntiles, kDistinctTile, 0, s>>>(P, rg, nr, T, slot_of, tile_off, O); break;
+    default: k_distinct_scatter<128><<<ntiles, kDistinctTile, 0, s>>>(P, rg, nr, T, slot_of, tile_off, O); break;
+  }
+  return 1;
+}
+
+}  // namespace mrhbm

@@ -223,4 +223,26 @@ int launch_value_gather(const uint64_t* ids, uint64_t n, const uint64_t* voff, c
                         uint64_t* row_off, const uint64_t* tile_pre, unsigned char* out, uint64_t* pieces,
                         unsigned long long* npieces, cudaStream_t s);
 
+// ---- MRHBM_COMBINE_DISTINCT (mrhbm_distinct.cu) ----
+// One map job's records: range k holds pool records [off, off + rg[k+1].vbase - vbase), which are the job's records
+// [vbase, ...) and its tiles of kDistinctTile records [tbase, rg[k+1].tbase).  nr ranges, none empty, then one entry
+// {0, total records, total tiles}.
+struct DistinctRange {
+  uint64_t off, vbase;
+  uint32_t tbase, pad;
+};
+constexpr uint32_t kDistinctTile = 256;
+// every record into the hash set tab (mask + 1 16-byte entries, a power of two >= 2 x the job's records, memset to
+// 0xff by the caller); slot_of[g] receives the entry of the job's record g
+int launch_distinct_mark(int rb, const void* pool, const DistinctRange* rg, uint32_t nr, uint32_t ntiles,
+                         const unsigned char* arena, const uint64_t* voff, void* tab, uint64_t mask, uint32_t* slot_of,
+                         cudaStream_t s);
+// tile_cnt[t] = the records of tile t that are the first copy of their pair
+int launch_distinct_count(const DistinctRange* rg, uint32_t nr, uint32_t ntiles, const void* tab, const uint32_t* slot_of,
+                          uint32_t* tile_cnt, cudaStream_t s);
+// those records, in pool order, to out: tile t's at out[tile_off[t] ..) (tile_off: the exclusive scan of tile_cnt)
+int launch_distinct_scatter(int rb, const void* pool, const DistinctRange* rg, uint32_t nr, uint32_t ntiles,
+                            const void* tab, const uint32_t* slot_of, const uint32_t* tile_off, void* out,
+                            cudaStream_t s);
+
 }  // namespace mrhbm

@@ -12,7 +12,11 @@
 //     remembers the arena offset of its first value.  The pairs of one tokeniser piece (mrhbm_map_words_value)
 //     share the id of the piece's first pair, which holds the value; the other ids of the piece hold empty values;
 //   - dead ranges at the tail give their room back when an abort finds them there; dead ranges with live or open
-//     records behind them keep their room (records and value bytes) until reset().
+//     records behind them keep their room (records and value bytes) until reset();
+//   - MRHBM_COMBINE_DISTINCT: shrink() keeps the first records of an open range (its distinct pairs, moved forward)
+//     and leaves the rest as lost room until reset(): a kept pair's value id may point past the new end, to bytes
+//     that must stay where they are.  A shrunk range that dies at the tail no longer ends at used(), so no abort
+//     gives that room back.
 #pragma once
 #include <cassert>
 #include <cstdint>
@@ -38,7 +42,7 @@ class PoolLedger {
   uint64_t arena_used() const { return arena_used_; }
   uint64_t new_owner() { return ++owners_; }
 
-  // rewind(mark()) undoes every take and add since the mark (no commit, abort or reset may lie between)
+  // rewind(mark()) undoes every take and add since the mark (no commit, shrink, abort or reset may lie between)
   Mark mark() const { return Mark{ranges_.size(), ranges_.empty() ? 0 : ranges_.back().cnt, used_, arena_used_}; }
   void rewind(const Mark& mk) {
     assert(mk.ranges <= ranges_.size() && mk.used <= used_ && mk.arena_used <= arena_used_);
@@ -67,6 +71,24 @@ class PoolLedger {
       }
     }
     ranges_.push_back(Range{off, cnt, job, OPEN, owner, aoff});
+  }
+
+  // the owner's open ranges that hold records, as (first, count), in pool order
+  std::vector<std::pair<uint64_t, uint64_t>> open_ranges(uint64_t owner) const {
+    std::vector<std::pair<uint64_t, uint64_t>> v;
+    for (const Range& r : ranges_)
+      if (r.owner == owner && r.state == OPEN && r.cnt) v.emplace_back(r.off, r.cnt);
+    return v;
+  }
+  // the owner's open range of records that starts at off keeps its first cnt records (see the invariants above)
+  void shrink(uint64_t owner, uint64_t off, uint64_t cnt) {
+    for (Range& r : ranges_)
+      if (r.owner == owner && r.state == OPEN && r.cnt && r.off == off) {
+        assert(cnt <= r.cnt);
+        r.cnt = cnt;
+        return;
+      }
+    assert(!"shrink: no such open range");
   }
 
   void commit(uint64_t owner, const std::string& job) {

@@ -16,7 +16,8 @@ local hbm = { _VERSION = "0.1", _NAME = "mapreduce.hbm" }
 --     or a key range: hbm_partitionfn = "range", hbm_splitters = { s_1, ..., s_{n-1} } (non-decreasing strings; u64
 --     keys as their 8 big-endian bytes; partition k takes the keys k splitters are <= to) or hbm_splitters = "sample"
 --     (quantiles of the map output, taken at the MAP -> REDUCE barrier).  The partitionfn must compute the same ranges.
---   reducefn / combinerfn module: hbm_reducefn = "sum"
+--   reducefn / combinerfn module: hbm_reducefn = "sum"; a combinerfn module of a value_kind = "bytes" job:
+--     hbm_combinerfn = "distinct" (its combinerfn emits the distinct values it is given)
 local ctx -- one context per worker process (job.lua keeps `funcs`/`initialized` per process too)
 local sample_splitters = false -- hbm_splitters = "sample": hbm.prepare_reduce samples them before the shuffle
 local tuple_keys = false -- hbm.configure(..., { key_kind = "tuple" }); an upvalue of configure, map_job and groups
@@ -39,19 +40,23 @@ function hbm.configure(partition_mod, reduce_mod, combiner_mod, opts)
   -- hbm_reducefn = "sum": reduced on the device.  No declaration: general reducer -- the device
   -- partitions, sorts and groups, job.lua:264-284 calls reducefn per group on the host.
   local builtin = reduce_mod.hbm_reducefn == "sum"
-  assert(not combiner_mod or (builtin and combiner_mod.hbm_reducefn == "sum"),
-         "a combinerfn runs on the device: it (and the reducefn) must declare hbm_reducefn = 'sum'")
   opts = opts or {}
   tuple_keys = opts.key_kind == "tuple" -- composite keys travel as encoded byte strings
   byte_values = opts.value_kind == "bytes" -- values travel as encoded byte strings (hbm.encode_value)
   assert(not (byte_values and builtin),
          "value_kind = 'bytes' hands string and number values to a general reducefn: the reducefn must not declare hbm_reducefn")
+  -- hbm_combinerfn = "distinct" (values = "bytes"): the combinerfn keeps one copy of each distinct value of a key, so
+  -- the device drops the repeated (key, value) pairs of each map job at its commit
+  local distinct = combiner_mod ~= nil and combiner_mod.hbm_combinerfn == "distinct"
+  assert(not distinct or byte_values, "hbm_combinerfn = 'distinct' needs value_kind = 'bytes'")
+  assert(not combiner_mod or distinct or (builtin and combiner_mod.hbm_reducefn == "sum"),
+         "a combinerfn runs on the device: it (and the reducefn) must declare hbm_reducefn = 'sum', or hbm_combinerfn = 'distinct' with value_kind = 'bytes'")
   local c, err = mrhbm.new{
     key_kind = tuple_keys and "str" or opts.key_kind or "str",
     max_key_bytes = opts.max_key_bytes or 123,
     num_partitions = assert(partition_mod.NUM_REDUCERS, "partitionfn module must expose NUM_REDUCERS"),
     partitioner = assert(partition_mod.hbm_partitionfn, "partitionfn module must declare hbm_partitionfn"),
-    combiner = combiner_mod ~= nil,
+    combiner = distinct and "distinct" or combiner_mod ~= nil,
     reducer = builtin and "sum" or "none",
     device = opts.device,
     values = byte_values and "bytes" or "int",

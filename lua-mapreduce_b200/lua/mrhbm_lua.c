@@ -18,6 +18,10 @@
 
 #include "mrhbm.h"
 
+#ifndef LUA_TSTRING
+#define LUA_TSTRING 4 /* the same in lua.h of every Lua 5.x (for declaration-only builds of this file) */
+#endif
+
 #define CTX_MT "mrhbm.ctx"
 #define MAP_MT "mrhbm.map"
 #define ITER_MT "mrhbm.iter"
@@ -33,7 +37,7 @@ static int fail(lua_State *L, mrhbm_ctx *c) { /* luamongo style: nil, msg */
 }
 
 /* mrhbm.new{ key_kind="str"|"u64", max_key_bytes=, num_partitions=, partitioner="fnv_lua"|"mulhash"|
- *            "wordhash"|"range", combiner=bool, reducer="sum"|"none", device=, values="int"|"bytes" }
+ *            "wordhash"|"range", combiner=bool|"distinct", reducer="sum"|"none", device=, values="int"|"bytes" }
  * values = "bytes" (MRHBM_F_BYTE_VALUES, needs reducer = "none"): m:emit takes string values and ctx:groups yields
  * tables of strings */
 static int l_new(lua_State *L) {
@@ -54,8 +58,9 @@ static int l_new(lua_State *L) {
   cfg.partitioner = strcmp(s, "fnv_lua") == 0 ? MRHBM_PART_FNV_LUA
                   : strcmp(s, "mulhash") == 0 ? MRHBM_PART_MULHASH
                   : strcmp(s, "range") == 0 ? MRHBM_PART_RANGE : MRHBM_PART_WORDHASH;
-  lua_getfield(L, 1, "combiner");
-  cfg.combiner = lua_toboolean(L, -1);
+  lua_getfield(L, 1, "combiner"); /* true (the built-in reducer) | "distinct" (values = "bytes") */
+  cfg.combiner = lua_type(L, -1) == LUA_TSTRING && strcmp(luaL_checkstring(L, -1), "distinct") == 0 ? MRHBM_COMBINE_DISTINCT
+               : lua_toboolean(L, -1) ? MRHBM_COMBINE_REDUCER : MRHBM_COMBINE_NONE;
   lua_getfield(L, 1, "device");
   cfg.device = (int32_t)luaL_optinteger(L, -1, -1);
   lua_getfield(L, 1, "reducer"); /* "sum" (built-in) | "none" (general reducefn on the host) */

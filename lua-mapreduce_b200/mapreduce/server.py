@@ -39,6 +39,33 @@ def range_splitters(part, nparts, key_kind):
     return norm
 
 
+# Values the declaration hbm_combinerfn = "distinct" is checked on, one key per list: strings (repeated, distinct, the
+# empty string) and numbers.  A list holds one type, as a Lua reducefn that sorts its values needs it.
+_DISTINCT_PROBES = ([b"b", b"a", b"b", b"", b"a", b"", b"c"], [3, 1.5, 3, 0, 1.5])
+
+
+def distinct_combiner(comb, value_kind):
+    """Checks a combinerfn module that declares hbm_combinerfn = "distinct": the device then keeps one copy of each
+    distinct (key, value) pair of a map job in its place, so the module's combinerfn must emit exactly the distinct
+    values it is given (compared as the shuffle compares them, by their encoded bytes)."""
+    from .tuple import encode_value
+    if comb.hbm_combinerfn != "distinct":
+        raise ValueError("unknown hbm_combinerfn %r (built-ins: 'distinct')" % (comb.hbm_combinerfn,))
+    if value_kind != "bytes":
+        raise ValueError("hbm_combinerfn = 'distinct' drops repeated string and number values: "
+                         "configure hbm = {'value_kind': 'bytes'}")
+    for values in _DISTINCT_PROBES:
+        out = []
+        try:
+            comb.combinerfn(b"probe", list(values), out.append)
+            got = sorted(encode_value(v) for v in out)
+        except Exception as e:
+            raise ValueError("hbm_combinerfn = 'distinct': combinerfn failed on the values %r: %r" % (values, e))
+        if got != sorted({encode_value(v) for v in values}):
+            raise ValueError("hbm_combinerfn = 'distinct', but combinerfn turns the values %r into %r instead of their "
+                             "distinct values: the declaration must describe what the combinerfn computes" % (values, out))
+
+
 class server:
     def __init__(self, connection_string, dbname, auth_table=None):
         self.cnn_string, self.dbname = connection_string, dbname
@@ -88,7 +115,10 @@ class server:
         # group on the host otherwise -- sees the raw values and produces the same result, just without the saving.
         device_combiner = "combinerfn" in mods and builtin_red == "sum" and \
             getattr(mods["combinerfn"], "hbm_reducefn", None) == "sum"
-        if "combinerfn" in mods and not device_combiner:
+        # hbm_combinerfn = "distinct" (value_kind = "bytes"): the combinerfn keeps one copy of each distinct value of a
+        # key, so the device drops the repeated (key, value) pairs of each map job at its commit
+        distinct = "combinerfn" in mods and getattr(mods["combinerfn"], "hbm_combinerfn", None) is not None
+        if "combinerfn" in mods and not device_combiner and not distinct:
             sys.stderr.write("# WARNING: combinerfn %s is not a device built-in (hbm_reducefn = 'sum'); it is skipped, "
                              "the reducefn sees the uncombined values\n" % params["combinerfn"])
         pname = getattr(part, "hbm_partitionfn", None)
@@ -109,7 +139,10 @@ class server:
         if getattr(mods["mapfn"], "hbm_mapfn", None) == "words_file" and hbm["value_kind"] != "bytes":
             raise ValueError("hbm_mapfn = 'words_file' pairs every word with the file name, a string value: "
                              "configure hbm = {'value_kind': 'bytes'}")
-        hbm.update(partitioner=_BUILTIN_PART[pname], num_partitions=nparts, combiner=device_combiner,
+        if distinct:
+            distinct_combiner(mods["combinerfn"], hbm["value_kind"])
+        hbm.update(partitioner=_BUILTIN_PART[pname], num_partitions=nparts,
+                   combiner="distinct" if distinct else device_combiner,
                    reducer=0 if builtin_red == "sum" else 1,
                    splitters=range_splitters(part, nparts, hbm["key_kind"]) if pname == "range" else None)
         self.config = dict(mapfn=params["mapfn"], reducefn=params["reducefn"], partitionfn=params["partitionfn"],
@@ -123,8 +156,9 @@ class server:
             return self.ctx_factory(h)
         from .. import mrhbm
         kind = mrhbm.KEY_U64 if h["key_kind"] == "u64" else mrhbm.KEY_STR
+        combiner = mrhbm.COMBINE_DISTINCT if h["combiner"] == "distinct" else h["combiner"]
         ctx = mrhbm.Ctx(kind, h["num_partitions"], h["partitioner"], max_key_bytes=h["max_key_bytes"],
-                        combiner=h["combiner"], device=h["device"], reducer=h["reducer"],
+                        combiner=combiner, device=h["device"], reducer=h["reducer"],
                         flags=mrhbm.F_BYTE_VALUES if h.get("value_kind") == "bytes" else 0)
         if isinstance(h.get("splitters"), list):  # (kept across reset)
             ctx.set_splitters(h["splitters"])
