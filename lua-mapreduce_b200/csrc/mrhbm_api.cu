@@ -117,7 +117,7 @@ struct mrhbm_ctx {
   // map-side combiner: the global (L2 resident) hash table and the records compacted out of it
   void *comb = nullptr, *gtab = nullptr;
   uint64_t comb_cap = 0, gtab_cap = 0;  // records
-  uint32_t gtab_extra = 0;              // log2 growth of the table beyond its L2-resident size after it filled up once
+  uint32_t gtab_grow = 0;               // doublings of the combiner's table beyond its L2-resident size (GtabLayout::sized)
   bool no_combine = false;              // sticky: more distinct keys than the largest table takes
   bool combine_checked = false;         // sticky: values large enough that u32 sums must be checked add by add
   // MRHBM_COMBINE_DISTINCT at commit: the hash set (kept across commits, grown by doubling), the entry of every record
@@ -1332,8 +1332,6 @@ struct Src {
   const char* p;
   uint64_t n;
 };
-constexpr uint32_t kGtabLog = 21;       // global combiner table: 2^21 16-byte entries = 32 MB, resident in the 50 MB L2
-constexpr uint32_t kGtabMaxExtra = 5;   // ... grown up to 32x (1 GB) when the keys do not fit
 
 // The pairs the shuffle partitions: the committed pool ranges, or -- with a combiner declared
 // (job.lua:92-96,198-202) and enough pairs to pay for it -- one record per distinct key of this rank's pairs
@@ -1353,8 +1351,7 @@ int collect_sources(mrhbm_ctx* c, std::vector<Src>& srcs, uint64_t* N, mrhbm_sta
   cudaStream_t s = c->stream;
   bool checked = c->combine_checked;
   for (;;) {
-    const uint32_t glog = kGtabLog + c->gtab_extra;
-    const GtabLayout tab{c->rb, glog};
+    const GtabLayout tab = GtabLayout::sized(c->rb, c->gtab_grow);
     const uint64_t tab_bytes = tab.bytes();
     int rc = ensure_records(c, &c->gtab, &c->gtab_cap, (tab_bytes + c->rb - 1) / c->rb);
     if (rc) return rc;
@@ -1363,16 +1360,16 @@ int collect_sources(mrhbm_ctx* c, std::vector<Src>& srcs, uint64_t* N, mrhbm_sta
     CU(c, cudaMemsetAsync(c->gtab, 0, tab_bytes, s));
     CU(c, cudaMemsetAsync(c->d_small, 0, 3 * sizeof(uint32_t), s));  // [0] flags, [1] records out, [2] largest value
     for (auto& sr : srcs)
-      st.launches += launch_combine(c->rb, sr.p, sr.n, (uint32_t*)c->gtab, glog, c->d_small, checked, c->sm_count, s);
-    st.launches += launch_gtab_compact(c->rb, (const uint32_t*)c->gtab, glog, c->comb, c->d_small + 1, s);
+      st.launches += launch_combine(sr.p, sr.n, (uint32_t*)c->gtab, tab, c->d_small, checked, c->sm_count, s);
+    st.launches += launch_gtab_compact((const uint32_t*)c->gtab, tab, c->comb, c->d_small + 1, s);
     CU(c, cudaGetLastError());
     CU(c, cudaMemcpyAsync(c->h_small, c->d_small, 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
     CU(c, cudaStreamSynchronize(s));
     const uint32_t ef = c->h_small[0];
     if (ef & ERRF_OVERFLOW) return 0;  // not sticky: the next shuffle's sums may fit again
     if (ef & ERRF_SKEW) {  // the table filled up: more distinct keys than it takes
-      if (c->gtab_extra < kGtabMaxExtra) {
-        c->gtab_extra++;
+      if (c->gtab_grow < GtabLayout::kMaxGrow) {
+        c->gtab_grow++;
         continue;
       }
       c->no_combine = true;  // the partition / sort / reduce stages take the raw pairs

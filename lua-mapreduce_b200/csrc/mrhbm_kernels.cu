@@ -700,7 +700,7 @@ __global__ void __launch_bounds__(1024) k_exscan_rows(const uint32_t* __restrict
 //  * Every CTA keeps an open-addressing table in SHARED memory for its lifetime: hot keys (Zipf) are summed
 //    there with shared-memory atomics and never travel further.
 //  * Whatever does not find a place there -- the long tail -- is added to ONE open-addressing table in GLOBAL
-//    memory sized to stay resident in the 50 MB L2 (2^21 16-byte entries = 32 MB): one L2 atomic per pair
+//    memory sized to stay resident in the 50 MB L2 (25 MB of two-entry buckets): one L2 atomic per pair
 //    instead of a partition pass, a sort pass and a reduce pass over that pair.  At its end every CTA flushes
 //    its shared table into the global one; k_gtab_compact then emits one record per table entry.
 // The result (one record per distinct key, in the common case) is what the partition/sort/reduce stages see.
@@ -764,12 +764,16 @@ __device__ __forceinline__ void bulk_prefetch_l2(const void* p, uint32_t bytes, 
   asm volatile("cp.async.bulk.prefetch.L2.global.L2::cache_hint [%0], %1, %2;" ::"l"(p), "r"(bytes), "l"(pol) : "memory");
 }
 // Distance in trips of the L2 bulk prefetch ahead of the trip in hand (0: none).  Prefetched pairs compete with the
-// 32 MB global table for the 50 MB L2.  Config 3 (32-byte records) on one H100 SXM at 700 W, ms of k_combine per 10^9
-// pairs, alternating runs in one call: no prefetch 15.47 against 16.61 with 2 trips (earlier sweep, 1 / 2 / 3 / 4
-// trips: 17.3 / 17.1 / 17.7 / 19.0).  Records of 64 and 128 bytes keep the 2 trips; they were not swept.
+// global table for the 50 MB L2.  Config 3 (32-byte records, with the earlier 32 MB table) on one H100 SXM at 700 W,
+// ms of k_combine per 10^9 pairs, alternating runs in one call: no prefetch 15.47 against 16.61 with 2 trips (earlier
+// sweep, 1 / 2 / 3 / 4 trips: 17.3 / 17.1 / 17.7 / 19.0).  Records of 64 and 128 bytes keep the 2 trips; they were
+// not swept.
 template <int RB>
 constexpr uint32_t kPrefetchTrips = RB <= 32 ? 0u : 2u;
-constexpr uint32_t kEpochTrips = 256;  // shared-table clean-up period: 256 trips = 196,608 pairs per CTA
+// Shared-table clean-up period: 128 trips = 98,304 pairs per CTA.  Config 3 with the 25 MB global table (H100 SXM,
+// 700 W, 5-6 alternating runs, ms of k_combine): 14.19-14.22 with 128 trips, 14.31-14.32 with 256, 14.57 with 512,
+// 14.74 with 1024; 128 trips with a threshold of 3 pairs instead of 2 took 14.52 (too many warm keys leave).
+constexpr uint32_t kEpochTrips = 128;
 __device__ __forceinline__ uint32_t ldv_u32(const uint32_t* p, uint64_t pol) {
   uint32_t v;
   asm volatile("ld.relaxed.gpu.global.L2::cache_hint.u32 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(pol) : "memory");
@@ -808,12 +812,15 @@ __device__ __forceinline__ void load_rec_hint(const uint4* p, uint32_t* w, uint6
 }
 
 // ---- the global table --------------------------------------------------------------------------------------
-// Layout: GtabLayout (mrhbm_kernels.h).  SHORT entries: open addressing with linear probing, ONE entry per probe.
+// Layout: GtabLayout (mrhbm_kernels.h).  SHORT entries: open addressing with linear probing over BUCKETS of two
+// entries, one 32-byte L2 sector each: a random L2 read costs per REQUEST, and a lane pair reads both halves of a
+// bucket in one load instruction, so one sector request looks at two entries.  The entries of a bucket are claimed
+// in order, so an empty first entry means an empty bucket.  A probe is never waited for: it is issued when 32 pairs
+// have queued up and looked at when the next 32 have.
 // String keys longer than 12 bytes (rare in word counts) go to the LONG entries of one record slot each behind the
 // short ones, walked entry by entry by the whole warp (state first, then the key).
-// Why one 16-byte entry per probe: a random L2 read costs the SM per REQUEST, not per byte, and
-// a probe is never waited for: it is issued when 32 pairs have queued up and looked at when the next 32 have.
-constexpr uint32_t kGtabMaxProbes = 192;  // linear probes before the table counts as full
+// A short key that finds no place within GtabLayout::kMaxProbes buckets raises ERRF_SKEW; from then on its table warp
+// drops its remaining pairs, whose result the host discards.
 constexpr int kGtabMaxLongProbes = 128;
 
 // A pair on its way to the global table and a short entry share one 16-byte form: strings of up to 12 bytes
@@ -870,15 +877,16 @@ __device__ __forceinline__ void gtab_add(State* st, State v, uint32_t* __restric
   }
 }
 
+// the home bucket of a short key
 template <int RB>
-__device__ __forceinline__ uint32_t gtab_slot(const uint4& E, uint32_t glog) {
+__device__ __forceinline__ uint32_t gtab_slot(const uint4& E, const GtabLayout& tab) {
   uint32_t g = (E.x ^ 0x9E3779B9u) * 0x85EBCA6Bu;
   g = (g ^ (g >> 15) ^ E.y) * 0x2C1B3C6Du;
   if (!Rec<RB>::kU64) g = (g ^ (g >> 13) ^ E.z) * 0x297A2D39u;
   g ^= g >> 16;
   g *= 0xC2B2AE35u;
   g ^= g >> 15;
-  return g >> (32 - glog);
+  return tab.bucket(g);
 }
 // One probe of the short table: entry `e` as read into x.  Returns 0 = the pair is settled (added, or inserted into
 // the empty entry), 1 = the entry holds another key (probe the next one), 2 = the entry is being written (look again).
@@ -901,14 +909,13 @@ __device__ __forceinline__ int gtab_probe(uint4* e, const uint4& x, const uint4&
 }
 // WARP-COLLECTIVE: string keys longer than 12 bytes, one record slot per entry, state first, then the key
 template <int RB, bool CHECKED>
-__device__ __forceinline__ void gtab_add_long(bool active, uint32_t* __restrict__ gtab, uint32_t glog, const uint32_t* w, uint32_t v32,
-                                              uint32_t* __restrict__ flags, uint64_t pol) {
+__device__ __forceinline__ void gtab_add_long(bool active, uint32_t* __restrict__ gtab, const GtabLayout& tab, const uint32_t* w,
+                                              uint32_t v32, uint32_t* __restrict__ flags, uint64_t pol) {
   using R = Rec<RB>;
   constexpr int W = R::kWords, KW = R::kKeyWords;
   constexpr uint32_t kLock = kGtabLock<uint32_t>;
-  const GtabLayout tab{RB, glog};
   uint32_t* ltab = gtab + tab.long_offset() / sizeof(uint32_t);
-  uint32_t slot = slot_hash<KW>(w) >> (32 - tab.long_log());
+  uint32_t slot = tab.long_slot(slot_hash<KW>(w));
   bool ldone = !active;
 #pragma unroll 1
   for (int probe = 0; probe < kGtabMaxLongProbes; probe++) {
@@ -939,7 +946,7 @@ __device__ __forceinline__ void gtab_add_long(bool active, uint32_t* __restrict_
           ldone = true;
         }
       }
-      slot = (slot + 1) & (tab.nlong() - 1u);
+      slot = tab.long_next(slot);
     }
   }
   if (!ldone) atomicOr(flags, (uint32_t)ERRF_SKEW);
@@ -963,7 +970,7 @@ struct CombineHandoff {
 // its record and the warp walks the long entries of the global table for all of them at once
 template <int RB, bool CHECKED>
 __device__ __forceinline__ void walk_long_keys(const uint32_t* lq, uint32_t nl, const uint4* __restrict__ recs,
-                                               uint32_t* __restrict__ gtab, uint32_t glog, uint32_t* __restrict__ flags,
+                                               uint32_t* __restrict__ gtab, const GtabLayout& tab, uint32_t* __restrict__ flags,
                                                const L2Policy& pol) {
   using R = Rec<RB>;
   uint32_t w[R::kWords];
@@ -971,34 +978,40 @@ __device__ __forceinline__ void walk_long_keys(const uint32_t* lq, uint32_t nl, 
   for (int k = 0; k < R::kWords; k++) w[k] = 0;
   const bool mine = (threadIdx.x & 31) < nl;
   if (mine) load_rec_hint<RB>(recs + (size_t)lq[threadIdx.x & 31] * R::kVec, w, pol.stream);
-  gtab_add_long<RB, CHECKED>(mine, gtab, glog, w, (uint32_t)rec_value<RB>(w), flags, pol.keep);
+  gtab_add_long<RB, CHECKED>(mine, gtab, tab, w, (uint32_t)rec_value<RB>(w), flags, pol.keep);
   __syncwarp();
 }
 
 // One TABLE warp: drains handoff queue t into the global table until every stream warp is done and the queue is
 // empty, then flushes what it still has in flight.
-// Its entries queue up as 16-byte compact entries in a ring of 64 (with the number of the probe they are at).  When
-// 32 are there the warp ISSUES their probes -- one 16-byte read per lane, into registers -- and takes the next
-// entries from the handoff queue; it LOOKS at them when the next 32 are ready (or the queue is idle): a match is
-// added to with a fire-and-forget red, an empty entry is claimed, anything else (another key: next probe; an entry
-// being written: same probe) goes back into the ring.  Long keys are collected by index and walked 32 at a time.
+// Its entries queue up as 16-byte compact entries in a ring of 64 (with the number of the bucket probe they are at).
+// When 32 are there the warp ISSUES their probes and takes the next entries from the handoff queue.  A probe reads
+// the entry's whole bucket: in each of two load instructions lane pair (2i, 2i+1) reads the two halves of one
+// bucket -- of lane 2i's entry in the first, of lane 2i+1's in the second -- so each instruction asks L2 for 16
+// sectors.  The warp LOOKS at them when the next 32 are ready (or the queue is idle): a lane trades the half it holds
+// of its partner's bucket for the half of its own with one shuffle and looks at the bucket's two entries in order.
+// A match is added to with a fire-and-forget red, an empty entry is claimed; a bucket of other keys sends the entry
+// on to the next bucket, an entry being written to the same bucket again (back into the ring).  Long keys are
+// collected by index and walked 32 at a time.
 template <int RB, bool CHECKED>
 __device__ __forceinline__ void combine_table_warp(CombineHandoff& hq, uint32_t t, const uint4* __restrict__ recs,
-                                                   uint32_t* __restrict__ gtab, uint32_t glog, uint32_t* __restrict__ flags,
+                                                   uint32_t* __restrict__ gtab, const GtabLayout& tab, uint32_t* __restrict__ flags,
                                                    const L2Policy& pol) {
   using R = Rec<RB>;
   __shared__ uint4 queue[kCombineTableWarps][64];
   __shared__ uint8_t queue_probe[kCombineTableWarps][64];
   __shared__ uint32_t long_queue[kCombineTableWarps][32];
-  const uint32_t lane = threadIdx.x & 31;
+  static_assert(GtabLayout::kMaxProbes <= 256u, "the ring keeps bucket probes below the limit in 8 bits");
+  const uint32_t lane = threadIdx.x & 31, odd = lane & 1u;
   uint4* q = queue[t];
   uint8_t* qp = queue_probe[t];
   uint32_t* lq = long_queue[t];
   uint32_t lq_n = 0;
   uint32_t q_tail = 0, q_pend = 0;  // ring: [.. in flight ..][.. q_pend pending ..] tail
   uint32_t fly_base = 0, fly_n = 0; // the batch in flight: fly_n entries from fly_base (0 = none)
-  uint4 fx;                         // ... this lane's probed table entry
-  const uint32_t gmask = GtabLayout{RB, glog}.nshort() - 1u;
+  uint4 fx0, fx1;                   // ... this lane's halves (lane & 1) of the buckets of lanes 2i and 2i + 1
+  bool full = false;                // (warp-uniform) this warp has found the table full
+  uint4* const bkt = (uint4*)gtab;  // bucket b: entries 2b and 2b + 1
   auto append = [&](bool p, const uint4& E, uint32_t probe) {  // collective: the entries of the lanes with p go to the tail
     const uint32_t m = __ballot_sync(0xffffffffu, p);
     if (p) {
@@ -1011,20 +1024,26 @@ __device__ __forceinline__ void combine_table_warp(CombineHandoff& hq, uint32_t 
     __syncwarp();
   };
   auto look = [&]() {  // collective: the batch in flight
+    const uint4 send = odd ? fx0 : fx1, o = make_uint4(__shfl_xor_sync(0xffffffffu, send.x, 1), __shfl_xor_sync(0xffffffffu, send.y, 1),
+                                                        __shfl_xor_sync(0xffffffffu, send.z, 1), __shfl_xor_sync(0xffffffffu, send.w, 1));
+    const uint4 h0 = odd ? o : fx0, h1 = odd ? fx1 : o;  // this lane's bucket
     const bool mine = lane < fly_n;
     uint4 E = make_uint4(0, 0, 0, 0);
     uint32_t probe = 0;
     int r = 0;
-    if (mine) {
+    if (mine && !full) {
       E = q[(fly_base + lane) & 63u];
       probe = qp[(fly_base + lane) & 63u];
-      const uint32_t slot = (gtab_slot<RB>(E, glog) + probe) & gmask;
-      r = gtab_probe<RB, CHECKED>((uint4*)gtab + slot, fx, E, flags, pol.keep);
-      if (r == 1 && ++probe >= kGtabMaxProbes) {
-        atomicOr(flags, (uint32_t)ERRF_SKEW);  // table full: the host retries with a larger one
+      uint4* e = bkt + 2u * tab.bucket_at(gtab_slot<RB>(E, tab), probe);
+      r = gtab_probe<RB, CHECKED>(e, h0, E, flags, pol.keep);
+      if (r == 1) r = gtab_probe<RB, CHECKED>(e + 1, h1, E, flags, pol.keep);
+      if (r == 1 && ++probe >= GtabLayout::kMaxProbes) {
+        atomicOr(flags, (uint32_t)ERRF_SKEW);  // table full: the host retries with a larger one and drops this result
+        full = true;
         r = 0;
       }
     }
+    full = __any_sync(0xffffffffu, full);
     fly_n = 0;
     __syncwarp();
     append(r != 0, E, probe);  // (never more than the batch just freed: the ring cannot overflow here)
@@ -1032,11 +1051,11 @@ __device__ __forceinline__ void combine_table_warp(CombineHandoff& hq, uint32_t 
   auto issue = [&]() {  // collective: the oldest min(32, q_pend) pending entries
     fly_n = q_pend < 32u ? q_pend : 32u;
     fly_base = (q_tail - q_pend) & 63u;
-    if (lane < fly_n) {
-      const uint4 E = q[(fly_base + lane) & 63u];
-      const uint32_t slot = (gtab_slot<RB>(E, glog) + qp[(fly_base + lane) & 63u]) & gmask;
-      fx = ldv_v4((const uint4*)gtab + slot, pol.keep);
-    }
+    uint32_t b = 0;
+    if (lane < fly_n) b = tab.bucket_at(gtab_slot<RB>(q[(fly_base + lane) & 63u], tab), qp[(fly_base + lane) & 63u]);
+    const uint32_t b0 = __shfl_sync(0xffffffffu, b, lane & ~1u), b1 = __shfl_sync(0xffffffffu, b, lane | 1u);
+    if ((lane & ~1u) < fly_n) fx0 = ldv_v4(bkt + 2u * b0 + odd, pol.keep);
+    if ((lane | 1u) < fly_n) fx1 = ldv_v4(bkt + 2u * b1 + odd, pol.keep);
     q_pend -= fly_n;
   };
   auto push = [&](bool p, const uint4& E) {  // collective: new entries; makes room first, starts a batch when 32 wait
@@ -1052,7 +1071,7 @@ __device__ __forceinline__ void combine_table_warp(CombineHandoff& hq, uint32_t 
     }
   };
   auto long_walk = [&]() {  // collective
-    walk_long_keys<RB, CHECKED>(lq, lq_n, recs, gtab, glog, flags, pol);
+    walk_long_keys<RB, CHECKED>(lq, lq_n, recs, gtab, tab, flags, pol);
     lq_n = 0;
   };
   const volatile uint32_t* seq = hq.seq[t];
@@ -1108,11 +1127,12 @@ __device__ __forceinline__ void combine_table_warp(CombineHandoff& hq, uint32_t 
 template <int RB, bool CHECKED>
 __global__ void __launch_bounds__(kCombineThreads, 1)
     k_combine(const uint4* __restrict__ recs, uint64_t n, uint32_t pf_trips, uint32_t vcap, uint32_t* __restrict__ gtab,
-              uint32_t glog, uint32_t* __restrict__ flags) {
+              GtabLayout layout, uint32_t* __restrict__ flags) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   using R = Rec<RB>;
   using G = GtabEntry<RB>;
   static_assert(!(CHECKED && R::kU64), "u64 keys keep u64 sums: their adds are never checked");
+  const GtabLayout tab{RB, layout.nbuckets, layout.long_log};  // (RB a constant)
   constexpr int W = R::kWords, KW = R::kKeyWords;
   constexpr int KC = KW < 3 ? KW : 3;  // key words of a shared-table entry: only keys of up to 12 bytes live there
   // Shared table, ARRAY PER FIELD (32 lanes probing 32 random entries hit 32 random banks, not the four a record
@@ -1136,7 +1156,7 @@ __global__ void __launch_bounds__(kCombineThreads, 1)
   if (tid == 0) hq.streams_done = 0;
   __syncthreads();  // (the last barrier of the whole CTA: from here on the stream warps sync among themselves)
   if (warp >= (uint32_t)kCombineStreamWarps) {
-    combine_table_warp<RB, CHECKED>(hq, warp - kCombineStreamWarps, recs, gtab, glog, flags, pol);
+    combine_table_warp<RB, CHECKED>(hq, warp - kCombineStreamWarps, recs, gtab, tab, flags, pol);
     return;
   }
   const uint32_t to = warp % kCombineTableWarps;  // the table warp this warp hands off to
@@ -1260,7 +1280,7 @@ __global__ void __launch_bounds__(kCombineThreads, 1)
       const uint32_t ml = __ballot_sync(0xffffffffu, need && !is_short);
       if (ml) {
         if (lq_n + __popc(ml) > 32) {
-          walk_long_keys<RB, CHECKED>(lq, lq_n, recs, gtab, glog, flags, pol);
+          walk_long_keys<RB, CHECKED>(lq, lq_n, recs, gtab, tab, flags, pol);
           lq_n = 0;
         }
         if (need && !is_short) lq[lq_n + __popc(ml & ((1u << lane) - 1u))] = i32;
@@ -1271,7 +1291,7 @@ __global__ void __launch_bounds__(kCombineThreads, 1)
     }
     if (__any_sync(0xffffffffu, need)) handoff(need, is_short ? G::pack(w[0], w[1], w[2], v) : make_uint4(i32, 0, 0, 0), !is_short);
   }
-  if (kStreamWalksLong<RB> && lq_n) walk_long_keys<RB, CHECKED>(lq, lq_n, recs, gtab, glog, flags, pol);
+  if (kStreamWalksLong<RB> && lq_n) walk_long_keys<RB, CHECKED>(lq, lq_n, recs, gtab, tab, flags, pol);
   stream_sync();
   evict(0xffffffffu);  // the shared table's entries take the same road as the misses
   __syncwarp();
@@ -1284,11 +1304,11 @@ __global__ void __launch_bounds__(kCombineThreads, 1)
 
 // one record per non-empty entry of the global table (short entries first, then the long ones), appended to out
 template <int RB>
-__global__ void __launch_bounds__(256) k_gtab_compact(const uint32_t* __restrict__ gtab, uint32_t glog, uint4* __restrict__ out,
+__global__ void __launch_bounds__(256) k_gtab_compact(const uint32_t* __restrict__ gtab, GtabLayout layout, uint4* __restrict__ out,
                                                       uint32_t* __restrict__ count) {
   using R = Rec<RB>;
+  const GtabLayout tab{RB, layout.nbuckets, layout.long_log};  // (RB a constant)
   constexpr int W = R::kWords, KW = R::kKeyWords;
-  const GtabLayout tab{RB, glog};
   const uint32_t nshort = tab.nshort(), lane = threadIdx.x & 31;
   const uint32_t* ltab = gtab + tab.long_offset() / sizeof(uint32_t);
   for (uint32_t base = (blockIdx.x * blockDim.x + threadIdx.x) & ~31u; base < tab.records(); base += gridDim.x * blockDim.x) {
@@ -1585,23 +1605,25 @@ int launch_tok_emit(int rb, const unsigned char* text, uint64_t len, const uint3
   }
   return 1;
 }
-int launch_combine(int rb, const void* recs, uint64_t n, uint32_t* gtab, uint32_t glog, uint32_t* flags, bool checked,
+int launch_combine(const void* recs, uint64_t n, uint32_t* gtab, const GtabLayout& tab, uint32_t* flags, bool checked,
                    int sm_count, cudaStream_t s) {
   if (!n) return 0;
+  const int rb = tab.rb;
   // the shared table only takes values whose per-CTA sum stays within kMaxCombinedSum
   const uint64_t per_cta = (n + sm_count - 1) / sm_count + kCombineThreads;
   const uint32_t vcap = (uint32_t)std::min<uint64_t>(0xffffull, kMaxCombinedSum / per_cta);
   if (checked) {  // (u64 keys keep u64 sums: never checked)
-    DISPATCH_RB(rb, (k_combine<RB, !Rec<RB>::kU64><<<sm_count, kCombineThreads, kCombineSmem, s>>>((const uint4*)recs, n, kPrefetchTrips<RB>, vcap, gtab, glog, flags)));
+    DISPATCH_RB(rb, (k_combine<RB, !Rec<RB>::kU64><<<sm_count, kCombineThreads, kCombineSmem, s>>>((const uint4*)recs, n, kPrefetchTrips<RB>, vcap, gtab, tab, flags)));
   } else {
-    DISPATCH_RB(rb, (k_combine<RB, false><<<sm_count, kCombineThreads, kCombineSmem, s>>>((const uint4*)recs, n, kPrefetchTrips<RB>, vcap, gtab, glog, flags)));
+    DISPATCH_RB(rb, (k_combine<RB, false><<<sm_count, kCombineThreads, kCombineSmem, s>>>((const uint4*)recs, n, kPrefetchTrips<RB>, vcap, gtab, tab, flags)));
   }
   return 1;
 }
-int launch_gtab_compact(int rb, const uint32_t* gtab, uint32_t glog, void* out, uint32_t* count, cudaStream_t s) {
-  const uint32_t slots = GtabLayout{rb, glog}.records();
+int launch_gtab_compact(const uint32_t* gtab, const GtabLayout& tab, void* out, uint32_t* count, cudaStream_t s) {
+  const int rb = tab.rb;
+  const uint32_t slots = tab.records();
   int grid = (int)std::min<uint32_t>((slots + 255) / 256, (uint32_t)g_sm_count * 8);
-  DISPATCH_RB(rb, (k_gtab_compact<RB><<<grid, 256, 0, s>>>(gtab, glog, (uint4*)out, count)));
+  DISPATCH_RB(rb, (k_gtab_compact<RB><<<grid, 256, 0, s>>>(gtab, tab, (uint4*)out, count)));
   return 1;
 }
 int launch_sum_src(const uint32_t* all, uint32_t world, uint32_t stride, uint32_t base, uint32_t n,

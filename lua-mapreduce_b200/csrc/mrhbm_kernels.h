@@ -122,29 +122,54 @@ int launch_tok_count(const unsigned char* text, uint64_t len, uint32_t* block_co
 int launch_tok_emit(int rb, const unsigned char* text, uint64_t len, const uint32_t* block_off, void* recs,
                     uint32_t value, uint32_t* flags, cudaStream_t s);
 inline uint64_t tok_blocks(uint64_t len) { return (len + 255) / 256; }
-// The map-side combiner's global table for records of rb bytes: 2^glog short entries of 16 bytes, then, for string
-// records only, 2^(glog-4) long entries of one record each.  The compaction emits at most one record per entry.
+// The map-side combiner's global table for records of rb bytes: `nbuckets` buckets of one 32-byte L2 sector each,
+// two 16-byte short entries per bucket, then, for string records only, 2^long_log long entries of one record each.
+// A short key probes buckets linearly from bucket(hash), wrapping at nbuckets (not a power of two: the table is
+// sized to the keys).  The compaction emits at most one record per entry.
 struct GtabLayout {
   int rb;
-  uint32_t glog;
-  MRHBM_HD uint32_t nshort() const { return 1u << glog; }
-  MRHBM_HD uint32_t long_log() const { return glog - 4; }
-  MRHBM_HD uint32_t nlong() const { return rb == 16 ? 0u : 1u << long_log(); }
-  MRHBM_HD uint64_t long_offset() const { return (uint64_t)16 << glog; }  // bytes
+  uint32_t nbuckets;  // a multiple of 16, so that short and long entries each fill whole warps of the compaction
+  uint32_t long_log;
+  // The size a shuffle starts at, and after `grow` tables that filled up (each doubles both parts).  25 MB of
+  // buckets: 1.64 M short entries, load 0.64 on config 3's 1.05 M keys.  On config 3 (H100 SXM, 700 W) k_combine
+  // took 14.72 ms with 20 MB (load 0.8: longer chains), 14.38-14.43 from 23 to 28 MB, 14.59 with 32 MB and 16.03
+  // with 48 MB (the table no longer stays in L2 beside the pair stream; DESIGN §4.4).  2^15 long entries: keys of
+  // more than 12 bytes are 0.64 % of config 3's pairs, ~16 K distinct keys.
+  static constexpr uint32_t kBuckets = 819200, kLongLog = 15, kMaxGrow = 6;
+  // Bucket probes of a short key before the table counts as full (and grows).  In a CPU model of linear probing with
+  // uniform hashes over 819,200 two-entry buckets, no key moved more than 132 buckets from its home at load 0.8,
+  // 239 at 0.85 and 560 at 0.9: a table below 0.8 never reports full, one above 0.9 does.  Fuller tables cost more
+  // than a retry: at load 0.92, 2^24 pairs over 1.5 M keys took k_combine 2.64 ms against 1.46 ms with the earlier
+  // 32 MB table (DESIGN §4.4).
+  static constexpr uint32_t kMaxProbes = 256;
+  static MRHBM_HD GtabLayout sized(int rb, uint32_t grow) { return GtabLayout{rb, kBuckets << grow, kLongLog + grow}; }
+  MRHBM_HD uint32_t nshort() const { return 2u * nbuckets; }
+  MRHBM_HD uint32_t nlong() const { return rb == 16 ? 0u : 1u << long_log; }
+  MRHBM_HD uint64_t long_offset() const { return (uint64_t)32 * nbuckets; }  // bytes
   MRHBM_HD uint64_t bytes() const { return long_offset() + (uint64_t)rb * nlong(); }
   MRHBM_HD uint32_t records() const { return nshort() + nlong(); }
+  // the home bucket of a 32-bit key hash (its top bits, scaled to nbuckets), and the bucket `probe` steps after it
+  // (probe < nbuckets)
+  MRHBM_HD uint32_t bucket(uint32_t h) const { return (uint32_t)(((uint64_t)h * nbuckets) >> 32); }
+  MRHBM_HD uint32_t bucket_at(uint32_t home, uint32_t probe) const {
+    const uint32_t b = home + probe;
+    return b >= nbuckets ? b - nbuckets : b;
+  }
+  // the home entry of a long key's 32-bit hash, and the entry after e
+  MRHBM_HD uint32_t long_slot(uint32_t h) const { return h >> (32 - long_log); }
+  MRHBM_HD uint32_t long_next(uint32_t e) const { return (e + 1) & (nlong() - 1u); }
 };
 // Largest sum (and so largest value) a combined string record carries in its u32 value: the table keeps sum + 1,
 // and all ones marks an entry being written.
 constexpr uint32_t kMaxCombinedSum = 0xffffffefu;
-// map-side combine of one committed range into the global table gtab (GtabLayout{rb, glog}.bytes(), zeroed by the
+// map-side combine of one committed range into the global table gtab (tab.bytes(), 32-byte aligned, zeroed by the
 // caller); flags[0] |= ERRF_SKEW when the table is full, ERRF_OVERFLOW when a u32 sum would pass kMaxCombinedSum
 // (checked mode only: unchecked adds are fire-and-forget and the caller verifies afterwards that pairs x flags[2],
 // the largest value seen, stays within it)
-int launch_combine(int rb, const void* recs, uint64_t n, uint32_t* gtab, uint32_t glog, uint32_t* flags, bool checked,
+int launch_combine(const void* recs, uint64_t n, uint32_t* gtab, const GtabLayout& tab, uint32_t* flags, bool checked,
                    int sm_count, cudaStream_t s);
 // one record per non-empty table entry appended to out; *count (zeroed by the caller) += entries
-int launch_gtab_compact(int rb, const uint32_t* gtab, uint32_t glog, void* out, uint32_t* count, cudaStream_t s);
+int launch_gtab_compact(const uint32_t* gtab, const GtabLayout& tab, void* out, uint32_t* count, cudaStream_t s);
 // tot[b] = sum over s < world of all[s * stride + base + b], b < n; *nover += bins (of all `stride`
 // bins) whose global total exceeds cap
 int launch_sum_src(const uint32_t* all, uint32_t world, uint32_t stride, uint32_t base, uint32_t n,
