@@ -69,7 +69,25 @@ enum {
    * Needs combiner = 0.  mrhbm_result_copy then returns one row per pair (keys repeat).  A key may
    * carry any number of values, on one GPU or several: a bin larger than one shared-memory sort is
    * sorted run by run on its owner and the iterator merges the runs. */
-  MRHBM_RED_NONE = 1
+  MRHBM_RED_NONE = 1,
+  /* MRHBM_F_BYTE_VALUES only, with combiner MRHBM_COMBINE_NONE or MRHBM_COMBINE_DISTINCT (any other combination fails
+   * mrhbm_init with MRHBM_E_INVAL; one GPU, as byte values are): the reducefn "each key's distinct values, ascending",
+   * an inverted index's, computed on the device -- no host reducefn runs.  After mrhbm_shuffle the result holds exactly
+   * one row per distinct (key, value bytes) pair over all committed pairs of all map jobs: keys compare as everywhere
+   * else, values by their bytes, never by their value id (two emits of the same bytes under different ids are one row;
+   * the empty value is a value like any other).  Which of several equal pairs gives the row its value id is
+   * unspecified.  Inside each run rows ascend by (key, value bytes), values in the key order's sense: unsigned
+   * bytewise, a proper prefix first.  So mrhbm_groups_next_values gives every group, long keys included, its distinct
+   * values ascending; mrhbm_result_copy / mrhbm_result_values rows follow info.sorted (with sorted = 1 a partition's
+   * rows ascend by (key, value) as a whole), and an oversized bin is one run, not several.  mrhbm_result_info: pairs_in
+   * = committed pairs, pairs_recv = distinct pairs the shuffle carried, groups = rows.  mrhbm_checksum_result's
+   * out[3..5] keep their meaning; in[0..2] == out[0..2] does not hold (duplicates are gone and a row's value id may be
+   * another copy's).  The ordering kernels are timed in mrhbm_stats.ms_bigbins, the dedupe in ms_combine, both inside
+   * ms_total.  Limits: fewer than 2^31 committed pairs per shuffle (else MRHBM_E_INVAL).  Extra device memory: the
+   * distinct set of MRHBM_COMBINE_DISTINCT sized for all committed pairs (16 bytes x a power of two >= 2 x pairs, plus
+   * 4 + record bytes per pair), and, in a shuffle with a bin of more rows than one shared-memory sort takes, key slot +
+   * 8 bytes per result row of scratch. */
+  MRHBM_RED_DISTINCT = 2
 };
 
 /* built-in combinerfn, run on the map side (job.lua:92-96,198-202: reducing the combined values must give what
@@ -123,7 +141,8 @@ typedef struct mrhbm_config {
  *   - the value field of a record (pool_read, result_copy) holds the pair's value id, its index in the emit pool,
  *     except that the pairs of one device piece of mrhbm_map_words_value share the id of the piece's first pair;
  *     fewer than 2^32 pairs may be emitted between mrhbm_reset calls, those of aborted and replaced jobs included.
- * The order of a key's values is unspecified, as for MRHBM_RED_NONE.  The new calls fail with MRHBM_E_INVAL on a ctx
+ * The order of a key's values is unspecified with MRHBM_RED_NONE; MRHBM_RED_DISTINCT gives each key's distinct values
+ * in ascending byte order.  The new calls fail with MRHBM_E_INVAL on a ctx
  * without the flag. */
 #define MRHBM_F_BYTE_VALUES 8u
 

@@ -125,6 +125,12 @@ struct mrhbm_ctx {
   void *dd_tab = nullptr, *dd_out = nullptr, *dd_rg = nullptr;
   uint32_t *dd_slot = nullptr, *dd_tiles = nullptr;
   uint64_t dd_tab_cap = 0, dd_rec_cap = 0, dd_rg_cap = 0, dd_tiles_cap = 0;  // entries, records, ranges, tiles
+  // MRHBM_RED_DISTINCT: the shuffle runs the same set over all committed pairs, and orders every bin's rows by value
+  // bytes; the merge of an oversized bin's chunks alternates with these scratch rows (out_cap of them)
+  bool red_distinct = false;
+  void* vo_keys = nullptr;
+  uint64_t* vo_ids = nullptr;
+  uint64_t vo_cap = 0;
   uint64_t N = 0, groups = 0;
   bool shuffled = false;
   std::vector<uint32_t> h_bin_off, h_uoff;
@@ -519,56 +525,72 @@ int ensure_compact(mrhbm_ctx* c) {
   return 0;
 }
 
-// MRHBM_COMBINE_DISTINCT, at commit: the map's open ranges are reduced to their distinct (key slot, value bytes) pairs
-// in place, the first copy of each in pool order surviving (mrhbm_distinct.cu), and its long-key pairs to their
-// distinct (key, value bytes) pairs.  kept receives every open range as (first, survivors); the caller shrinks the
-// ranges in the ledger once the whole commit has succeeded.
-int distinct_pairs(mrhbm_map* m, std::vector<std::pair<uint64_t, uint64_t>>& kept) {
-  mrhbm_ctx* c = m->ctx;
+// The distinct set over the pool ranges `ranges` (first, count; none empty): k_distinct_mark, k_distinct_count and the
+// scan of the tile counts (mrhbm_distinct.cu), then, when some pair repeats, k_distinct_scatter of the first copy of
+// each distinct (key slot, value bytes) pair, in pool order, to dd_out.  off[t] receives the survivors before tile t
+// (off.back(): all of them); rg the ranges as the kernels saw them (rg[k].tbase: the first tile of range k).
+// `what` names the caller in the error of a set larger than it takes; *launches (optional) += kernels launched.
+int distinct_set(mrhbm_ctx* c, const std::vector<std::pair<uint64_t, uint64_t>>& ranges, const char* what,
+                 std::vector<DistinctRange>& rg, std::vector<uint32_t>& off, uint32_t* launches = nullptr) {
   cudaStream_t s = c->stream;
-  kept = c->led.open_ranges(m->serial);
-  std::vector<DistinctRange> rg;
+  rg.clear();
   uint64_t n = 0, nt = 0;
-  for (const auto& r : kept) {
+  for (const auto& r : ranges) {
     rg.push_back(DistinctRange{r.first, n, (uint32_t)nt, 0});
     n += r.second;
     nt += (r.second + kDistinctTile - 1) / kDistinctTile;
   }
   rg.push_back(DistinctRange{0, n, (uint32_t)nt, 0});
+  off.assign(nt + 1, 0);
   const uint32_t nr = (uint32_t)rg.size() - 1;
-  if (n > (1ull << 31)) return fail(c, MRHBM_E_INVAL, "distinct combiner: a map job of %llu pairs (limit 2^31)", (unsigned long long)n);
-  if (n) {
-    uint64_t T = 1024;
-    while (T < 2 * n) T <<= 1;
-    int rc = grow(c, &c->dd_tab_cap, T, std::max(T, 2 * c->dd_tab_cap), {{&c->dd_tab, 16}});
-    if (!rc) rc = grow(c, &c->dd_rec_cap, n, n, {{(void**)&c->dd_slot, 4}, {&c->dd_out, (size_t)c->rb}});
-    if (!rc) rc = grow(c, &c->dd_rg_cap, nr + 1, nr + 1, {{&c->dd_rg, sizeof(DistinctRange)}});
-    if (!rc) rc = grow(c, &c->dd_tiles_cap, 2 * (nt + 1), 2 * (nt + 1), {{(void**)&c->dd_tiles, 4}});
-    if (rc) return rc;
-    uint32_t *tile_cnt = c->dd_tiles, *tile_off = c->dd_tiles + nt + 1;
-    const DistinctRange* drg = (const DistinctRange*)c->dd_rg;
-    CU(c, cudaMemsetAsync(c->dd_tab, 0xff, T * 16, s));
-    CU(c, cudaMemcpyAsync(c->dd_rg, rg.data(), rg.size() * sizeof(DistinctRange), cudaMemcpyHostToDevice, s));
-    launch_distinct_mark(c->rb, c->pool, drg, nr, (uint32_t)nt, c->arena, c->voff, c->dd_tab, T - 1, c->dd_slot, s);
-    launch_distinct_count(drg, nr, (uint32_t)nt, c->dd_tab, c->dd_slot, tile_cnt, s);
-    launch_exscan(tile_cnt, (uint32_t)nt, tile_off, nullptr, nullptr, 0xffffffffu, nullptr, nullptr, nullptr, 0, s,
-                  c->d_small + 64);
+  if (n > (1ull << 31)) return fail(c, MRHBM_E_INVAL, "%s: %llu pairs (limit 2^31)", what, (unsigned long long)n);
+  if (!n) return 0;
+  uint64_t T = 1024;
+  while (T < 2 * n) T <<= 1;
+  int rc = grow(c, &c->dd_tab_cap, T, std::max(T, 2 * c->dd_tab_cap), {{&c->dd_tab, 16}});
+  if (!rc) rc = grow(c, &c->dd_rec_cap, n, n, {{(void**)&c->dd_slot, 4}, {&c->dd_out, (size_t)c->rb}});
+  if (!rc) rc = grow(c, &c->dd_rg_cap, nr + 1, nr + 1, {{&c->dd_rg, sizeof(DistinctRange)}});
+  if (!rc) rc = grow(c, &c->dd_tiles_cap, 2 * (nt + 1), 2 * (nt + 1), {{(void**)&c->dd_tiles, 4}});
+  if (rc) return rc;
+  uint32_t *tile_cnt = c->dd_tiles, *tile_off = c->dd_tiles + nt + 1;
+  const DistinctRange* drg = (const DistinctRange*)c->dd_rg;
+  CU(c, cudaMemsetAsync(c->dd_tab, 0xff, T * 16, s));
+  CU(c, cudaMemcpyAsync(c->dd_rg, rg.data(), rg.size() * sizeof(DistinctRange), cudaMemcpyHostToDevice, s));
+  uint32_t k = launch_distinct_mark(c->rb, c->pool, drg, nr, (uint32_t)nt, c->arena, c->voff, c->dd_tab, T - 1, c->dd_slot, s);
+  k += launch_distinct_count(drg, nr, (uint32_t)nt, c->dd_tab, c->dd_slot, tile_cnt, s);
+  k += launch_exscan(tile_cnt, (uint32_t)nt, tile_off, nullptr, nullptr, 0xffffffffu, nullptr, nullptr, nullptr, 0, s,
+                     c->d_small + 64);
+  CU(c, cudaGetLastError());
+  CU(c, cudaMemcpyAsync(off.data(), tile_off, (nt + 1) * 4, cudaMemcpyDeviceToHost, s));
+  CU(c, cudaStreamSynchronize(s));
+  if (off[nt] < n) {
+    k += launch_distinct_scatter(c->rb, c->pool, drg, nr, (uint32_t)nt, c->dd_tab, c->dd_slot, tile_off, c->dd_out, s);
     CU(c, cudaGetLastError());
-    std::vector<uint32_t> off(nt + 1);
-    CU(c, cudaMemcpyAsync(off.data(), tile_off, (nt + 1) * 4, cudaMemcpyDeviceToHost, s));
-    CU(c, cudaStreamSynchronize(s));
-    if (off[nt] < n) {
-      launch_distinct_scatter(c->rb, c->pool, drg, nr, (uint32_t)nt, c->dd_tab, c->dd_slot, tile_off, c->dd_out, s);
-      CU(c, cudaGetLastError());
-      for (size_t k = 0; k < kept.size(); k++) {
-        const uint64_t a = off[rg[k].tbase], b = off[rg[k + 1].tbase];
-        if (b - a < kept[k].second && b > a)
-          CU(c, cudaMemcpyAsync((char*)c->pool + kept[k].first * c->rb, (char*)c->dd_out + a * c->rb, (b - a) * c->rb,
-                                cudaMemcpyDeviceToDevice, s));
-        kept[k].second = b - a;
-      }
-      CU(c, cudaStreamSynchronize(s));
+  }
+  if (launches) *launches += k;
+  return 0;
+}
+
+// MRHBM_COMBINE_DISTINCT, at commit: the map's open ranges are reduced to their distinct (key slot, value bytes) pairs
+// in place, the first copy of each in pool order surviving (distinct_set), and its long-key pairs to their distinct
+// (key, value bytes) pairs.  kept receives every open range as (first, survivors); the caller shrinks the ranges in
+// the ledger once the whole commit has succeeded.
+int distinct_pairs(mrhbm_map* m, std::vector<std::pair<uint64_t, uint64_t>>& kept) {
+  mrhbm_ctx* c = m->ctx;
+  kept = c->led.open_ranges(m->serial);
+  std::vector<DistinctRange> rg;
+  std::vector<uint32_t> off;
+  int rc = distinct_set(c, kept, "distinct combiner: a map job", rg, off);
+  if (rc) return rc;
+  if (off.back() < rg.back().vbase) {
+    for (size_t k = 0; k < kept.size(); k++) {
+      const uint64_t a = off[rg[k].tbase], b = off[rg[k + 1].tbase];
+      if (b - a < kept[k].second && b > a)
+        CU(c, cudaMemcpyAsync((char*)c->pool + kept[k].first * c->rb, (char*)c->dd_out + a * c->rb, (b - a) * c->rb,
+                              cudaMemcpyDeviceToDevice, c->stream));
+      kept[k].second = b - a;
     }
+    CU(c, cudaStreamSynchronize(c->stream));
   }
   std::set<std::pair<std::string, std::string>> seen;
   std::vector<LongPair> longs;
@@ -635,15 +657,18 @@ int mrhbm_init(const mrhbm_config* cfg, mrhbm_ctx** out) {
       return fail(c, MRHBM_E_INVAL, "string keys need partitioner FNV_LUA, WORDHASH or RANGE");
   } else
     return fail(c, MRHBM_E_INVAL, "unknown key_kind %u", cfg->key_kind);
-  if (cfg->reducer != MRHBM_RED_SUM && cfg->reducer != MRHBM_RED_NONE) return fail(c, MRHBM_E_INVAL, "unknown reducer %u", cfg->reducer);
+  if (cfg->reducer > MRHBM_RED_DISTINCT) return fail(c, MRHBM_E_INVAL, "unknown reducer %u", cfg->reducer);
   if (cfg->combiner > MRHBM_COMBINE_DISTINCT) return fail(c, MRHBM_E_INVAL, "unknown combiner %u", cfg->combiner);
   if (cfg->combiner == MRHBM_COMBINE_DISTINCT && !(cfg->flags & MRHBM_F_BYTE_VALUES))
     return fail(c, MRHBM_E_INVAL, "combiner MRHBM_COMBINE_DISTINCT needs byte values (MRHBM_F_BYTE_VALUES)");
   if (cfg->reducer == MRHBM_RED_NONE && cfg->combiner == MRHBM_COMBINE_REDUCER) return fail(c, MRHBM_E_INVAL, "a general reducer cannot be combined on the device (combiner must be 0)");
-  if ((cfg->flags & MRHBM_F_BYTE_VALUES) && (cfg->reducer != MRHBM_RED_NONE || cfg->combiner == MRHBM_COMBINE_REDUCER))
-    return fail(c, MRHBM_E_INVAL, "byte values (MRHBM_F_BYTE_VALUES) need reducer MRHBM_RED_NONE and combiner 0 or MRHBM_COMBINE_DISTINCT");
+  if (cfg->reducer == MRHBM_RED_DISTINCT && !(cfg->flags & MRHBM_F_BYTE_VALUES))
+    return fail(c, MRHBM_E_INVAL, "reducer MRHBM_RED_DISTINCT needs byte values (MRHBM_F_BYTE_VALUES)");
+  if ((cfg->flags & MRHBM_F_BYTE_VALUES) && (cfg->reducer == MRHBM_RED_SUM || cfg->combiner == MRHBM_COMBINE_REDUCER))
+    return fail(c, MRHBM_E_INVAL, "byte values (MRHBM_F_BYTE_VALUES) need reducer MRHBM_RED_NONE or MRHBM_RED_DISTINCT and combiner 0 or MRHBM_COMBINE_DISTINCT");
   c->bytevals = c->led.byte_values = (cfg->flags & MRHBM_F_BYTE_VALUES) != 0;
-  c->sb.no_reduce = cfg->reducer == MRHBM_RED_NONE;
+  c->red_distinct = cfg->reducer == MRHBM_RED_DISTINCT;
+  c->sb.no_reduce = cfg->reducer != MRHBM_RED_SUM;
   CU(c, cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
   if (cfg->partitioner == MRHBM_PART_RANGE && cfg->num_partitions == 1) {  // one key range, no splitters: its table now
     int rc = install_splitters(c, {});
@@ -688,7 +713,7 @@ void mrhbm_destroy(mrhbm_ctx* c) {
                    c->gtab,        c->l1buf,       c->regions,    c->d_l1all,     c->d_sample,   c->d_tok_text[0],
                    c->d_tok_text[1], c->d_tok_cnt, c->d_tok_off, c->d_spl,     c->arena,       c->voff,
                    c->cvals,       c->row_off,     c->val_tile,   c->val_pieces, c->dd_tab,     c->dd_out,
-                   c->dd_rg,       c->dd_slot,     c->dd_tiles};
+                   c->dd_rg,       c->dd_slot,     c->dd_tiles,   c->vo_keys,    c->vo_ids};
   for (void* p : frees)
     if (p) cudaFree(p);
   if (c->h_counters) cudaFreeHost(c->h_counters);
@@ -1338,15 +1363,28 @@ struct Src {
 // with their sum (shared-memory table per SM + one L2-resident global table, see k_combine).  A rank-local
 // decision: the stages that follow only see "the pairs this rank contributes".  The combiner never fails a
 // shuffle: when a string key's sum does not fit the u32 value of a combined record (or one value is too large
-// for the table's state word), this shuffle hands on the raw pairs instead.  EV_START .. EV_CSTART.
+// for the table's state word), this shuffle hands on the raw pairs instead.  MRHBM_RED_DISTINCT: the first copy of
+// each distinct (key slot, value bytes) pair over all committed pairs (distinct_set), in the set's scratch; the pool
+// and the ledger stay as they are.  EV_START .. EV_CSTART.
 int collect_sources(mrhbm_ctx* c, std::vector<Src>& srcs, uint64_t* N, mrhbm_stats& st) {
   srcs.clear();
   uint64_t n = 0;
+  std::vector<std::pair<uint64_t, uint64_t>> live;
   for (auto& r : c->led.live()) {
     srcs.push_back(Src{(const char*)c->pool + r.first * c->rb, r.second});
+    if (r.second) live.push_back(r);
     n += r.second;
   }
   *N = n;
+  if (c->red_distinct) {
+    std::vector<DistinctRange> rg;
+    std::vector<uint32_t> off;
+    int rc = distinct_set(c, live, "distinct reducer: a shuffle of", rg, off, &st.launches);
+    if (rc || off.back() == n) return rc;
+    srcs.assign(1, Src{(const char*)c->dd_out, off.back()});
+    *N = off.back();
+    return 0;
+  }
   if (c->cfg.combiner != MRHBM_COMBINE_REDUCER || c->no_combine || n < (1u << 20)) return 0;
   cudaStream_t s = c->stream;
   bool checked = c->combine_checked;
@@ -1510,14 +1548,31 @@ int exact_split(mrhbm_ctx* c, const std::vector<Src>& live, const RangeBinParams
   return 0;
 }
 
+// MRHBM_RED_DISTINCT, after the sort of the nb bins of view v and k_big_bins: every bin's rows in (key, value bytes)
+// order, an oversized bin (nbig of them) as one run (mrhbm_value_order.cu).  Inside ms_bigbins.
+int order_values(mrhbm_ctx* c, const ShuffleBuffers& v, uint64_t nb, uint32_t nbig, mrhbm_stats& st) {
+  st.launches += launch_value_order(c->rb, v, (uint32_t)nb, nbig, c->cap, c->arena, c->voff, c->stream);
+  if (nbig) {
+    int rc = grow(c, &c->vo_cap, c->out_cap, c->out_cap, {{&c->vo_keys, (size_t)c->kb}, {(void**)&c->vo_ids, sizeof(uint64_t)}});
+    if (rc) return rc;
+    st.launches += launch_value_merge(c->rb, v, nbig, c->cap, c->arena, c->voff, c->vo_keys, c->vo_ids, c->stream);
+  }
+  CU(c, cudaGetLastError());
+  return 0;
+}
+
 // Exact layout, after the sort of the nb bins of view v (nbig of them oversized): k_big_bins, the group offsets, and
 // the bin offsets (v.bin_off), group offsets and counters read back.  EV_BIG, EV_END; synchronises the stream.
 int exact_tail(mrhbm_ctx* c, const ShuffleBuffers& v, uint64_t nb, uint32_t nbig, mrhbm_stats& st) {
   cudaStream_t s = c->stream;
   st.launches += launch_big_bins(c->rb, v, nbig, c->cap, s);
+  if (c->red_distinct) {
+    int rc = order_values(c, v, nb, nbig, st);
+    if (rc) return rc;
+  }
   CU(c, cudaEventRecord(c->ev[EV_BIG], s));
   c->h_big.clear();
-  if (c->sb.no_reduce && nbig) {  // group-only mode: the iterator merges the runs of an oversized bin
+  if (c->sb.no_reduce && !c->red_distinct && nbig) {  // group-only mode: the iterator merges the runs of an oversized bin
     c->h_big.resize(nbig);
     CU(c, cudaMemcpyAsync(c->h_big.data(), c->sb.big_list, nbig * 4, cudaMemcpyDeviceToHost, s));
   }
@@ -1700,6 +1755,7 @@ int shuffle_fast(mrhbm_ctx* c, std::vector<Src>& live, uint64_t N, uint64_t N_in
   set_range_hint(c, v, S, ordered);
   if (Bl) st.launches += launch_sort_reduce(c->rb, v, (uint32_t)Bl, c->cap, c->sm_count, s);
   CU(c, cudaEventRecord(c->ev[EV_SORT], s));
+  if (c->red_distinct && (rc = order_values(c, v, Bl, 0, st))) return rc;
   CU(c, cudaEventRecord(c->ev[EV_BIG], s));
   c->h_uoff.assign(Bl + 1, 0);
   if (Bl) {
@@ -2052,7 +2108,7 @@ int build_long_groups(mrhbm_ctx* c) {
   }
   // group the pairs of the partitions this rank owns (partition p lives on rank p % G, slot p / G)
   std::vector<std::map<std::string, std::vector<uint64_t>>> acc(c->Pl);
-  const bool sum = c->cfg.reducer != MRHBM_RED_NONE;
+  const bool sum = !c->sb.no_reduce;
   for (size_t w = 0; w + 3 <= all_blobs.size();) {
     const uint32_t klen = all_blobs[w];
     uint64_t v;
@@ -2072,6 +2128,13 @@ int build_long_groups(mrhbm_ctx* c) {
   c->long_groups.resize(c->Pl);
   for (uint32_t sl = 0; sl < c->Pl; sl++)
     for (auto& kv : acc[sl]) {  // std::map iterates in ascending bytewise key order (unsigned char_traits compare)
+      if (c->red_distinct) {  // the key's distinct values, ascending by their bytes (std::string compares unsigned)
+        std::vector<uint64_t>& vals = kv.second;
+        auto bytes = [c](uint64_t i) -> const std::string& { return *c->long_vals[i]; };
+        std::sort(vals.begin(), vals.end(), [&](uint64_t a, uint64_t b) { return bytes(a) < bytes(b); });
+        vals.erase(std::unique(vals.begin(), vals.end(), [&](uint64_t a, uint64_t b) { return bytes(a) == bytes(b); }),
+                   vals.end());
+      }
       c->long_groups[sl].push_back(LongGroup{kv.first, std::move(kv.second)});
       c->long_group_count++;
     }
@@ -2428,7 +2491,7 @@ static int next_group(mrhbm_iter* it, const LongGroup** lg) {
   const unsigned char* k = &it->keys[i * c->kb];
   it->rows.clear();
   it->rows.push_back(i);
-  if (c->cfg.reducer == MRHBM_RED_NONE) {
+  if (c->sb.no_reduce) {
     // every row of this key: adjacent in its run, and -- for an oversized bin -- at the head of
     // sibling runs too
     for (;;) {  // the run on top, then whichever run comes to the top with the same key

@@ -11,6 +11,7 @@
 #include <cstdint>
 
 #include "mrhbm_dev.cuh"
+#include "mrhbm_valbytes.cuh"
 
 namespace mrhbm {
 
@@ -39,29 +40,6 @@ __device__ __forceinline__ bool tile_record(const DistinctRange* __restrict__ rg
   return true;
 }
 
-// A value's bytes as little-endian 32-bit words, whatever the alignment of its first byte in the arena: word i holds
-// bytes 4i .. 4i+3, zero past the end.  Only aligned words that hold a byte of the value are read.
-struct ValView {
-  const uint32_t* w;
-  uint32_t sh;
-  uint64_t len;
-};
-__device__ __forceinline__ ValView val_view(const unsigned char* __restrict__ arena, const uint64_t* __restrict__ voff,
-                                            uint64_t id) {
-  const uint64_t s = voff[id];
-  ValView v;
-  v.len = voff[id + 1] - s;
-  v.sh = (uint32_t)(s & 3);
-  v.w = (const uint32_t*)(arena + s - v.sh);
-  return v;
-}
-__device__ __forceinline__ uint32_t val_word(const ValView& v, uint64_t i) {
-  uint32_t x = __ldg(v.w + i);
-  if (v.sh) x = __funnelshift_r(x, 4 * (i + 1) < v.sh + v.len ? __ldg(v.w + i + 1) : 0u, 8 * v.sh);
-  const uint64_t rem = v.len - 4 * i;
-  return rem < 4 ? x & ((1u << (8 * rem)) - 1) : x;
-}
-
 __device__ __forceinline__ uint64_t fp_step(uint64_t h, uint64_t x) {
   h = (h ^ x) * 0x9E3779B97F4A7C15ull;
   return h ^ (h >> 29);
@@ -87,12 +65,7 @@ __device__ __forceinline__ bool same_pair(const uint32_t* r, uint64_t id, const 
   if (!key_eq<RB>(r, q)) return false;
   const uint64_t qid = rec_value<RB>(q);
   if (qid == id) return true;  // (the pairs of one tokeniser piece share their id)
-  const ValView u = val_view(arena, voff, qid);
-  if (u.len != v.len) return false;
-  const uint64_t nw = (v.len + 3) / 4;
-  for (uint64_t i = 0; i < nw; i++)
-    if (val_word(u, i) != val_word(v, i)) return false;
-  return true;
+  return val_eq(val_view(arena, voff, qid), v);
 }
 
 template <int RB>

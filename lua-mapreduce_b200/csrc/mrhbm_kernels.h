@@ -270,4 +270,13 @@ int launch_distinct_scatter(int rb, const void* pool, const DistinctRange* rg, u
                             const void* tab, const uint32_t* slot_of, const uint32_t* tile_off, void* out,
                             cudaStream_t s);
 
+// ---- MRHBM_RED_DISTINCT (mrhbm_value_order.cu) ----
+// Every bin's rows (ucount[bin] of them at out_start, sorted by key, value ids in out_sums) in (key, value bytes)
+// order: the nb bins of at most cap rows, and the cap-row chunks of the nbig oversized bins of big_list
+int launch_value_order(int rb, const ShuffleBuffers& b, uint32_t nb, uint32_t nbig, uint32_t cap,
+                       const unsigned char* arena, const uint64_t* voff, cudaStream_t s);
+// then each oversized bin's chunks merged into one run; tmp_keys / tmp_ids: scratch rows laid out as out_keys / out_sums
+int launch_value_merge(int rb, const ShuffleBuffers& b, uint32_t nbig, uint32_t cap, const unsigned char* arena,
+                       const uint64_t* voff, void* tmp_keys, uint64_t* tmp_ids, cudaStream_t s);
+
 }  // namespace mrhbm

@@ -139,6 +139,7 @@ class Job:
 
         decode = tuple_keys.decode if cfg["hbm"]["key_kind"] == "tuple" else None
         byte_values = cfg["hbm"].get("value_kind") == "bytes"
+        device_distinct = cfg["hbm"].get("reducer") == 2  # hbm_reducefn = "distinct": the values are its output
         bulk = self._bulk_groups(part) if (aci and cfg["hbm"].get("reducer", 0) == 0 and decode is None) else None
         if bulk is not None:
             # built-in reducer + ACI flags: every value list is the singleton the device produced and the reference
@@ -155,7 +156,7 @@ class Job:
             # The device applied the declared built-in (combiner semantics).  The reference
             # skips the reducer on singletons when the ACI flags are set (job.lua:264-274),
             # otherwise it always calls it (job.lua:275-284).
-            if not (aci and len(values) == 1):
+            if not device_distinct and not (aci and len(values) == 1):
                 del result[:]
                 mod.reducefn(key, values, emit)
                 values = list(result)

@@ -66,6 +66,26 @@ def distinct_combiner(comb, value_kind):
                              "distinct values: the declaration must describe what the combinerfn computes" % (values, out))
 
 
+def distinct_reducer(red, value_kind):
+    """Checks a reducefn module that declares hbm_reducefn = "distinct": the device then hands every key its distinct
+    values, ascending by their encoded bytes, and the reducefn is not called, so it must emit exactly that sequence."""
+    from .tuple import encode_value
+    if value_kind != "bytes":
+        raise ValueError("hbm_reducefn = 'distinct' orders string and number values by their bytes: "
+                         "configure hbm = {'value_kind': 'bytes'}")
+    for values in _DISTINCT_PROBES:
+        out = []
+        try:
+            red.reducefn(b"probe", list(values), out.append)
+            got = [encode_value(v) for v in out]
+        except Exception as e:
+            raise ValueError("hbm_reducefn = 'distinct': reducefn failed on the values %r: %r" % (values, e))
+        if got != sorted({encode_value(v) for v in values}):
+            raise ValueError("hbm_reducefn = 'distinct', but reducefn turns the values %r into %r instead of their "
+                             "distinct values in ascending order: the declaration must describe what the reducefn "
+                             "computes" % (values, out))
+
+
 class server:
     def __init__(self, connection_string, dbname, auth_table=None):
         self.cnn_string, self.dbname = connection_string, dbname
@@ -105,8 +125,8 @@ class server:
         # associative/commutative/idempotent flags, examples/WordCount/reducefn.lua:10-14)
         red, part = mods["reducefn"], mods["partitionfn"]
         builtin_red = getattr(red, "hbm_reducefn", None)
-        if builtin_red not in (None, "sum"):
-            raise NotImplementedError("unknown hbm_reducefn %r (built-ins: 'sum')" % (builtin_red,))
+        if builtin_red not in (None, "sum", "distinct"):
+            raise NotImplementedError("unknown hbm_reducefn %r (built-ins: 'sum', 'distinct')" % (builtin_red,))
         # no declaration = general reducer: the device partitions, sorts and groups, reducefn runs
         # on the host per group (job.lua:264-284); values are unsigned integers < 2^32
         # A combinerfn only ever runs on the device, as the declared built-in (it must equal the reducefn there).
@@ -133,9 +153,12 @@ class server:
         # value_kind = "bytes": values are Lua strings and numbers (tuple.encode_value), handed to a general reducefn
         if hbm["value_kind"] not in ("int", "bytes"):
             raise ValueError("hbm value_kind must be 'int' or 'bytes', got %r" % (hbm["value_kind"],))
-        if hbm["value_kind"] == "bytes" and builtin_red is not None:
+        if hbm["value_kind"] == "bytes" and builtin_red not in (None, "distinct"):
             raise ValueError("hbm value_kind = 'bytes' hands string and number values to a general reducefn: "
-                             "the reducefn module must not declare hbm_reducefn (it declares %r)" % (builtin_red,))
+                             "the reducefn module must not declare an hbm_reducefn other than 'distinct' (it declares "
+                             "%r)" % (builtin_red,))
+        if builtin_red == "distinct":  # every key's distinct values, ascending, on the device: reducefn is not called
+            distinct_reducer(red, hbm["value_kind"])
         if getattr(mods["mapfn"], "hbm_mapfn", None) == "words_file" and hbm["value_kind"] != "bytes":
             raise ValueError("hbm_mapfn = 'words_file' pairs every word with the file name, a string value: "
                              "configure hbm = {'value_kind': 'bytes'}")
@@ -143,7 +166,7 @@ class server:
             distinct_combiner(mods["combinerfn"], hbm["value_kind"])
         hbm.update(partitioner=_BUILTIN_PART[pname], num_partitions=nparts,
                    combiner="distinct" if distinct else device_combiner,
-                   reducer=0 if builtin_red == "sum" else 1,
+                   reducer={"sum": 0, "distinct": 2}.get(builtin_red, 1),
                    splitters=range_splitters(part, nparts, hbm["key_kind"]) if pname == "range" else None)
         self.config = dict(mapfn=params["mapfn"], reducefn=params["reducefn"], partitionfn=params["partitionfn"],
                            combinerfn=params.get("combinerfn"), init_args=self.init_args,
