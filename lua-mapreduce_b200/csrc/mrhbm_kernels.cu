@@ -15,6 +15,7 @@
 
 #include "mrhbm_dev.cuh"
 #include "mrhbm_sort.cuh"
+#include "mrhbm_split_plan.h"
 
 namespace mrhbm {
 
@@ -1699,19 +1700,7 @@ int launch_split_l2(int rb, const RangeBinParams& bp, const SplitPlan& pl, cudaS
   const int ctas = 2 * g_sm_count;
   const uint32_t regions = pl.C1_local;
   if (!regions) return 0;
-  // x CTAs per region (each takes every x-th tile of all the region's streams), chosen so that all CTAs fill whole waves of `ctas` resident CTAs
-  // (e.g. C1 = 220, x = 2 on 264 slots would run 440 CTAs = 1.67 waves: a third of the second wave idle)
-  int x = 1;
-  double best = 0;
-  const uint64_t tiles = pl.ndest * ((pl.sub_stride * rb + kSplitTileBytes - 1) / kSplitTileBytes);
-  for (int cand = 1; cand <= 16 && (uint64_t)cand <= std::max<uint64_t>(1, tiles / 4); cand++) {
-    uint64_t total = (uint64_t)cand * regions, waves = (total + ctas - 1) / ctas;
-    double eff = (double)total / (double)(waves * ctas);
-    if (eff > best + 0.02) {
-      best = eff;
-      x = cand;
-    }
-  }
+  const int x = split_l2_ctas_per_region(regions, pl.sub_stride, pl.ndest, rb, ctas);
   DISPATCH_RB(rb, (launch_split_rb<RB>(dim3(x, regions), pl, 2, nullptr, 0, bp, s)));
   return 1;
 }
