@@ -87,7 +87,32 @@ enum {
    * distinct set of MRHBM_COMBINE_DISTINCT sized for all committed pairs (16 bytes x a power of two >= 2 x pairs, plus
    * 4 + record bytes per pair), and, in a shuffle with a bin of more rows than one shared-memory sort takes, key slot +
    * 8 bytes per result row of scratch. */
-  MRHBM_RED_DISTINCT = 2
+  MRHBM_RED_DISTINCT = 2,
+  /* MRHBM_F_BYTE_VALUES only, with combiner MRHBM_COMBINE_NONE (any other combination fails mrhbm_init with
+   * MRHBM_E_INVAL; one GPU, as byte values are): the reducefn "count = count + v" over Lua numbers (weighted word
+   * counts, PageRank contributions, loss totals), computed on the device -- no host reducefn runs.  Every value must be
+   * a number as the bindings encode it (mapreduce/tuple.py _enc_num with key=False, hbm.lua enc_num): 11 bytes, 0x10,
+   * then the IEEE double's bits u sign-folded (u | 2^63 when the sign bit is 0, ~u when it is 1) as ten big-endian
+   * 7-bit groups of u (the first holding bit 63 alone), each OR 0x80.  A value that is not such an encoding, or that
+   * encodes a NaN, fails mrhbm_shuffle with MRHBM_E_INVAL and leaves no result (Lua's arithmetic on a non-number
+   * breaks the reduce job).  After mrhbm_shuffle there is exactly one row per key; its value is the key's values
+   * summed exactly and rounded once to the nearest double, ties to even: float(sum(Fraction(v) for v in values)) in
+   * Python.  A sum whose magnitude rounds beyond DBL_MAX is +-inf; infinities of one sign give that infinity; +inf and
+   * -inf on one key fail mrhbm_shuffle with MRHBM_E_INVAL (Lua would make a NaN, which the reference's "%.14g" spill
+   * cannot load back); an exact zero is +0 unless every value is -0, then -0.  The result does not depend on emission
+   * order, map jobs, bins or runs, and is bit-identical for every MRHBM_F_* layout flag.  Where the reference's own
+   * left-to-right double sum is exact (integers whose partial sums stay below 2^53, say) the two are equal, so an
+   * integer word count gives what MRHBM_RED_SUM gives.  Reading the result: mrhbm_groups_next_values gives every
+   * group, long keys included, its one value in the encoding above; mrhbm_result_values gives one value per
+   * mrhbm_result_copy row, and the row's value field is the row index.  mrhbm_result_info: pairs_in = committed pairs,
+   * pairs_recv = pairs the shuffle carried, groups = keys.  mrhbm_checksum_result's out[3..5] keep their meaning;
+   * in[0..2] == out[0..2] does not hold (a row holds a sum, not a value id).  The summing kernels are timed in
+   * mrhbm_stats.ms_bigbins, inside ms_total.  Limits: fewer than 2^31 committed pairs per shuffle (else
+   * MRHBM_E_INVAL).  Extra device memory: 11 bytes of value and 8 of offset per result row; and, in a shuffle with a
+   * bin of more rows than one shared-memory sort takes, key slot + 8 bytes per result row of merge scratch and, for
+   * the groups that span a chunk of such a bin, partial accumulators of 1096 bytes per slot, 2 ceil(rows / cap) + 2
+   * slots (cap = 32 KB / record bytes). */
+  MRHBM_RED_FSUM = 3
 };
 
 /* built-in combinerfn, run on the map side (job.lua:92-96,198-202: reducing the combined values must give what
@@ -131,7 +156,8 @@ typedef struct mrhbm_config {
 #define MRHBM_F_SMALL_BINS 2u   /* test hook: tiny smem bins to exercise the overflow paths */
 #define MRHBM_F_NO_OPTIMISTIC 4u /* always run the exact two-pass (histogram) partition layout */
 /* Byte-string values (lua-mapreduce's emit(key, value) takes any Lua string or number, utils.lua:100-120): a value is
- * opaque bytes, 0 to 1 GiB long, carried through group-only mode.  Needs reducer = MRHBM_RED_NONE and combiner
+ * opaque bytes, 0 to 1 GiB long, carried through group-only mode.  Needs reducer = MRHBM_RED_NONE (or a byte-values
+ * reducer: MRHBM_RED_DISTINCT, MRHBM_RED_FSUM) and combiner
  * MRHBM_COMBINE_NONE or MRHBM_COMBINE_DISTINCT (else mrhbm_init fails with MRHBM_E_INVAL) and one GPU (mrhbm_comm_init with world > 1 fails).  On such a ctx:
  *   - pairs are emitted with mrhbm_emit_str_value / mrhbm_emit_u64_value / mrhbm_emit_batch_values /
  *     mrhbm_map_words_value; the integer-valued emits (emit_str, emit_u64, emit_batch, emit_device, map_gen_*,
@@ -142,7 +168,7 @@ typedef struct mrhbm_config {
  *     except that the pairs of one device piece of mrhbm_map_words_value share the id of the piece's first pair;
  *     fewer than 2^32 pairs may be emitted between mrhbm_reset calls, those of aborted and replaced jobs included.
  * The order of a key's values is unspecified with MRHBM_RED_NONE; MRHBM_RED_DISTINCT gives each key's distinct values
- * in ascending byte order.  The new calls fail with MRHBM_E_INVAL on a ctx
+ * in ascending byte order; MRHBM_RED_FSUM gives each key one value, the exact sum of its numbers.  The new calls fail with MRHBM_E_INVAL on a ctx
  * without the flag. */
 #define MRHBM_F_BYTE_VALUES 8u
 

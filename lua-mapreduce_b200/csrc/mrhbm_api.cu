@@ -7,6 +7,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <deque>
 #include <initializer_list>
 #include <map>
 #include <mutex>
@@ -20,6 +21,7 @@
 #include "mrhbm_kernels.h"
 #include "mrhbm_dev.cuh"  // splitmix64
 #include "mrhbm_keys.h"
+#include "mrhbm_numsum.cuh"
 #include "mrhbm_pool.h"
 #include "mrhbm_split_plan.h"
 
@@ -64,6 +66,7 @@ struct mrhbm_ctx {
   uint64_t *row_off = nullptr, *val_tile = nullptr, *val_pieces = nullptr;
   uint64_t cvals_cap = 0, row_cap = 0, tile_cap = 0, pieces_cap = 0, cvals_bytes = 0;
   std::vector<const std::string*> long_vals;  // values of the long-key groups (LongGroup::values index them)
+  std::deque<std::string> long_sums;          // MRHBM_RED_FSUM: the long-key groups' encoded sums (long_vals point here)
   // Keys that do not fit a record slot (rare: the reference takes any key length, utils.lua:104-110) never reach the
   // device: their pairs wait on the host, per committed map job, are partitioned and grouped at the barrier (on several
   // GPUs after an all-gather) and merged into the reduce-side iteration at their place in the key order.
@@ -132,6 +135,12 @@ struct mrhbm_ctx {
   void* vo_keys = nullptr;
   uint64_t* vo_ids = nullptr;
   uint64_t vo_cap = 0;
+  // MRHBM_RED_FSUM: the shuffle sums every key's numbers (mrhbm_num_sum.cu); the partial accumulators of the groups
+  // that cross a chunk of an oversized bin live here (ns_cap slots, see NumScratch)
+  bool red_fsum = false;
+  int64_t* ns_acc = nullptr;
+  uint32_t *ns_flags = nullptr, *ns_head = nullptr;
+  uint64_t ns_cap = 0;
   uint64_t N = 0, groups = 0;
   bool shuffled = false;
   std::vector<uint32_t> h_bin_off, h_uoff;
@@ -443,6 +452,7 @@ void invalidate(mrhbm_ctx* c) {
   c->long_groups.clear();
   c->long_group_count = 0;
   c->long_vals.clear();
+  c->long_sums.clear();
 }
 
 struct DevBuf {
@@ -501,7 +511,16 @@ int ensure_compact(mrhbm_ctx* c) {
   if (rc) return rc;
   launch_compact(c->rb, c->rv, c->B, c->ckeys, c->csums, c->stream);
   CU(c, cudaGetLastError());
-  if (c->bytevals) {
+  if (c->red_fsum) {
+    // every row's sum (double bits) is in csums: its 11-byte number at cvals[11 r ..), and the row index as its id
+    const uint64_t n = c->groups;
+    rc = grow(c, &c->row_cap, n + 1, n + 1, {{(void**)&c->row_off, sizeof(uint64_t)}});
+    if (!rc) rc = grow(c, &c->cvals_cap, kNumBytes * n + 1, kNumBytes * n + 1, {{(void**)&c->cvals, 1}});
+    if (rc) return rc;
+    launch_num_encode(c->csums, n, c->cvals, c->row_off, c->stream);
+    CU(c, cudaGetLastError());
+    c->cvals_bytes = kNumBytes * n;
+  } else if (c->bytevals) {
     // the value id of every row is in csums: lengths, their offsets, then the bytes in row order
     const uint64_t n = c->groups, nt = val_tiles(n);
     rc = grow(c, &c->row_cap, n + 1, n + 1, {{(void**)&c->row_off, sizeof(uint64_t)}});
@@ -658,17 +677,20 @@ int mrhbm_init(const mrhbm_config* cfg, mrhbm_ctx** out) {
       return fail(c, MRHBM_E_INVAL, "string keys need partitioner FNV_LUA, WORDHASH or RANGE");
   } else
     return fail(c, MRHBM_E_INVAL, "unknown key_kind %u", cfg->key_kind);
-  if (cfg->reducer > MRHBM_RED_DISTINCT) return fail(c, MRHBM_E_INVAL, "unknown reducer %u", cfg->reducer);
+  if (cfg->reducer > MRHBM_RED_FSUM) return fail(c, MRHBM_E_INVAL, "unknown reducer %u", cfg->reducer);
   if (cfg->combiner > MRHBM_COMBINE_DISTINCT) return fail(c, MRHBM_E_INVAL, "unknown combiner %u", cfg->combiner);
   if (cfg->combiner == MRHBM_COMBINE_DISTINCT && !(cfg->flags & MRHBM_F_BYTE_VALUES))
     return fail(c, MRHBM_E_INVAL, "combiner MRHBM_COMBINE_DISTINCT needs byte values (MRHBM_F_BYTE_VALUES)");
   if (cfg->reducer == MRHBM_RED_NONE && cfg->combiner == MRHBM_COMBINE_REDUCER) return fail(c, MRHBM_E_INVAL, "a general reducer cannot be combined on the device (combiner must be 0)");
   if (cfg->reducer == MRHBM_RED_DISTINCT && !(cfg->flags & MRHBM_F_BYTE_VALUES))
     return fail(c, MRHBM_E_INVAL, "reducer MRHBM_RED_DISTINCT needs byte values (MRHBM_F_BYTE_VALUES)");
+  if (cfg->reducer == MRHBM_RED_FSUM && (!(cfg->flags & MRHBM_F_BYTE_VALUES) || cfg->combiner != MRHBM_COMBINE_NONE))
+    return fail(c, MRHBM_E_INVAL, "reducer MRHBM_RED_FSUM needs byte values (MRHBM_F_BYTE_VALUES) and combiner MRHBM_COMBINE_NONE");
   if ((cfg->flags & MRHBM_F_BYTE_VALUES) && (cfg->reducer == MRHBM_RED_SUM || cfg->combiner == MRHBM_COMBINE_REDUCER))
-    return fail(c, MRHBM_E_INVAL, "byte values (MRHBM_F_BYTE_VALUES) need reducer MRHBM_RED_NONE or MRHBM_RED_DISTINCT and combiner 0 or MRHBM_COMBINE_DISTINCT");
+    return fail(c, MRHBM_E_INVAL, "byte values (MRHBM_F_BYTE_VALUES) need reducer MRHBM_RED_NONE, MRHBM_RED_DISTINCT or MRHBM_RED_FSUM and combiner 0 or MRHBM_COMBINE_DISTINCT");
   c->bytevals = c->led.byte_values = (cfg->flags & MRHBM_F_BYTE_VALUES) != 0;
   c->red_distinct = cfg->reducer == MRHBM_RED_DISTINCT;
+  c->red_fsum = cfg->reducer == MRHBM_RED_FSUM;
   c->sb.no_reduce = cfg->reducer != MRHBM_RED_SUM;
   CU(c, cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
   if (cfg->partitioner == MRHBM_PART_RANGE && cfg->num_partitions == 1) {  // one key range, no splitters: its table now
@@ -714,7 +736,8 @@ void mrhbm_destroy(mrhbm_ctx* c) {
                    c->gtab,        c->l1buf,       c->regions,    c->d_l1all,     c->d_sample,   c->d_tok_text[0],
                    c->d_tok_text[1], c->d_tok_cnt, c->d_tok_off, c->d_spl,     c->arena,       c->voff,
                    c->cvals,       c->row_off,     c->val_tile,   c->val_pieces, c->dd_tab,     c->dd_out,
-                   c->dd_rg,       c->dd_slot,     c->dd_tiles,   c->vo_keys,    c->vo_ids};
+                   c->dd_rg,       c->dd_slot,     c->dd_tiles,   c->vo_keys,    c->vo_ids,
+                   c->ns_acc,      c->ns_flags,    c->ns_head};
   for (void* p : frees)
     if (p) cudaFree(p);
   if (c->h_counters) cudaFreeHost(c->h_counters);
@@ -1514,18 +1537,36 @@ int order_values(mrhbm_ctx* c, const ShuffleBuffers& v, uint64_t nb, uint32_t nb
   return 0;
 }
 
+// MRHBM_RED_FSUM, after the sort of the nb bins of view v and k_big_bins: an oversized bin's chunks merged into one run
+// by key (k_num_key_merge, many CTAs per bin), then every bin reduced to one row per key holding its values' exact sum, rounded
+// (mrhbm_num_sum.cu).  Inside ms_bigbins; a value that is not a number or a NaN sum is flagged in counters[CNT_ERR].
+int sum_values(mrhbm_ctx* c, const ShuffleBuffers& v, uint64_t nb, uint32_t nbig, mrhbm_stats& st) {
+  if (nbig) {  // (exact layout: rows [0, out_cap))
+    int rc = grow(c, &c->vo_cap, c->out_cap, c->out_cap, {{&c->vo_keys, (size_t)c->kb}, {(void**)&c->vo_ids, sizeof(uint64_t)}});
+    const uint64_t slots = num_slots(c->out_cap, c->cap);
+    if (!rc) rc = grow(c, &c->ns_cap, slots, slots, {{(void**)&c->ns_acc, 2 * kAccWords * sizeof(int64_t)},
+                                                     {(void**)&c->ns_flags, 4}, {(void**)&c->ns_head, 4}});
+    if (rc) return rc;
+    st.launches += launch_num_key_merge(c->rb, v, nbig, c->cap, c->out_cap, c->vo_keys, c->vo_ids, c->stream);
+  }
+  const NumScratch sc{c->ns_acc, c->ns_flags, c->ns_head};
+  st.launches += launch_num_sum(c->rb, v, (uint32_t)nb, nbig, c->cap, c->arena, c->voff, sc, c->stream);
+  CU(c, cudaGetLastError());
+  return 0;
+}
+
 // Exact layout, after the sort of the nb bins of view v (nbig of them oversized): k_big_bins, the group offsets, and
 // the bin offsets (v.bin_off), group offsets and counters read back.  EV_BIG, EV_END; synchronises the stream.
 int exact_tail(mrhbm_ctx* c, const ShuffleBuffers& v, uint64_t nb, uint32_t nbig, mrhbm_stats& st) {
   cudaStream_t s = c->stream;
   st.launches += launch_big_bins(c->rb, v, nbig, c->cap, s);
-  if (c->red_distinct) {
-    int rc = order_values(c, v, nb, nbig, st);
+  if (c->red_distinct || c->red_fsum) {
+    int rc = c->red_distinct ? order_values(c, v, nb, nbig, st) : sum_values(c, v, nb, nbig, st);
     if (rc) return rc;
   }
   CU(c, cudaEventRecord(c->ev[EV_BIG], s));
   c->h_big.clear();
-  if (c->sb.no_reduce && !c->red_distinct && nbig) {  // group-only mode: the iterator merges the runs of an oversized bin
+  if (c->sb.no_reduce && !c->red_distinct && !c->red_fsum && nbig) {  // group-only mode: the iterator merges the runs of an oversized bin
     c->h_big.resize(nbig);
     CU(c, cudaMemcpyAsync(c->h_big.data(), c->sb.big_list, nbig * 4, cudaMemcpyDeviceToHost, s));
   }
@@ -1709,6 +1750,7 @@ int shuffle_fast(mrhbm_ctx* c, std::vector<Src>& live, uint64_t N, uint64_t N_in
   if (Bl) st.launches += launch_sort_reduce(c->rb, v, (uint32_t)Bl, c->cap, c->sm_count, s);
   CU(c, cudaEventRecord(c->ev[EV_SORT], s));
   if (c->red_distinct && (rc = order_values(c, v, Bl, 0, st))) return rc;
+  if (c->red_fsum && (rc = sum_values(c, v, Bl, 0, st))) return rc;
   CU(c, cudaEventRecord(c->ev[EV_BIG], s));
   c->h_uoff.assign(Bl + 1, 0);
   if (Bl) {
@@ -2000,6 +2042,7 @@ int build_long_groups(mrhbm_ctx* c) {
   c->long_groups.clear();
   c->long_group_count = 0;
   c->long_vals.clear();
+  c->long_sums.clear();
   const int G = c->world;
   // this rank's committed long pairs as one blob: {u32 key bytes, u64 value, key bytes padded to 4}*
   // (byte values, one GPU only: the value travels as its index in long_vals)
@@ -2081,6 +2124,23 @@ int build_long_groups(mrhbm_ctx* c) {
   c->long_groups.resize(c->Pl);
   for (uint32_t sl = 0; sl < c->Pl; sl++)
     for (auto& kv : acc[sl]) {  // std::map iterates in ascending bytewise key order (unsigned char_traits compare)
+      if (c->red_fsum) {  // the key's values summed with the kernels' accumulator, into one encoded number
+        int64_t sum[kAccWords];
+        acc_clear(sum);
+        for (uint64_t i : kv.second) {
+          uint64_t bits;
+          const std::string& b = *c->long_vals[i];
+          if (!num_decode((const unsigned char*)b.data(), b.size(), &bits))
+            return fail(c, MRHBM_E_INVAL, "reducer MRHBM_RED_FSUM: a value of a long key is not a number");
+          acc_add(sum, bits);
+        }
+        uint64_t bits;
+        if (!acc_round(sum, &bits)) return fail(c, MRHBM_E_INVAL, "reducer MRHBM_RED_FSUM: a long key's sum is NaN (+inf and -inf)");
+        std::string& e = c->long_sums.emplace_back(kNumBytes, '\0');
+        num_encode(bits, (unsigned char*)&e[0]);
+        kv.second.assign(1, c->long_vals.size());
+        c->long_vals.push_back(&e);
+      }
       if (c->red_distinct) {  // the key's distinct values, ascending by their bytes (std::string compares unsigned)
         std::vector<uint64_t>& vals = kv.second;
         auto bytes = [c](uint64_t i) -> const std::string& { return *c->long_vals[i]; };
@@ -2092,6 +2152,21 @@ int build_long_groups(mrhbm_ctx* c) {
       c->long_group_count++;
     }
   return MRHBM_OK;
+}
+
+// After the device part of a shuffle: MRHBM_RED_FSUM's error flags (read back with the counters at its end), then the
+// long keys.  A shuffle that fails here leaves no result.
+int finish_shuffle(mrhbm_ctx* c) {
+  int rc = 0;
+  const uint32_t ef = c->red_fsum ? c->h_counters[CNT_ERR] : 0u;
+  if (ef & ERRF_NOTNUM)
+    rc = fail(c, MRHBM_E_INVAL, "reducer MRHBM_RED_FSUM: a value is not a number (11-byte encoding, tag 0x10)");
+  else if (ef & ERRF_NAN)
+    rc = fail(c, MRHBM_E_INVAL, "reducer MRHBM_RED_FSUM: a key's sum is NaN (+inf and -inf among its values)");
+  else
+    rc = build_long_groups(c);
+  if (rc) invalidate(c);
+  return rc;
 }
 }  // namespace
 
@@ -2105,6 +2180,8 @@ int mrhbm_shuffle(mrhbm_ctx* c) {
   uint64_t N_in = 0, N = 0;
   for (auto& r : c->led.live()) N_in += r.second;
   if (N_in >= 0xfffffff0ull) return fail(c, MRHBM_E_INVAL, "more than 2^32 pairs on one GPU (%llu)", (unsigned long long)N_in);
+  if (c->red_fsum && N_in >= (1ull << 31))  // (each accumulator digit takes fewer than 2^31 addends)
+    return fail(c, MRHBM_E_INVAL, "reducer MRHBM_RED_FSUM: a shuffle of %llu pairs (limit 2^31)", (unsigned long long)N_in);
   if (c->cfg.partitioner == MRHBM_PART_RANGE && c->world == 1 && !c->spl_set)  // (several GPUs: at the first all-gather)
     return fail(c, MRHBM_E_INVAL, "MRHBM_PART_RANGE needs splitters: call mrhbm_set_splitters or mrhbm_sample_splitters");
   mrhbm_stats st{};
@@ -2118,10 +2195,10 @@ int mrhbm_shuffle(mrhbm_ctx* c) {
     bool done = false;
     rc = shuffle_fast(c, live, N, N_in, st, &done);
     if (rc) return rc;
-    if (done) return build_long_groups(c);
+    if (done) return finish_shuffle(c);
   }
   rc = c->world > 1 ? shuffle_multi_exact(c, live, N, N_in, st) : shuffle_single_exact(c, live, N, N_in, st);
-  return rc ? rc : build_long_groups(c);
+  return rc ? rc : finish_shuffle(c);
 }
 
 int mrhbm_set_splitters(mrhbm_ctx* c, const void* keys, const uint64_t* off, size_t n) {

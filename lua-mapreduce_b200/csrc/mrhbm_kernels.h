@@ -93,7 +93,8 @@ MRHBM_HD inline uint32_t bin_count(const ShuffleBuffers& b, uint32_t bin) {
   return b.bin_off[bin + 1] - b.bin_off[bin];
 }
 enum { CNT_NBIG = 0, CNT_TICKET = 1, CNT_ERR = 2, CNT_TOTAL = 3, CNT_GBIG = 4 };
-enum { ERRF_SKEW = 1, ERRF_OVERFLOW = 2, ERRF_CAPACITY = 4, ERRF_KEYLEN = 8 };
+// ERRF_NOTNUM / ERRF_NAN (MRHBM_RED_FSUM): a value that is not a number encoding, a key whose sum is NaN
+enum { ERRF_SKEW = 1, ERRF_OVERFLOW = 2, ERRF_CAPACITY = 4, ERRF_KEYLEN = 8, ERRF_NOTNUM = 16, ERRF_NAN = 32 };
 
 // every launcher returns the number of kernels it launched
 int launch_gen_u64(void* dst, uint64_t seed, uint64_t start, uint64_t n, cudaStream_t s);
@@ -278,5 +279,35 @@ int launch_value_order(int rb, const ShuffleBuffers& b, uint32_t nb, uint32_t nb
 // then each oversized bin's chunks merged into one run; tmp_keys / tmp_ids: scratch rows laid out as out_keys / out_sums
 int launch_value_merge(int rb, const ShuffleBuffers& b, uint32_t nbig, uint32_t cap, const unsigned char* arena,
                        const uint64_t* voff, void* tmp_keys, uint64_t* tmp_ids, cudaStream_t s);
+
+// ---- MRHBM_RED_FSUM (mrhbm_num_sum.cu) ----
+// Oversized bins (exact layout, rows [0, N)): the partial accumulators of the groups that cross the edge of a cap-row
+// chunk.  The chunk that starts at row r is slot num_slot(r, ...): no two chunks of oversized bins share a slot (chunks
+// of one bin lie cap rows apart; a bin's first chunk and another bin's later chunk differ in parity), so 2 ceil(N / cap)
+// + 2 slots take every chunk.  Slot s: acc[2 s] (the chunk's leading part of a group), acc[2 s + 1] (its trailing
+// group), kAccWords each (mrhbm_numsum.cuh); flags[s]; head_row[s]: the trailing group's first row.
+struct NumScratch {
+  int64_t* acc;
+  uint32_t* flags;
+  uint32_t* head_row;
+};
+MRHBM_HD inline uint64_t num_slot(uint64_t first_row, uint32_t cap, bool first_chunk) {
+  return 2 * (first_row / cap) + (first_chunk ? 1 : 0);
+}
+inline uint64_t num_slots(uint64_t N, uint32_t cap) { return 2 * ((N + cap - 1) / cap) + 2; }
+// The cap-row chunks of each of the nbig oversized bins of big_list (ascending by key, as k_big_bins leaves them)
+// merged by key into one run, pass after pass of doubling width up to max_rows (at least every such bin's rows), each
+// pass spread over many CTAs per bin; tmp_keys / tmp_ids: scratch rows laid out as out_keys / out_sums.  The run ends in
+// the output rows.
+int launch_num_key_merge(int rb, const ShuffleBuffers& b, uint32_t nbig, uint32_t cap, uint64_t max_rows, void* tmp_keys,
+                         uint64_t* tmp_ids, cudaStream_t s);
+// Every bin's rows (ucount[bin] of them at out_start, sorted by key, value ids in out_sums; the nbig oversized bins of
+// big_list merged into one run each) become one row per key, out_sums its values' exact sum rounded to a double (bits),
+// ucount[bin] the keys.  ERRF_NOTNUM / ERRF_NAN in counters[CNT_ERR].
+int launch_num_sum(int rb, const ShuffleBuffers& b, uint32_t nb, uint32_t nbig, uint32_t cap, const unsigned char* arena,
+                   const uint64_t* voff, const NumScratch& sc, cudaStream_t s);
+// compacted rows whose ids hold double bits -> row r's encoded number at vals[11 r ..), row_off[r] = 11 r (n + 1
+// entries), ids[r] = r
+int launch_num_encode(uint64_t* ids, uint64_t n, unsigned char* vals, uint64_t* row_off, cudaStream_t s);
 
 }  // namespace mrhbm

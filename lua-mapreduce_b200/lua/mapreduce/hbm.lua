@@ -18,7 +18,9 @@ local hbm = { _VERSION = "0.1", _NAME = "mapreduce.hbm" }
 --     (quantiles of the map output, taken at the MAP -> REDUCE barrier).  The partitionfn must compute the same ranges.
 --   reducefn / combinerfn module: hbm_reducefn = "sum"; a combinerfn module of a value_kind = "bytes" job:
 --     hbm_combinerfn = "distinct" (its combinerfn emits the distinct values it is given); a reducefn module of a
---     value_kind = "bytes" job: hbm_reducefn = "distinct" (its reducefn emits the distinct values ascending by their
+--     value_kind = "bytes" job: hbm_reducefn = "fsum" (its reducefn emits the sum of its number values; the device
+--     sums them exactly, rounds once, and hbm.groups hands out that one number), or hbm_reducefn = "distinct" (its
+--     reducefn emits the distinct values ascending by their
 --     encoded bytes; the device computes them and hbm.groups hands them out as the reducefn's result)
 local ctx -- one context per worker process (job.lua keeps `funcs`/`initialized` per process too)
 local sample_splitters = false -- hbm_splitters = "sample": hbm.prepare_reduce samples them before the shuffle
@@ -43,12 +45,15 @@ function hbm.configure(partition_mod, reduce_mod, combiner_mod, opts)
   -- partitions, sorts and groups, job.lua:264-284 calls reducefn per group on the host.
   local builtin = reduce_mod.hbm_reducefn == "sum"
   local distinct_red = reduce_mod.hbm_reducefn == "distinct"
+  local fsum_red = reduce_mod.hbm_reducefn == "fsum"
   opts = opts or {}
   tuple_keys = opts.key_kind == "tuple" -- composite keys travel as encoded byte strings
   byte_values = opts.value_kind == "bytes" -- values travel as encoded byte strings (hbm.encode_value)
-  assert(not (byte_values and reduce_mod.hbm_reducefn ~= nil and not distinct_red),
-         "value_kind = 'bytes' hands string and number values to a general reducefn: the reducefn must not declare an hbm_reducefn other than 'distinct'")
+  assert(not (byte_values and reduce_mod.hbm_reducefn ~= nil and not distinct_red and not fsum_red),
+         "value_kind = 'bytes' hands string and number values to a general reducefn: the reducefn must not declare an hbm_reducefn other than 'distinct' or 'fsum'")
   assert(not distinct_red or byte_values, "hbm_reducefn = 'distinct' needs value_kind = 'bytes'")
+  assert(not fsum_red or byte_values, "hbm_reducefn = 'fsum' needs value_kind = 'bytes'")
+  assert(not fsum_red or combiner_mod == nil, "hbm_reducefn = 'fsum' takes no combinerfn")
   -- hbm_combinerfn = "distinct" (values = "bytes"): the combinerfn keeps one copy of each distinct value of a key, so
   -- the device drops the repeated (key, value) pairs of each map job at its commit
   local distinct = combiner_mod ~= nil and combiner_mod.hbm_combinerfn == "distinct"
@@ -61,7 +66,7 @@ function hbm.configure(partition_mod, reduce_mod, combiner_mod, opts)
     num_partitions = assert(partition_mod.NUM_REDUCERS, "partitionfn module must expose NUM_REDUCERS"),
     partitioner = assert(partition_mod.hbm_partitionfn, "partitionfn module must declare hbm_partitionfn"),
     combiner = distinct and "distinct" or combiner_mod ~= nil,
-    reducer = builtin and "sum" or (distinct_red and "distinct" or "none"),
+    reducer = builtin and "sum" or (distinct_red and "distinct" or (fsum_red and "fsum" or "none")),
     device = opts.device,
     values = byte_values and "bytes" or "int",
   }

@@ -37,10 +37,11 @@ static int fail(lua_State *L, mrhbm_ctx *c) { /* luamongo style: nil, msg */
 }
 
 /* mrhbm.new{ key_kind="str"|"u64", max_key_bytes=, num_partitions=, partitioner="fnv_lua"|"mulhash"|
- *            "wordhash"|"range", combiner=bool|"distinct", reducer="sum"|"none"|"distinct", device=,
+ *            "wordhash"|"range", combiner=bool|"distinct", reducer="sum"|"none"|"distinct"|"fsum", device=,
  *            values="int"|"bytes" }
- * values = "bytes" (MRHBM_F_BYTE_VALUES, needs reducer = "none" or "distinct"): m:emit takes string values and
- * ctx:groups yields tables of strings (reducer = "distinct": each key's distinct values, ascending) */
+ * values = "bytes" (MRHBM_F_BYTE_VALUES, needs reducer = "none", "distinct" or "fsum"): m:emit takes string
+ * values and ctx:groups yields tables of strings (reducer = "distinct": each key's distinct values, ascending;
+ * reducer = "fsum": one value, the exact sum of the key's numbers) */
 static int l_new(lua_State *L) {
   mrhbm_config cfg;
   const char *s;
@@ -64,9 +65,12 @@ static int l_new(lua_State *L) {
                : lua_toboolean(L, -1) ? MRHBM_COMBINE_REDUCER : MRHBM_COMBINE_NONE;
   lua_getfield(L, 1, "device");
   cfg.device = (int32_t)luaL_optinteger(L, -1, -1);
-  lua_getfield(L, 1, "reducer"); /* "sum" (built-in) | "none" (general reducefn on the host) | "distinct" */
+  lua_getfield(L, 1, "reducer"); /* "sum" (built-in) | "none" (general reducefn on the host) | "distinct" | "fsum" */
   s = luaL_optstring(L, -1, "sum");
-  cfg.reducer = strcmp(s, "none") == 0 ? MRHBM_RED_NONE : strcmp(s, "distinct") == 0 ? MRHBM_RED_DISTINCT : MRHBM_RED_SUM;
+  cfg.reducer = strcmp(s, "none") == 0       ? MRHBM_RED_NONE
+                : strcmp(s, "distinct") == 0 ? MRHBM_RED_DISTINCT
+                : strcmp(s, "fsum") == 0     ? MRHBM_RED_FSUM
+                                             : MRHBM_RED_SUM;
   lua_getfield(L, 1, "values");
   s = luaL_optstring(L, -1, "int");
   if (strcmp(s, "bytes") == 0) cfg.flags |= MRHBM_F_BYTE_VALUES;

@@ -5,6 +5,7 @@ keys_sorted / combiner / partitionfn / text spill are what mrhbm_shuffle does on
 Reduce job (job.lua:230-296): the (key, values) stream of utils.merge_iterator becomes
 mrhbm_groups_next; the reducer algebra (job.lua:264-284) is kept."""
 import importlib
+import math
 import time
 
 from . import tuple as tuple_keys
@@ -125,6 +126,52 @@ class Job:
                 ks = [x.replace(b"\x01\x01", b"\x00").replace(b"\x01\x02", b"\x01") if b"\x01" in x else x for x in ks]
         return [(kk, [vv]) for kk, vv in zip(ks, v.tolist())]
 
+    def _bulk_fsum(self, part):
+        """hbm_reducefn = "fsum": [(key, [sum])] of one partition in ascending key order from one bulk copy of the
+        shuffle's keys and values (mrhbm_result_copy + mrhbm_result_values, cached on the board per shuffle), the
+        device's single value per key handed out as the reducefn's result.  None when the ctx offers no bulk access
+        (keys longer than a result slot, test stand-ins): the iterator gives the same values."""
+        import numpy as np
+        b, ctx = self.board, self.board.ctx
+        if not hasattr(ctx, "result_values"):
+            return None
+        cache = getattr(b, "_bulk_fsum", None)
+        if cache is None or cache[0] is not ctx or cache[1] != b.iteration:
+            try:
+                keys, _, po = ctx.result_copy()
+                blob, _ = ctx.result_values()
+            except Exception as e:
+                if getattr(e, "code", None) != -4:  # MRHBM_E_KEY
+                    raise
+                b._bulk_fsum = (ctx, b.iteration, None, None, None, False)
+                return None
+            cache = b._bulk_fsum = (ctx, b.iteration, keys, blob, po, bool(ctx.result_info().sorted))
+        _, _, keys, blob, po, is_sorted = cache
+        if keys is None:
+            return None
+        a, e = int(po[part]), int(po[part + 1])
+        k = keys[a:e]
+        # every row's value is the 11-byte number at 11 r: the sign-folded double in ten 7-bit groups
+        g = blob[11 * a:11 * e].reshape(-1, 11)[:, 1:].astype(np.uint64) & np.uint64(0x7F)
+        u = np.zeros(e - a, dtype=np.uint64)
+        for j in range(10):
+            u = (u << np.uint64(7)) | g[:, j]
+        top = (u >> np.uint64(63)).astype(bool)
+        bits = np.where(top, u & np.uint64(0x7FFFFFFFFFFFFFFF), ~u)
+        v = bits.view(np.float64)
+        if not is_sorted:  # several ascending runs (hash sub-bins): merge = stable sort by key
+            order = np.argsort(k, kind="stable")
+            k, v = k[order], v[order]
+        if k.dtype.kind == "u":
+            ks = [int(x).to_bytes(8, "big") for x in k.tolist()]
+        else:
+            ks = k.tolist()
+            if any(b"\x01" in x for x in ks):  # escaped 0x00 / 0x01 bytes (mrhbm_emit_str)
+                ks = [x.replace(b"\x01\x01", b"\x00").replace(b"\x01\x02", b"\x01") if b"\x01" in x else x for x in ks]
+        # as tuple.decode_value gives them: integral numbers as ints, -0 as -0.0
+        return [(kk, [int(f) if f.is_integer() and abs(f) <= (1 << 53) and not (f == 0 and math.copysign(1, f) < 0)
+                      else f]) for kk, f in zip(ks, v.tolist())]
+
     # ---- job.lua:230-296
     def _reduce(self):
         cfg, ctx = self.cfg, self.board.ctx
@@ -140,6 +187,14 @@ class Job:
         decode = tuple_keys.decode if cfg["hbm"]["key_kind"] == "tuple" else None
         byte_values = cfg["hbm"].get("value_kind") == "bytes"
         device_distinct = cfg["hbm"].get("reducer") == 2  # hbm_reducefn = "distinct": the values are its output
+        if cfg["hbm"].get("reducer") == 3 and decode is None:  # hbm_reducefn = "fsum": one number per key, in bulk
+            fsum = self._bulk_fsum(part)
+            if fsum is not None:
+                self.doc["value"]["pairs"] = fsum
+                self.written = True
+                self.board.mark(self.doc, STATUS.WRITTEN, written_time=time.time(), real_time=time.time() - self.t)
+                return
+        device_distinct |= cfg["hbm"].get("reducer") == 3  # (tuple keys, long keys: the iterator's one value per key)
         bulk = self._bulk_groups(part) if (aci and cfg["hbm"].get("reducer", 0) == 0 and decode is None) else None
         if bulk is not None:
             # built-in reducer + ACI flags: every value list is the singleton the device produced and the reference

@@ -3,6 +3,7 @@ server_prepare_map (249-276), server_prepare_reduce (279-329), server_final (348
 The MongoDB task/job collections are an in-process board; GridFS spill files are the HBM
 shuffle (storage "hbm").  Jobs run on attached workers or, when none is attached, inline."""
 import bisect
+import math
 import importlib
 import sys
 import time
@@ -66,6 +67,32 @@ def distinct_combiner(comb, value_kind):
                              "distinct values: the declaration must describe what the combinerfn computes" % (values, out))
 
 
+# Number sums whose every summation order is exact (dyadic fractions, negatives, -0, cancellation across 2^60, in
+# Python integers): any reducefn that adds its values one by one, in whatever order, gives the exact sum on them.  The
+# sign of a zero sum is not checked: "count = 0; count = count + v" gives +0 where the device gives -0 for all -0.
+_FSUM_PROBES = ([1, 2, 3], [0.5, 0.25, -1.75, 3], [2 ** 60, 1, -2 ** 60], [-0.0, -0.0], [0.0, -0.0],
+                [-3.5], [1.5, -1.5, 0.125], [-2, -0.5, -0.75], [7])
+
+
+def fsum_reducer(red, value_kind):
+    """Checks a reducefn module that declares hbm_reducefn = "fsum": the device then hands every key the exact sum of
+    its number values, rounded once, and the reducefn is not called, so it must emit exactly that one number."""
+    from fractions import Fraction
+    if value_kind != "bytes":
+        raise ValueError("hbm_reducefn = 'fsum' sums number values carried as bytes: configure hbm = {'value_kind': 'bytes'}")
+    for values in _FSUM_PROBES:
+        out = []
+        try:
+            red.reducefn(b"probe", list(values), out.append)
+        except Exception as e:
+            raise ValueError("hbm_reducefn = 'fsum': reducefn failed on the values %r: %r" % (values, e))
+        want = float(sum(Fraction(v) for v in values))
+        ok = len(out) == 1 and isinstance(out[0], (int, float)) and not isinstance(out[0], bool) and out[0] == want
+        if not ok:
+            raise ValueError("hbm_reducefn = 'fsum', but reducefn turns the values %r into %r instead of their sum %r: "
+                             "the declaration must describe what the reducefn computes" % (values, out, want))
+
+
 def distinct_reducer(red, value_kind):
     """Checks a reducefn module that declares hbm_reducefn = "distinct": the device then hands every key its distinct
     values, ascending by their encoded bytes, and the reducefn is not called, so it must emit exactly that sequence."""
@@ -125,8 +152,8 @@ class server:
         # associative/commutative/idempotent flags, examples/WordCount/reducefn.lua:10-14)
         red, part = mods["reducefn"], mods["partitionfn"]
         builtin_red = getattr(red, "hbm_reducefn", None)
-        if builtin_red not in (None, "sum", "distinct"):
-            raise NotImplementedError("unknown hbm_reducefn %r (built-ins: 'sum', 'distinct')" % (builtin_red,))
+        if builtin_red not in (None, "sum", "distinct", "fsum"):
+            raise NotImplementedError("unknown hbm_reducefn %r (built-ins: 'sum', 'distinct', 'fsum')" % (builtin_red,))
         # no declaration = general reducer: the device partitions, sorts and groups, reducefn runs
         # on the host per group (job.lua:264-284); values are unsigned integers < 2^32
         # A combinerfn only ever runs on the device, as the declared built-in (it must equal the reducefn there).
@@ -153,12 +180,17 @@ class server:
         # value_kind = "bytes": values are Lua strings and numbers (tuple.encode_value), handed to a general reducefn
         if hbm["value_kind"] not in ("int", "bytes"):
             raise ValueError("hbm value_kind must be 'int' or 'bytes', got %r" % (hbm["value_kind"],))
-        if hbm["value_kind"] == "bytes" and builtin_red not in (None, "distinct"):
+        if hbm["value_kind"] == "bytes" and builtin_red not in (None, "distinct", "fsum"):
             raise ValueError("hbm value_kind = 'bytes' hands string and number values to a general reducefn: "
-                             "the reducefn module must not declare an hbm_reducefn other than 'distinct' (it declares "
-                             "%r)" % (builtin_red,))
+                             "the reducefn module must not declare an hbm_reducefn other than 'distinct' or 'fsum' (it "
+                             "declares %r)" % (builtin_red,))
         if builtin_red == "distinct":  # every key's distinct values, ascending, on the device: reducefn is not called
             distinct_reducer(red, hbm["value_kind"])
+        if builtin_red == "fsum":  # every key's numbers summed exactly on the device: reducefn is not called
+            fsum_reducer(red, hbm["value_kind"])
+            if distinct:  # a device combiner would drop repeated values before they are summed
+                raise ValueError("hbm_reducefn = 'fsum' takes no device combiner: the combinerfn module declares "
+                                 "hbm_combinerfn = %r" % (mods["combinerfn"].hbm_combinerfn,))
         if getattr(mods["mapfn"], "hbm_mapfn", None) == "words_file" and hbm["value_kind"] != "bytes":
             raise ValueError("hbm_mapfn = 'words_file' pairs every word with the file name, a string value: "
                              "configure hbm = {'value_kind': 'bytes'}")
@@ -166,7 +198,7 @@ class server:
             distinct_combiner(mods["combinerfn"], hbm["value_kind"])
         hbm.update(partitioner=_BUILTIN_PART[pname], num_partitions=nparts,
                    combiner="distinct" if distinct else device_combiner,
-                   reducer={"sum": 0, "distinct": 2}.get(builtin_red, 1),
+                   reducer={"sum": 0, "distinct": 2, "fsum": 3}.get(builtin_red, 1),
                    splitters=range_splitters(part, nparts, hbm["key_kind"]) if pname == "range" else None)
         self.config = dict(mapfn=params["mapfn"], reducefn=params["reducefn"], partitionfn=params["partitionfn"],
                            combinerfn=params.get("combinerfn"), init_args=self.init_args,
