@@ -132,7 +132,36 @@ enum {
    * surviving pairs.  The room of the dropped pairs and of their value bytes is not reused before mrhbm_reset.  Device
    * memory: a hash set of 16 bytes x (a power of two >= 2 x the job's pairs), kept across commits, plus 4 + record
    * bytes per pair of the job. */
-  MRHBM_COMBINE_DISTINCT = 2
+  MRHBM_COMBINE_DISTINCT = 2,
+  /* MRHBM_F_BYTE_VALUES and reducer MRHBM_RED_FSUM only (any other combination fails mrhbm_init with MRHBM_E_INVAL;
+   * one GPU, as byte values are): the combinerfn "count = count + v" of a number-sum job, run on the device at
+   * mrhbm_map_commit without rounding anything away.  Keys compare by their stored slot bytes (long keys, see
+   * mrhbm_emit_str, by their bytes, on the host).  For each key of the handle's pairs, with m its values in this job
+   * and S their exact sum:
+   *   - a value that is not a number encoding (see MRHBM_RED_FSUM; a NaN encoding included), or +inf and -inf among
+   *     the key's values, fails the commit with MRHBM_E_INVAL; the job stays uncommitted (the handle is consumed, an
+   *     earlier commit under the same id stays), as a Lua combinerfn's count + v would break the map job;
+   *   - infinities of one sign: one value, that infinity;
+   *   - S = 0: one value, -0 if all m values are -0, else +0;
+   *   - otherwise the greedy expansion: c1 = S rounded to the nearest double, ties to even (what MRHBM_RED_FSUM gives
+   *     for these values alone), c(k+1) = S - c1 - ... - ck rounded the same way, until the remainder is 0 (one or
+   *     two values in practice; two values never need more than two);
+   *   - but if |S| >= 2^1024 - 2^970 (c1 would be +-inf) or the expansion has more than m terms, the key keeps its m
+   *     values as emitted.
+   * The surviving pairs are new pairs at the tail of the pool, ordered by the pool position of each key's first pair,
+   * a key's values in the order c1, c2, ... (kept values in emission order).  Every survivor holds its own 11-byte
+   * value and its value id is its own pool index, also in a job of mrhbm_map_words_value pieces.  mrhbm_pool_read,
+   * mrhbm_checksum_input, mrhbm_result_info.pairs_in and everything after the commit see only the survivors.  The
+   * job's original room is not reused before mrhbm_reset; survivors count against the 2^32 pairs between resets.
+   * Replace-by-job-id, abort, reset and repeated shuffles are unchanged.  After mrhbm_shuffle every result is
+   * bit-identical to the same commits without the combiner: mrhbm_groups_next_values, the rows of mrhbm_result_copy
+   * with mrhbm_result_values (their order follows info.sorted, which the shuffle picks from the pairs
+   * it carries), the groups count, and the shuffle's failures (+inf in one job and -inf in another still fail
+   * it); pairs_in and pairs_recv count the survivors the shuffle carried.  The combine is not part of mrhbm_stats.  Limits: fewer than 2^31 pairs per map job (else
+   * MRHBM_E_INVAL).  Device memory: the distinct combiner's hash set and per-pair scratch, plus 16 bytes x the set's
+   * entries, 16 bytes per pair of the job, and 548 bytes per 4096 pairs; a commit where some key keeps its values
+   * also copies the job's entries to the host and back. */
+  MRHBM_COMBINE_FSUM = 3
 };
 
 typedef struct mrhbm_ctx mrhbm_ctx;

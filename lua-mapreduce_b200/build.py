@@ -7,7 +7,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "lib", "libmrhbm.so")
-SOURCES = ["mrhbm_kernels.cu", "mrhbm_values.cu", "mrhbm_distinct.cu", "mrhbm_value_order.cu", "mrhbm_num_sum.cu", "mrhbm_api.cu", "mrhbm_comm.cu"]
+SOURCES = ["mrhbm_kernels.cu", "mrhbm_values.cu", "mrhbm_distinct.cu", "mrhbm_value_order.cu", "mrhbm_num_sum.cu", "mrhbm_num_combine.cu", "mrhbm_api.cu", "mrhbm_comm.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
 

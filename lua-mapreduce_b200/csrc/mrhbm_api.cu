@@ -129,6 +129,12 @@ struct mrhbm_ctx {
   void *dd_tab = nullptr, *dd_out = nullptr, *dd_rg = nullptr;
   uint32_t *dd_slot = nullptr, *dd_tiles = nullptr;
   uint64_t dd_tab_cap = 0, dd_rec_cap = 0, dd_rg_cap = 0, dd_tiles_cap = 0;  // entries, records, ranges, tiles
+  // MRHBM_COMBINE_FSUM at commit: the distinct combiner's hash set, entry of every record, ranges and tiles (dd_*), and
+  // FsumScratch's per-entry words, values, big keys and their accumulators, and flag words
+  uint32_t *fs_words = nullptr, *fs_big = nullptr, *fs_small = nullptr;
+  uint64_t* fs_vals = nullptr;
+  int64_t* fs_gacc = nullptr;
+  uint64_t fs_words_cap = 0, fs_vals_cap = 0, fs_big_cap = 0;
   // MRHBM_RED_DISTINCT: the shuffle runs the same set over all committed pairs, and orders every bin's rows by value
   // bytes; the merge of an oversized bin's chunks alternates with these scratch rows (out_cap of them)
   bool red_distinct = false;
@@ -265,6 +271,11 @@ struct Reservation {
   }
   void add(const mrhbm_map* m) {
     led->add(m->serial, m->job, off, n, aoff);
+    led = nullptr;
+  }
+  // MRHBM_COMBINE_FSUM: the room replaces all of the map's open ranges
+  void replace(const mrhbm_map* m) {
+    led->replace_open(m->serial, m->job, off, n, aoff);
     led = nullptr;
   }
 };
@@ -620,6 +631,139 @@ int distinct_pairs(mrhbm_map* m, std::vector<std::pair<uint64_t, uint64_t>>& kep
   return 0;
 }
 
+// MRHBM_COMBINE_FSUM, for keys longer than a record slot: the pairs of each key (by their bytes, in the order of its
+// first pair) replaced by acc_split's terms, or kept as emitted
+int fsum_long_pairs(mrhbm_ctx* c, std::vector<LongPair>& pairs) {
+  std::map<std::string, std::vector<size_t>> by_key;
+  std::vector<const std::string*> order;
+  for (size_t i = 0; i < pairs.size(); i++) {
+    auto it = by_key.emplace(pairs[i].esc, std::vector<size_t>()).first;
+    if (it->second.empty()) order.push_back(&it->first);
+    it->second.push_back(i);
+  }
+  std::vector<LongPair> out;
+  for (const std::string* k : order) {
+    const std::vector<size_t>& idx = by_key[*k];
+    int64_t acc[kAccWords];
+    acc_clear(acc);
+    for (size_t i : idx) {
+      uint64_t bits;
+      const std::string& b = pairs[i].bytes;
+      if (!num_decode((const unsigned char*)b.data(), b.size(), &bits))
+        return fail(c, MRHBM_E_INVAL, "combiner MRHBM_COMBINE_FSUM: a value of a long key is not a number");
+      acc_add(acc, bits);
+    }
+    std::vector<uint64_t> terms(idx.size());
+    const int n = acc_split(acc, terms.data(), (int)idx.size());
+    if (n < 0) return fail(c, MRHBM_E_INVAL, "combiner MRHBM_COMBINE_FSUM: a long key has +inf and -inf among its values");
+    if (n == 0) {
+      for (size_t i : idx) out.push_back(pairs[i]);
+      continue;
+    }
+    for (int t = 0; t < n; t++) {
+      std::string enc(kNumBytes, '\0');
+      num_encode(terms[t], (unsigned char*)&enc[0]);
+      out.push_back(LongPair{*k, 0, std::move(enc)});
+    }
+  }
+  pairs.swap(out);
+  return 0;
+}
+
+// MRHBM_COMBINE_FSUM, at commit: the map's pairs replaced by each key's terms (launch_fsum_split), as new pairs at the
+// tail of the pool in the order of their keys' first pairs, each with its own value; the keys that keep their values
+// are then placed in pool order by the host (only when some key does).  The map's open ranges are replaced by the new
+// room once everything has succeeded; a failure rewinds the room.  One host synchronisation, plus the pool's growth
+// and the kept keys' placement when they happen.
+int fsum_pairs(mrhbm_map* m) {
+  mrhbm_ctx* c = m->ctx;
+  cudaStream_t s = c->stream;
+  const std::vector<std::pair<uint64_t, uint64_t>> ranges = c->led.open_ranges(m->serial);
+  std::vector<DistinctRange> rg;
+  uint64_t n = 0, nt = 0;
+  for (const auto& r : ranges) {
+    rg.push_back(DistinctRange{r.first, n, (uint32_t)nt, 0});
+    n += r.second;
+    nt += (r.second + kDistinctTile - 1) / kDistinctTile;
+  }
+  rg.push_back(DistinctRange{0, n, (uint32_t)nt, 0});
+  const uint32_t nr = (uint32_t)rg.size() - 1;
+  if (n >= (1ull << 31))  // (each accumulator digit takes fewer than 2^31 addends; counts are u32)
+    return fail(c, MRHBM_E_INVAL, "combiner MRHBM_COMBINE_FSUM: a map job of %llu pairs (limit 2^31)", (unsigned long long)n);
+  std::vector<LongPair> longs = m->long_pairs;
+  int rc = fsum_long_pairs(c, longs);
+  if (rc) return rc;
+  if (n) {
+    uint64_t T = 1024;
+    while (T < 2 * n) T <<= 1;
+    const uint64_t nbig = n / kFsumWarpValues + 1;
+    rc = grow(c, &c->dd_tab_cap, T, std::max(T, 2 * c->dd_tab_cap), {{&c->dd_tab, 16}});
+    if (!rc) rc = grow(c, &c->dd_rec_cap, n, n, {{(void**)&c->dd_slot, 4}, {&c->dd_out, (size_t)c->rb}});
+    if (!rc) rc = grow(c, &c->dd_rg_cap, nr + 1, nr + 1, {{&c->dd_rg, sizeof(DistinctRange)}});
+    if (!rc) rc = grow(c, &c->dd_tiles_cap, 2 * (nt + 1), 2 * (nt + 1), {{(void**)&c->dd_tiles, 4}});
+    if (!rc) rc = grow(c, &c->fs_words_cap, 4 * T, 4 * T, {{(void**)&c->fs_words, 4}});
+    if (!rc) rc = grow(c, &c->fs_vals_cap, 2 * n, 2 * n, {{(void**)&c->fs_vals, 8}});
+    if (!rc) rc = grow(c, &c->fs_big_cap, nbig, nbig, {{(void**)&c->fs_big, 4}, {(void**)&c->fs_gacc, kAccWords * 8}});
+    if (!rc && !c->fs_small) CU(c, cudaMalloc((void**)&c->fs_small, 4 * sizeof(uint32_t)));
+    if (rc) return rc;
+    FsumScratch fs{c->dd_tab, T - 1, c->dd_slot, c->fs_words, c->fs_big, c->fs_small, c->fs_vals, c->fs_vals + n, c->fs_gacc};
+    uint32_t *tile_cnt = c->dd_tiles, *tile_off = c->dd_tiles + nt + 1;
+    const DistinctRange* drg = (const DistinctRange*)c->dd_rg;
+    CU(c, cudaMemsetAsync(c->dd_tab, 0xff, T * 16, s));
+    CU(c, cudaMemsetAsync(c->fs_words, 0, T * 4, s));
+    CU(c, cudaMemsetAsync(c->fs_small, 0, 4 * sizeof(uint32_t), s));
+    CU(c, cudaMemsetAsync(c->fs_gacc, 0, nbig * kAccWords * 8, s));
+    CU(c, cudaMemcpyAsync(c->dd_rg, rg.data(), rg.size() * sizeof(DistinctRange), cudaMemcpyHostToDevice, s));
+    launch_fsum_split(c->rb, c->pool, drg, nr, (uint32_t)nt, n, c->arena, c->voff, fs, tile_cnt, c->sm_count, s);
+    launch_exscan(tile_cnt, (uint32_t)nt, tile_off, nullptr, nullptr, 0xffffffffu, nullptr, nullptr, nullptr, 0, s,
+                  c->d_small + 64);
+    CU(c, cudaGetLastError());
+    CU(c, cudaMemcpyAsync(c->h_counters, c->fs_small, 4, cudaMemcpyDeviceToHost, s));
+    CU(c, cudaMemcpyAsync(c->h_counters + 1, tile_off + nt, 4, cudaMemcpyDeviceToHost, s));
+    CU(c, cudaStreamSynchronize(s));
+    const uint32_t flags = c->h_counters[0];
+    const uint64_t total = c->h_counters[1];
+    if (flags & ERRF_NOTNUM)
+      return fail(c, MRHBM_E_INVAL, "combiner MRHBM_COMBINE_FSUM: a value is not a number (11-byte encoding, tag 0x10)");
+    if (flags & ERRF_NAN)
+      return fail(c, MRHBM_E_INVAL, "combiner MRHBM_COMBINE_FSUM: a key has +inf and -inf among its values");
+    Reservation r;
+    rc = reserve(c, nullptr, total, kNumBytes * total, r);
+    if (rc) return rc;
+    launch_fsum_write(c->rb, c->pool, drg, nr, (uint32_t)nt, fs, tile_off, r.off, r.aoff, c->voff, c->arena, s);
+    CU(c, cudaGetLastError());
+    if (flags & kFsumKeep) {
+      // the kept keys' pairs in pool order, each after the key's first new pair (the cursor words of its entry)
+      std::vector<uint32_t> slot_of(n), nterm(T), first(T);
+      CU(c, cudaMemcpyAsync(slot_of.data(), c->dd_slot, n * 4, cudaMemcpyDeviceToHost, s));
+      CU(c, cudaMemcpyAsync(nterm.data(), c->fs_words + 3 * T, T * 4, cudaMemcpyDeviceToHost, s));
+      CU(c, cudaMemcpyAsync(first.data(), c->fs_words + 2 * T, T * 4, cudaMemcpyDeviceToHost, s));
+      CU(c, cudaStreamSynchronize(s));
+      std::vector<uint64_t> cp;
+      for (size_t k = 0; k < ranges.size(); k++)
+        for (uint64_t j = 0; j < ranges[k].second; j++) {
+          const uint64_t g = rg[k].vbase + j;
+          const uint32_t e = slot_of[g];
+          if (!(nterm[e] & kFsumKeep)) continue;
+          cp.insert(cp.end(), {(uint64_t)first[e]++, ranges[k].first + j, g});
+        }
+      uint64_t* d_cp = nullptr;
+      CU(c, cudaMalloc((void**)&d_cp, cp.size() * 8));
+      cudaError_t e = cudaMemcpyAsync(d_cp, cp.data(), cp.size() * 8, cudaMemcpyHostToDevice, s);
+      if (e == cudaSuccess) {
+        launch_fsum_copy(c->rb, c->pool, d_cp, cp.size() / 3, fs, r.off, r.aoff, c->voff, c->arena, s);
+        e = cudaGetLastError();
+      }
+      if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+      cudaFree(d_cp);
+      if (e != cudaSuccess) return fail(c, MRHBM_E_CUDA, "combiner MRHBM_COMBINE_FSUM: %s", cudaGetErrorString(e));
+    }
+    r.replace(m);
+  }
+  m->long_pairs.swap(longs);
+  return 0;
+}
+
 float ev_ms(mrhbm_ctx* c, int a, int b) {
   float ms = 0;
   if (cudaEventElapsedTime(&ms, c->ev[a], c->ev[b]) != cudaSuccess) {
@@ -678,14 +822,17 @@ int mrhbm_init(const mrhbm_config* cfg, mrhbm_ctx** out) {
   } else
     return fail(c, MRHBM_E_INVAL, "unknown key_kind %u", cfg->key_kind);
   if (cfg->reducer > MRHBM_RED_FSUM) return fail(c, MRHBM_E_INVAL, "unknown reducer %u", cfg->reducer);
-  if (cfg->combiner > MRHBM_COMBINE_DISTINCT) return fail(c, MRHBM_E_INVAL, "unknown combiner %u", cfg->combiner);
+  if (cfg->combiner > MRHBM_COMBINE_FSUM) return fail(c, MRHBM_E_INVAL, "unknown combiner %u", cfg->combiner);
+  if (cfg->combiner == MRHBM_COMBINE_FSUM && (!(cfg->flags & MRHBM_F_BYTE_VALUES) || cfg->reducer != MRHBM_RED_FSUM))
+    return fail(c, MRHBM_E_INVAL, "combiner MRHBM_COMBINE_FSUM needs byte values (MRHBM_F_BYTE_VALUES) and reducer MRHBM_RED_FSUM");
   if (cfg->combiner == MRHBM_COMBINE_DISTINCT && !(cfg->flags & MRHBM_F_BYTE_VALUES))
     return fail(c, MRHBM_E_INVAL, "combiner MRHBM_COMBINE_DISTINCT needs byte values (MRHBM_F_BYTE_VALUES)");
   if (cfg->reducer == MRHBM_RED_NONE && cfg->combiner == MRHBM_COMBINE_REDUCER) return fail(c, MRHBM_E_INVAL, "a general reducer cannot be combined on the device (combiner must be 0)");
   if (cfg->reducer == MRHBM_RED_DISTINCT && !(cfg->flags & MRHBM_F_BYTE_VALUES))
     return fail(c, MRHBM_E_INVAL, "reducer MRHBM_RED_DISTINCT needs byte values (MRHBM_F_BYTE_VALUES)");
-  if (cfg->reducer == MRHBM_RED_FSUM && (!(cfg->flags & MRHBM_F_BYTE_VALUES) || cfg->combiner != MRHBM_COMBINE_NONE))
-    return fail(c, MRHBM_E_INVAL, "reducer MRHBM_RED_FSUM needs byte values (MRHBM_F_BYTE_VALUES) and combiner MRHBM_COMBINE_NONE");
+  if (cfg->reducer == MRHBM_RED_FSUM && (!(cfg->flags & MRHBM_F_BYTE_VALUES) ||
+                                         (cfg->combiner != MRHBM_COMBINE_NONE && cfg->combiner != MRHBM_COMBINE_FSUM)))
+    return fail(c, MRHBM_E_INVAL, "reducer MRHBM_RED_FSUM needs byte values (MRHBM_F_BYTE_VALUES) and combiner MRHBM_COMBINE_NONE or MRHBM_COMBINE_FSUM");
   if ((cfg->flags & MRHBM_F_BYTE_VALUES) && (cfg->reducer == MRHBM_RED_SUM || cfg->combiner == MRHBM_COMBINE_REDUCER))
     return fail(c, MRHBM_E_INVAL, "byte values (MRHBM_F_BYTE_VALUES) need reducer MRHBM_RED_NONE, MRHBM_RED_DISTINCT or MRHBM_RED_FSUM and combiner 0 or MRHBM_COMBINE_DISTINCT");
   c->bytevals = c->led.byte_values = (cfg->flags & MRHBM_F_BYTE_VALUES) != 0;
@@ -737,7 +884,8 @@ void mrhbm_destroy(mrhbm_ctx* c) {
                    c->d_tok_text[1], c->d_tok_cnt, c->d_tok_off, c->d_spl,     c->arena,       c->voff,
                    c->cvals,       c->row_off,     c->val_tile,   c->val_pieces, c->dd_tab,     c->dd_out,
                    c->dd_rg,       c->dd_slot,     c->dd_tiles,   c->vo_keys,    c->vo_ids,
-                   c->ns_acc,      c->ns_flags,    c->ns_head};
+                   c->ns_acc,      c->ns_flags,    c->ns_head,    c->fs_words,   c->fs_big,     c->fs_small,
+                   c->fs_vals,     c->fs_gacc};
   for (void* p : frees)
     if (p) cudaFree(p);
   if (c->h_counters) cudaFreeHost(c->h_counters);
@@ -1196,6 +1344,7 @@ int mrhbm_map_commit(mrhbm_map* m) {
   }
   std::vector<std::pair<uint64_t, uint64_t>> kept;
   if (rc == 0 && c->cfg.combiner == MRHBM_COMBINE_DISTINCT) rc = distinct_pairs(m, kept);
+  if (rc == 0 && c->cfg.combiner == MRHBM_COMBINE_FSUM) rc = fsum_pairs(m);
   if (rc) {
     mrhbm_map_abort(m);
     return rc;

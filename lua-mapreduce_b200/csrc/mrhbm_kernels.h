@@ -310,4 +310,36 @@ int launch_num_sum(int rb, const ShuffleBuffers& b, uint32_t nb, uint32_t nbig, 
 // entries), ids[r] = r
 int launch_num_encode(uint64_t* ids, uint64_t n, unsigned char* vals, uint64_t* row_off, cudaStream_t s);
 
+// ---- MRHBM_COMBINE_FSUM (mrhbm_num_combine.cu) ----
+// One map job's records (DistinctRange, as the distinct combiner takes them) grouped by key slot and each key's numbers
+// split into the greedy expansion of their exact sum (acc_split, mrhbm_numsum.cuh).  Scratch, all sized by the caller:
+//   tab      mask + 1 16-byte entries {fingerprint, smallest pool index of the key}, memset to 0xff
+//   slot_of  the entry of each of the job's n records; vbits: their values' double bits
+//   words    4 (mask + 1) words: the entries' counts (zeroed), rooms in vals, cursors, terms (see kFsumKeep)
+//   vals     n: each key's values, then its terms, in a room of its own
+//   big      n / kFsumWarpValues + 1 keys longer than a warp takes; gacc: an accumulator for each (zeroed)
+//   small    4 zeroed words: flags (ERRF_NOTNUM, ERRF_NAN, kFsumKeep), the rooms' bump, the number of big keys
+constexpr uint32_t kFsumWarpValues = 4096;
+constexpr uint32_t kFsumKeep = 1u << 31;  // in a key's term count and in the flags: the key keeps its values
+struct FsumScratch {
+  void* tab;
+  uint64_t mask;
+  uint32_t *slot_of, *words, *big, *small;
+  uint64_t *vbits, *vals;
+  int64_t* gacc;
+};
+// The sums and terms of every key, and tile_cnt[t] = the new pairs of the keys whose first pair lies in tile t
+int launch_fsum_split(int rb, const void* pool, const DistinctRange* rg, uint32_t nr, uint32_t ntiles, uint64_t n,
+                      const unsigned char* arena, const uint64_t* voff, const FsumScratch& fs, uint32_t* tile_cnt,
+                      int sm_count, cudaStream_t s);
+// The new pairs (tile_off: the exclusive scan of tile_cnt) at pool records first + i with value id first + i, voff
+// entries from aoff on (11 bytes each, voff[first + total] included) and their encoded values in the arena.  A key
+// that keeps its values is left to launch_fsum_copy: the words' cursor of its entry receives its first new pair.
+int launch_fsum_write(int rb, void* pool, const DistinctRange* rg, uint32_t nr, uint32_t ntiles, const FsumScratch& fs,
+                      const uint32_t* tile_off, uint64_t first, uint64_t aoff, uint64_t* voff, unsigned char* arena,
+                      cudaStream_t s);
+// The kept values: cp[3 i .. 3 i + 2] = {new pair's index after first, its record's pool index, its job index}
+int launch_fsum_copy(int rb, void* pool, const uint64_t* cp, uint64_t m, const FsumScratch& fs, uint64_t first,
+                     uint64_t aoff, uint64_t* voff, unsigned char* arena, cudaStream_t s);
+
 }  // namespace mrhbm

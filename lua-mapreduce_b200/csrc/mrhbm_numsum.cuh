@@ -1,6 +1,7 @@
 // mrhbm_numsum.cuh -- MRHBM_RED_FSUM: a byte value as a Lua number, and the exact sum of many of them, rounded once.
-// One definition for the kernels (mrhbm_num_sum.cu) and the host's long keys (mrhbm_api.cu), host-callable so that
-// tests/native/num_sum_check.cu checks it against exact rational arithmetic on the CPU.
+// One definition for the kernels (mrhbm_num_sum.cu, and MRHBM_COMBINE_FSUM's split in mrhbm_num_combine.cu) and the
+// host's long keys (mrhbm_api.cu), host-callable so that tests/native/num_sum_check.cu and fsum_split_check.cu check it
+// against exact rational arithmetic on the CPU.
 //
 // Number encoding (include/mrhbm.h, mapreduce/tuple.py _enc_num, hbm.lua enc_num): 11 bytes, 0x10, then the IEEE
 // double's bits u sign-folded (u | 2^63 for a sign bit of 0, ~u otherwise) as ten big-endian 7-bit groups, each OR 0x80
@@ -13,6 +14,7 @@
 // when the sum is rounded.  Infinities, NaN and "some value is not -0" are kept as flags in the last word.
 #pragma once
 #include <cstdint>
+#include <cstring>
 
 #include "mrhbm_kernels.h"  // MRHBM_HD
 
@@ -161,6 +163,74 @@ MRHBM_HDI bool acc_round(int64_t* w, uint64_t* bits) {
   if (b >= kDblInf) b = kDblInf;
   *bits = sign | b;
   return true;
+}
+
+// MRHBM_COMBINE_FSUM: the greedy expansion of the accumulated sum S of a key's m values.  c1 = S rounded as acc_round
+// rounds it, c(k+1) = (S - c1 - ... - ck) rounded the same way, until the remainder is 0; infinities of one sign and an
+// exact zero give one term (acc_round's value).  Writes the terms' bits to out[0 ..] and returns their number; returns
+// 0 when the key keeps its values as emitted (|S| rounds to +-inf, or more than `max` = m terms; out[0 .. max) may
+// then hold anything) and -1 for a NaN (as acc_round).  The accumulator is consumed.
+//
+// After acc_round the accumulator holds |X| for the X it held, and the term is X rounded, so the remainder is
+// sign(X) (|X| - |term|): subtracting |term| and tracking the sign keeps the whole split in the accumulator.
+MRHBM_HDI int acc_split(int64_t* w, uint64_t* out, int max) {
+  const uint64_t f = (uint64_t)w[kAccFlags];
+  uint64_t c;
+  if (!acc_round(w, &c)) return -1;
+  if ((f & (NUM_PINF | NUM_NINF)) || (c << 1) == 0) {
+    out[0] = c;
+    return 1;
+  }
+  if ((c << 1) == kDblInf << 1) return 0;
+  uint64_t sign = 0;  // the sign bit of the factor in remainder = factor x (the accumulator's value)
+  int n = 0;
+  do {
+    if (n == max) return 0;
+    out[n++] = c ^ sign;
+    acc_add(w, c | 1ull << 63);  // minus |term|
+    sign ^= c & 1ull << 63;
+    acc_round(w, &c);
+  } while ((c << 1) != 0);
+  return n;
+}
+
+// The same split for a key of one or two finite or infinite values a, b (n = 1 or 2), in IEEE arithmetic: a + b
+// rounded is c1, and where it does not overflow TwoSum's error term is the exact remainder, so it is c2 (when not 0).
+// Returns as acc_split with max = n.
+MRHBM_HDI int two_split(uint64_t a, uint64_t b, int n, uint64_t* out) {
+  if (n == 1) {
+    out[0] = a;
+    return 1;
+  }
+#ifdef __CUDA_ARCH__
+  const double x = __longlong_as_double((long long)a), y = __longlong_as_double((long long)b);
+  const double s = __dadd_rn(x, y);
+  const double bv = __dsub_rn(s, x), av = __dsub_rn(s, bv);
+  const double e = __dadd_rn(__dsub_rn(x, av), __dsub_rn(y, bv));
+  const uint64_t sb = (uint64_t)__double_as_longlong(s), eb = (uint64_t)__double_as_longlong(e);
+#else
+  double x, y;
+  memcpy(&x, &a, 8);
+  memcpy(&y, &b, 8);
+  const volatile double s = x + y;  // (volatile: no reassociation or extended precision)
+  const volatile double bv = s - x, av = s - bv;
+  const volatile double e = (x - av) + (y - bv);
+  uint64_t sb, eb;
+  const double s_ = s, e_ = e;
+  memcpy(&sb, &s_, 8);
+  memcpy(&eb, &e_, 8);
+#endif
+  const bool ia = (a << 1) == kDblInf << 1, ib = (b << 1) == kDblInf << 1;
+  if (ia || ib) {
+    if (ia && ib && a != b) return -1;
+    out[0] = ia ? a : b;
+    return 1;
+  }
+  if ((sb << 1) == kDblInf << 1) return 0;
+  out[0] = sb;
+  if ((eb << 1) == 0) return 1;
+  out[1] = eb;
+  return 2;
 }
 
 }  // namespace mrhbm

@@ -17,6 +17,11 @@
 //     and leaves the rest as lost room until reset(): a kept pair's value id may point past the new end, to bytes
 //     that must stay where they are.  A shrunk range that dies at the tail no longer ends at used(), so no abort
 //     gives that room back.
+//   - MRHBM_COMBINE_FSUM: replace_open() empties all of an owner's open ranges and makes room taken at the tail, which
+//     holds the job's new pairs with values of their own, the owner's only open range with records.  The emptied
+//     ranges' room is lost until reset(); the new range is like any other: it dies, and at the tail gives its room
+//     back, as a whole.  An emptied range never ends at used() again (the new range lies behind it), so no abort
+//     reaches past the new range into the job's original room.
 #pragma once
 #include <cassert>
 #include <cstdint>
@@ -89,6 +94,14 @@ class PoolLedger {
         return;
       }
     assert(!"shrink: no such open range");
+  }
+  // taken room [off, off + cnt) replaces all of the owner's open ranges: they keep no records, and the room becomes an
+  // open range of the owner's of its own, never one with a range before it (see the invariants above)
+  void replace_open(uint64_t owner, const std::string& job, uint64_t off, uint64_t cnt, uint64_t aoff) {
+    assert(off + cnt == used_);
+    for (Range& r : ranges_)
+      if (r.owner == owner && r.state == OPEN) r.cnt = 0;
+    ranges_.push_back(Range{off, cnt, job, OPEN, owner, aoff});
   }
 
   void commit(uint64_t owner, const std::string& job) {

@@ -17,7 +17,9 @@ local hbm = { _VERSION = "0.1", _NAME = "mapreduce.hbm" }
 --     keys as their 8 big-endian bytes; partition k takes the keys k splitters are <= to) or hbm_splitters = "sample"
 --     (quantiles of the map output, taken at the MAP -> REDUCE barrier).  The partitionfn must compute the same ranges.
 --   reducefn / combinerfn module: hbm_reducefn = "sum"; a combinerfn module of a value_kind = "bytes" job:
---     hbm_combinerfn = "distinct" (its combinerfn emits the distinct values it is given); a reducefn module of a
+--     hbm_combinerfn = "distinct" (its combinerfn emits the distinct values it is given), or, with hbm_reducefn =
+--     "fsum", hbm_combinerfn = "fsum" (its combinerfn emits the sum of its number values; the device keeps each map
+--     job's sum per key exactly, as one or two numbers, so the result is the reducer's alone); a reducefn module of a
 --     value_kind = "bytes" job: hbm_reducefn = "fsum" (its reducefn emits the sum of its number values; the device
 --     sums them exactly, rounds once, and hbm.groups hands out that one number), or hbm_reducefn = "distinct" (its
 --     reducefn emits the distinct values ascending by their
@@ -53,19 +55,23 @@ function hbm.configure(partition_mod, reduce_mod, combiner_mod, opts)
          "value_kind = 'bytes' hands string and number values to a general reducefn: the reducefn must not declare an hbm_reducefn other than 'distinct' or 'fsum'")
   assert(not distinct_red or byte_values, "hbm_reducefn = 'distinct' needs value_kind = 'bytes'")
   assert(not fsum_red or byte_values, "hbm_reducefn = 'fsum' needs value_kind = 'bytes'")
-  assert(not fsum_red or combiner_mod == nil, "hbm_reducefn = 'fsum' takes no combinerfn")
+  -- hbm_combinerfn = "fsum" (hbm_reducefn = "fsum"): each map job's numbers per key become the exact expansion of
+  -- their sum at its commit (include/mrhbm.h, MRHBM_COMBINE_FSUM)
+  local fsum_comb = combiner_mod ~= nil and combiner_mod.hbm_combinerfn == "fsum"
+  assert(not fsum_comb or fsum_red, "hbm_combinerfn = 'fsum' needs hbm_reducefn = 'fsum' and value_kind = 'bytes'")
+  assert(not fsum_red or combiner_mod == nil or fsum_comb, "hbm_reducefn = 'fsum' takes no combinerfn but hbm_combinerfn = 'fsum'")
   -- hbm_combinerfn = "distinct" (values = "bytes"): the combinerfn keeps one copy of each distinct value of a key, so
   -- the device drops the repeated (key, value) pairs of each map job at its commit
   local distinct = combiner_mod ~= nil and combiner_mod.hbm_combinerfn == "distinct"
   assert(not distinct or byte_values, "hbm_combinerfn = 'distinct' needs value_kind = 'bytes'")
-  assert(not combiner_mod or distinct or (builtin and combiner_mod.hbm_reducefn == "sum"),
-         "a combinerfn runs on the device: it (and the reducefn) must declare hbm_reducefn = 'sum', or hbm_combinerfn = 'distinct' with value_kind = 'bytes'")
+  assert(not combiner_mod or distinct or fsum_comb or (builtin and combiner_mod.hbm_reducefn == "sum"),
+         "a combinerfn runs on the device: it (and the reducefn) must declare hbm_reducefn = 'sum', or hbm_combinerfn = 'distinct' or 'fsum' with value_kind = 'bytes'")
   local c, err = mrhbm.new{
     key_kind = tuple_keys and "str" or opts.key_kind or "str",
     max_key_bytes = opts.max_key_bytes or 123,
     num_partitions = assert(partition_mod.NUM_REDUCERS, "partitionfn module must expose NUM_REDUCERS"),
     partitioner = assert(partition_mod.hbm_partitionfn, "partitionfn module must declare hbm_partitionfn"),
-    combiner = distinct and "distinct" or combiner_mod ~= nil,
+    combiner = distinct and "distinct" or (fsum_comb and "fsum" or combiner_mod ~= nil),
     reducer = builtin and "sum" or (distinct_red and "distinct" or (fsum_red and "fsum" or "none")),
     device = opts.device,
     values = byte_values and "bytes" or "int",

@@ -37,7 +37,7 @@ static int fail(lua_State *L, mrhbm_ctx *c) { /* luamongo style: nil, msg */
 }
 
 /* mrhbm.new{ key_kind="str"|"u64", max_key_bytes=, num_partitions=, partitioner="fnv_lua"|"mulhash"|
- *            "wordhash"|"range", combiner=bool|"distinct", reducer="sum"|"none"|"distinct"|"fsum", device=,
+ *            "wordhash"|"range", combiner=bool|"distinct"|"fsum", reducer="sum"|"none"|"distinct"|"fsum", device=,
  *            values="int"|"bytes" }
  * values = "bytes" (MRHBM_F_BYTE_VALUES, needs reducer = "none", "distinct" or "fsum"): m:emit takes string
  * values and ctx:groups yields tables of strings (reducer = "distinct": each key's distinct values, ascending;
@@ -60,8 +60,9 @@ static int l_new(lua_State *L) {
   cfg.partitioner = strcmp(s, "fnv_lua") == 0 ? MRHBM_PART_FNV_LUA
                   : strcmp(s, "mulhash") == 0 ? MRHBM_PART_MULHASH
                   : strcmp(s, "range") == 0 ? MRHBM_PART_RANGE : MRHBM_PART_WORDHASH;
-  lua_getfield(L, 1, "combiner"); /* true (the built-in reducer) | "distinct" (values = "bytes") */
+  lua_getfield(L, 1, "combiner"); /* true (the built-in reducer) | "distinct" | "fsum" (values = "bytes") */
   cfg.combiner = lua_type(L, -1) == LUA_TSTRING && strcmp(luaL_checkstring(L, -1), "distinct") == 0 ? MRHBM_COMBINE_DISTINCT
+               : lua_type(L, -1) == LUA_TSTRING && strcmp(luaL_checkstring(L, -1), "fsum") == 0   ? MRHBM_COMBINE_FSUM
                : lua_toboolean(L, -1) ? MRHBM_COMBINE_REDUCER : MRHBM_COMBINE_NONE;
   lua_getfield(L, 1, "device");
   cfg.device = (int32_t)luaL_optinteger(L, -1, -1);

@@ -51,7 +51,7 @@ def distinct_combiner(comb, value_kind):
     values it is given (compared as the shuffle compares them, by their encoded bytes)."""
     from .tuple import encode_value
     if comb.hbm_combinerfn != "distinct":
-        raise ValueError("unknown hbm_combinerfn %r (built-ins: 'distinct')" % (comb.hbm_combinerfn,))
+        raise ValueError("unknown hbm_combinerfn %r (built-ins: 'distinct', 'fsum')" % (comb.hbm_combinerfn,))
     if value_kind != "bytes":
         raise ValueError("hbm_combinerfn = 'distinct' drops repeated string and number values: "
                          "configure hbm = {'value_kind': 'bytes'}")
@@ -74,23 +74,40 @@ _FSUM_PROBES = ([1, 2, 3], [0.5, 0.25, -1.75, 3], [2 ** 60, 1, -2 ** 60], [-0.0,
                 [-3.5], [1.5, -1.5, 0.125], [-2, -0.5, -0.75], [7])
 
 
-def fsum_reducer(red, value_kind):
-    """Checks a reducefn module that declares hbm_reducefn = "fsum": the device then hands every key the exact sum of
-    its number values, rounded once, and the reducefn is not called, so it must emit exactly that one number."""
+def _check_sums(fn, name):
+    """Raises unless fn (a reducefn or combinerfn, declared with hbm_<name> = "fsum") emits exactly one number, the sum,
+    on every probe."""
     from fractions import Fraction
-    if value_kind != "bytes":
-        raise ValueError("hbm_reducefn = 'fsum' sums number values carried as bytes: configure hbm = {'value_kind': 'bytes'}")
     for values in _FSUM_PROBES:
         out = []
         try:
-            red.reducefn(b"probe", list(values), out.append)
+            fn(b"probe", list(values), out.append)
         except Exception as e:
-            raise ValueError("hbm_reducefn = 'fsum': reducefn failed on the values %r: %r" % (values, e))
+            raise ValueError("hbm_%s = 'fsum': %s failed on the values %r: %r" % (name, name, values, e))
         want = float(sum(Fraction(v) for v in values))
         ok = len(out) == 1 and isinstance(out[0], (int, float)) and not isinstance(out[0], bool) and out[0] == want
         if not ok:
-            raise ValueError("hbm_reducefn = 'fsum', but reducefn turns the values %r into %r instead of their sum %r: "
-                             "the declaration must describe what the reducefn computes" % (values, out, want))
+            raise ValueError("hbm_%s = 'fsum', but %s turns the values %r into %r instead of their sum %r: "
+                             "the declaration must describe what the %s computes" % (name, name, values, out, want, name))
+
+
+def fsum_reducer(red, value_kind):
+    """Checks a reducefn module that declares hbm_reducefn = "fsum": the device then hands every key the exact sum of
+    its number values, rounded once, and the reducefn is not called, so it must emit exactly that one number."""
+    if value_kind != "bytes":
+        raise ValueError("hbm_reducefn = 'fsum' sums number values carried as bytes: configure hbm = {'value_kind': 'bytes'}")
+    _check_sums(red.reducefn, "reducefn")
+
+
+def fsum_combiner(comb, builtin_red, value_kind):
+    """Checks a combinerfn module that declares hbm_combinerfn = "fsum": the device then replaces each map job's
+    numbers per key by the exact expansion of their sum, which only the fsum reducer reads back exactly, so the
+    combinerfn must emit exactly that one sum."""
+    if builtin_red != "fsum" or value_kind != "bytes":
+        raise ValueError("hbm_combinerfn = 'fsum' keeps each map job's sums exactly for the fsum reducer: it needs "
+                         "hbm_reducefn = 'fsum' and hbm = {'value_kind': 'bytes'} (got hbm_reducefn = %r, value_kind "
+                         "= %r)" % (builtin_red, value_kind))
+    _check_sums(comb.combinerfn, "combinerfn")
 
 
 def distinct_reducer(red, value_kind):
@@ -164,8 +181,12 @@ class server:
             getattr(mods["combinerfn"], "hbm_reducefn", None) == "sum"
         # hbm_combinerfn = "distinct" (value_kind = "bytes"): the combinerfn keeps one copy of each distinct value of a
         # key, so the device drops the repeated (key, value) pairs of each map job at its commit
-        distinct = "combinerfn" in mods and getattr(mods["combinerfn"], "hbm_combinerfn", None) is not None
-        if "combinerfn" in mods and not device_combiner and not distinct:
+        declared = getattr(mods["combinerfn"], "hbm_combinerfn", None) if "combinerfn" in mods else None
+        # hbm_combinerfn = "fsum" (hbm_reducefn = "fsum", value_kind = "bytes"): each map job's numbers per key become
+        # the exact expansion of their sum at its commit
+        fsum_comb = declared == "fsum"
+        distinct = declared is not None and not fsum_comb
+        if "combinerfn" in mods and not device_combiner and not distinct and not fsum_comb:
             sys.stderr.write("# WARNING: combinerfn %s is not a device built-in (hbm_reducefn = 'sum'); it is skipped, "
                              "the reducefn sees the uncombined values\n" % params["combinerfn"])
         pname = getattr(part, "hbm_partitionfn", None)
@@ -180,6 +201,8 @@ class server:
         # value_kind = "bytes": values are Lua strings and numbers (tuple.encode_value), handed to a general reducefn
         if hbm["value_kind"] not in ("int", "bytes"):
             raise ValueError("hbm value_kind must be 'int' or 'bytes', got %r" % (hbm["value_kind"],))
+        if fsum_comb:
+            fsum_combiner(mods["combinerfn"], builtin_red, hbm["value_kind"])
         if hbm["value_kind"] == "bytes" and builtin_red not in (None, "distinct", "fsum"):
             raise ValueError("hbm value_kind = 'bytes' hands string and number values to a general reducefn: "
                              "the reducefn module must not declare an hbm_reducefn other than 'distinct' or 'fsum' (it "
@@ -197,7 +220,7 @@ class server:
         if distinct:
             distinct_combiner(mods["combinerfn"], hbm["value_kind"])
         hbm.update(partitioner=_BUILTIN_PART[pname], num_partitions=nparts,
-                   combiner="distinct" if distinct else device_combiner,
+                   combiner="distinct" if distinct else "fsum" if fsum_comb else device_combiner,
                    reducer={"sum": 0, "distinct": 2, "fsum": 3}.get(builtin_red, 1),
                    splitters=range_splitters(part, nparts, hbm["key_kind"]) if pname == "range" else None)
         self.config = dict(mapfn=params["mapfn"], reducefn=params["reducefn"], partitionfn=params["partitionfn"],
@@ -211,7 +234,7 @@ class server:
             return self.ctx_factory(h)
         from .. import mrhbm
         kind = mrhbm.KEY_U64 if h["key_kind"] == "u64" else mrhbm.KEY_STR
-        combiner = mrhbm.COMBINE_DISTINCT if h["combiner"] == "distinct" else h["combiner"]
+        combiner = {"distinct": mrhbm.COMBINE_DISTINCT, "fsum": mrhbm.COMBINE_FSUM}.get(h["combiner"], h["combiner"])
         ctx = mrhbm.Ctx(kind, h["num_partitions"], h["partitioner"], max_key_bytes=h["max_key_bytes"],
                         combiner=combiner, device=h["device"], reducer=h["reducer"],
                         flags=mrhbm.F_BYTE_VALUES if h.get("value_kind") == "bytes" else 0)

@@ -13,7 +13,7 @@ from . import build as _build
 KEY_U64, KEY_STR = 0, 1
 PART_FNV_LUA, PART_MULHASH, PART_WORDHASH, PART_RANGE = 0, 1, 2, 3
 RED_SUM, RED_NONE, RED_DISTINCT, RED_FSUM = 0, 1, 2, 3
-COMBINE_NONE, COMBINE_REDUCER, COMBINE_DISTINCT = 0, 1, 2
+COMBINE_NONE, COMBINE_REDUCER, COMBINE_DISTINCT, COMBINE_FSUM = 0, 1, 2, 3
 F_FORCE_RUNS, F_SMALL_BINS, F_NO_OPTIMISTIC, F_BYTE_VALUES = 1, 2, 4, 8
 E_NODEVICE = -8
 UNIQUE_ID_BYTES = 128
@@ -272,8 +272,9 @@ class Ctx:
         self.L = load()
         if partitioner is None:
             partitioner = PART_MULHASH if key_kind == KEY_U64 else PART_FNV_LUA
-        # combiner: a bool (False / True = COMBINE_REDUCER) or COMBINE_DISTINCT (byte values, see include/mrhbm.h)
-        combiner = COMBINE_DISTINCT if combiner == COMBINE_DISTINCT else int(bool(combiner))
+        # combiner: a bool (False / True = COMBINE_REDUCER), COMBINE_DISTINCT or COMBINE_FSUM (byte values, see
+        # include/mrhbm.h)
+        combiner = combiner if combiner in (COMBINE_DISTINCT, COMBINE_FSUM) else int(bool(combiner))
         self.cfg = Config(C.sizeof(Config), device, key_kind, max_key_bytes, num_partitions, partitioner,
                           reducer, combiner, reserve_pairs, flags, 0)
         self.h = C.c_void_p()
