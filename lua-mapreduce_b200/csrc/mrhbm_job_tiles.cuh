@@ -30,9 +30,21 @@ __device__ __forceinline__ bool tile_record(const DistinctRange* __restrict__ rg
   return true;
 }
 
-__device__ __forceinline__ uint64_t fp_step(uint64_t h, uint64_t x) {
+// (host-callable, so that tests/native/fsum_fingerprint_check.cu can check the tests' model of the hash set)
+__host__ __device__ __forceinline__ uint64_t fp_step(uint64_t h, uint64_t x) {
   h = (h ^ x) * 0x9E3779B97F4A7C15ull;
   return h ^ (h >> 29);
+}
+
+// MRHBM_COMBINE_FSUM's 64-bit fingerprint of the key slot words (never ~0, the empty entry)
+template <int RB>
+__host__ __device__ __forceinline__ uint64_t key_fingerprint(const uint32_t* r) {
+  uint64_t h = 0x5851F42D4C957F2Dull;
+#pragma unroll
+  for (int i = 0; i < Rec<RB>::kKeyWords; i += 2)
+    h = fp_step(h, (uint64_t)r[i] | (i + 1 < Rec<RB>::kKeyWords ? (uint64_t)r[i + 1] << 32 : 0ull));
+  h = mix64(h);
+  return h == ~0ull ? 0 : h;
 }
 
 template <int RB>

@@ -33,17 +33,6 @@ constexpr int kThreads = 256;
 // stride (a half warp's 8-byte words in different banks), so that the adds need no atomics however alike the values
 constexpr int kAccThreads = 64, kAccWarps = kAccThreads / 32, kAccStride = kAccWords + 1;
 
-// 64-bit fingerprint of the key slot words (never kEmpty)
-template <int RB>
-__device__ __forceinline__ uint64_t key_fingerprint(const uint32_t* r) {
-  uint64_t h = 0x5851F42D4C957F2Dull;
-#pragma unroll
-  for (int i = 0; i < Rec<RB>::kKeyWords; i += 2)
-    h = fp_step(h, (uint64_t)r[i] | (i + 1 < Rec<RB>::kKeyWords ? (uint64_t)r[i + 1] << 32 : 0ull));
-  h = mix64(h);
-  return h == kEmpty ? 0 : h;
-}
-
 struct Words {
   uint32_t *cnt, *start, *cursor, *nterm;
   __device__ Words(const FsumScratch& fs) {
