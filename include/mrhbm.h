@@ -189,7 +189,7 @@ typedef struct mrhbm_config {
  * reducer: MRHBM_RED_DISTINCT, MRHBM_RED_FSUM) and combiner
  * MRHBM_COMBINE_NONE or MRHBM_COMBINE_DISTINCT (else mrhbm_init fails with MRHBM_E_INVAL) and one GPU (mrhbm_comm_init with world > 1 fails).  On such a ctx:
  *   - pairs are emitted with mrhbm_emit_str_value / mrhbm_emit_u64_value / mrhbm_emit_batch_values /
- *     mrhbm_map_words_value; the integer-valued emits (emit_str, emit_u64, emit_batch, emit_device, map_gen_*,
+ *     mrhbm_map_words_value / mrhbm_map_key_numbers; the integer-valued emits (emit_str, emit_u64, emit_batch, emit_device, map_gen_*,
  *     map_wordcount) fail with MRHBM_E_INVAL;
  *   - groups are read with mrhbm_groups_next_values (mrhbm_groups_next fails) and rows with mrhbm_result_values;
  *     mrhbm_result_copy needs sums = NULL;
@@ -275,6 +275,23 @@ int mrhbm_emit_batch_values(mrhbm_map *, const void *records, size_t n, const vo
  * name as the value).  val is copied before return (vlen <= 1 GiB, 0 allowed).  *words (optional) receives the token
  * count.  String-key ctx only. */
 int mrhbm_map_words_value(mrhbm_map *, const void *text, size_t len, const void *val, size_t vlen, uint64_t *words);
+/* MRHBM_F_BYTE_VALUES, string-key ctx only (else MRHBM_E_INVAL): the map side of a number sum over text lines
+ * "key number" (bytes per URL, sales per product, edge weights per node), parsed on the device.
+ *   - Lines: the text is cut into lines at '\n'; a last line without '\n' counts.  A line made only of C-locale white
+ *     space (' ' \t \n \v \f \r) emits nothing.  A field is a maximal run of non-space bytes; every other line must
+ *     have exactly two fields, the key, then the number.
+ *   - Key: the first field's bytes, 0x00 and 0x01 escaped as in mrhbm_emit_str; a key longer than the record class
+ *     takes the long-key path of mrhbm_emit_str_value (its 64 MB piece is parsed on the host).
+ *   - Number: the second field must match [+-]?(D+(\.D*)?|\.D+)([eE][+-]?D+)? -- the decimal form Lua 5.2's tonumber
+ *     takes through strtod.  Unlike Lua, hexadecimal numbers (0x10), inf, nan and anything else are refused.  Its
+ *     value is the nearest double, ties to even (Python's float()): a magnitude beyond the largest double gives +-inf,
+ *     underflow a correctly rounded subnormal or +-0, and -0 stays -0.  The value is stored as the 11-byte number
+ *     encoding (see MRHBM_RED_FSUM), the bytes of tuple.encode_value(float(field)).
+ *   - Pairs: one per line, in text order; each has its own 11-byte value and its value id is its own pool index.
+ *   - Failure: a line that breaks these rules, or one longer than a 64 MB piece, fails the call with MRHBM_E_INVAL and
+ *     a message giving the line's byte offset.  A failed call emits nothing.
+ * *lines (optional) receives the number of pairs emitted. */
+int mrhbm_map_key_numbers(mrhbm_map *, const void *text, size_t len, uint64_t *lines);
 
 /* ---- barrier between MAP and REDUCE (server.lua:279-329) ---- */
 /* hash-partition [+ NCCL all-to-all] + sort + segmented reduce of everything committed */

@@ -18,6 +18,7 @@
 
 #include "../../include/mrhbm.h"
 #include "mrhbm_comm.h"
+#include "mrhbm_decimal.cuh"
 #include "mrhbm_kernels.h"
 #include "mrhbm_dev.cuh"  // splitmix64
 #include "mrhbm_keys.h"
@@ -118,6 +119,9 @@ struct mrhbm_ctx {
   uint32_t *d_tok_cnt = nullptr, *d_tok_off = nullptr;
   cudaStream_t copy_stream = nullptr;
   cudaEvent_t tok_ev[2] = {nullptr, nullptr};
+  // mrhbm_map_key_numbers: the power-of-five table of the decimal conversion and the fix-up list (kKnFixCap entries)
+  uint64_t* d_pow5 = nullptr;
+  void* d_kn_fix = nullptr;
   // map-side combiner: the global (L2 resident) hash table and the records compacted out of it
   void *comb = nullptr, *gtab = nullptr;
   uint64_t comb_cap = 0, gtab_cap = 0;  // records
@@ -885,7 +889,7 @@ void mrhbm_destroy(mrhbm_ctx* c) {
                    c->cvals,       c->row_off,     c->val_tile,   c->val_pieces, c->dd_tab,     c->dd_out,
                    c->dd_rg,       c->dd_slot,     c->dd_tiles,   c->vo_keys,    c->vo_ids,
                    c->ns_acc,      c->ns_flags,    c->ns_head,    c->fs_words,   c->fs_big,     c->fs_small,
-                   c->fs_vals,     c->fs_gacc};
+                   c->fs_vals,     c->fs_gacc,     c->d_pow5,     c->d_kn_fix};
   for (void* p : frees)
     if (p) cudaFree(p);
   if (c->h_counters) cudaFreeHost(c->h_counters);
@@ -1092,21 +1096,21 @@ int mrhbm_map_gen_zipf(mrhbm_map* m, uint64_t seed, uint64_t start, uint64_t n, 
 
 namespace {
 
-// The device tokeniser of mrhbm_map_wordcount and mrhbm_map_words_value (the caller has checked the ctx and the
-// arguments): every maximal run of non-space bytes of the text becomes the pair (word, 1), or on a byte-values ctx
-// (word, val[0 .. vlen)).  With byte values the value bytes go to the arena once per device piece and every pair of
-// the piece carries the value id of the piece's first pair (see PoolLedger).
-int map_words(mrhbm_map* m, const unsigned char* t, size_t len, const void* val, size_t vlen, uint64_t* words) {
+constexpr size_t kTokPiece = 64u << 20;  // bytes of text per device piece
+inline bool is_space(unsigned char ch) { return ch == ' ' || (ch >= 9 && ch <= 13); }
+
+// The piece driver of the device mapfns over text (the caller has checked the ctx and the arguments).  The text is
+// handled in pieces of <= kTokPiece bytes through two device buffers: the upload of piece k+1 (copy stream) runs while
+// piece k is counted, scanned and emitted (ctx stream).  The scratch (text x 2, per-256-byte-block counts and offsets)
+// lives with the ctx.  Job says where a piece may end -- after white space, or with Job::kLines after '\n' -- and
+// handles one piece: job.device(...) on the device, which may leave it to job.host(...) on the host (a key that does
+// not fit the record class, say).  A failure of either emits nothing of the call.
+template <class Job>
+int map_pieces(mrhbm_map* m, const unsigned char* t, size_t len, Job& job, uint64_t* count) {
   mrhbm_ctx* c = m->ctx;
-  const char* what = c->bytevals ? "words_value" : "wordcount";
   if (!len) return MRHBM_OK;
   int rc = stage_flush(m);
   if (rc) return rc;
-  // The text is tokenised in pieces of <= kTokPiece bytes that end at white space, through two device buffers: the
-  // upload of piece k+1 (copy stream) runs while piece k is counted, scanned and emitted (ctx stream).  The scratch
-  // (text x 2, per-256-byte-block word counts and offsets) lives with the ctx.
-  constexpr size_t kTokPiece = 64u << 20;
-  auto is_space = [](unsigned char ch) { return ch == ' ' || (ch >= 9 && ch <= 13); };
   if (!c->d_tok_text[0]) {
     const uint64_t tcap = kTokPiece + 4096, bcap = tok_blocks(tcap) + 1;
     cudaError_t ea = cudaMalloc((void**)&c->d_tok_text[0], tcap);
@@ -1117,85 +1121,54 @@ int map_words(mrhbm_map* m, const unsigned char* t, size_t len, const void* val,
     for (int i = 0; i < 2 && ea == cudaSuccess; i++) ea = cudaEventCreateWithFlags(&c->tok_ev[i], cudaEventDisableTiming);
     if (ea != cudaSuccess) {
       cudaGetLastError();
-      return fail(c, MRHBM_E_NOMEM, "%s: %s", what, cudaGetErrorString(ea));
+      return fail(c, MRHBM_E_NOMEM, "%s: %s", job.what, cudaGetErrorString(ea));
     }
   }
-  // undo information: a word that does not fit emits NOTHING of this call
+  // undo information: a piece that fails emits NOTHING of this call
   const PoolLedger::Mark mark0 = c->led.mark();
   const size_t long0 = m->long_pairs.size();
-  auto piece_end = [&](size_t p) -> size_t {  // end of the piece that starts at p: <= kTokPiece bytes, cut after white space
+  auto piece_end = [&](size_t p) -> size_t {  // end of the piece that starts at p: <= kTokPiece bytes
     size_t e = std::min(len, p + kTokPiece);
     if (e < len) {
       size_t q = e;
+      if constexpr (Job::kLines) {  // cut after the last '\n'; p itself when the line is longer than a piece
+        while (q > p && t[q - 1] != '\n') q--;
+        return q;
+      }
       while (q > p && !is_space(t[q - 1])) q--;
       if (q > p) e = q;  // (no white space in 64 MB: one giant "word", the length check below refuses it)
     }
     return e;
   };
+  auto long_line = [&](size_t p) {
+    return fail(c, MRHBM_E_INVAL, "%s: the line at byte %zu is longer than a piece (%zu bytes)", job.what, p, kTokPiece);
+  };
   cudaError_t e = cudaSuccess;
-  uint64_t total_words = 0;
-  uint32_t* flagw = c->d_small + 1;
+  uint64_t total_pairs = 0;
   size_t p = 0, pe = piece_end(0);
+  if (pe == 0) return long_line(0);
   int k = 0;
   e = cudaMemcpyAsync(c->d_tok_text[0], t, pe, cudaMemcpyHostToDevice, c->copy_stream);
   if (e == cudaSuccess) e = cudaEventRecord(c->tok_ev[0], c->copy_stream);
   while (e == cudaSuccess && rc == 0 && p < len) {
     const size_t n = pe - p, pn = pe, pne = pe < len ? piece_end(pe) : pe;
+    if (pne == pn && pn < len) {
+      rc = long_line(pn);
+      break;
+    }
     unsigned char* d_text = c->d_tok_text[k & 1];
     if (pn < len) {  // next piece's upload: its buffer was last read by piece k-1, whose kernels are behind a sync
       e = cudaMemcpyAsync(c->d_tok_text[(k + 1) & 1], t + pn, pne - pn, cudaMemcpyHostToDevice, c->copy_stream);
       if (e == cudaSuccess) e = cudaEventRecord(c->tok_ev[(k + 1) & 1], c->copy_stream);
       if (e != cudaSuccess) break;
     }
-    const uint64_t nb = tok_blocks(n);
     if ((e = cudaStreamWaitEvent(c->stream, c->tok_ev[k & 1], 0)) != cudaSuccess) break;
-    launch_tok_count(d_text, n, c->d_tok_cnt, c->stream);
-    launch_exscan(c->d_tok_cnt, (uint32_t)nb, c->d_tok_off, nullptr, nullptr, 0xffffffffu, nullptr, nullptr, c->d_small, 0, c->stream,
-                  c->d_small + 64);
-    if ((e = cudaMemcpyAsync(c->h_small, c->d_small, 4, cudaMemcpyDeviceToHost, c->stream)) != cudaSuccess) break;
-    if ((e = cudaStreamSynchronize(c->stream)) != cudaSuccess) break;
-    const uint64_t total = c->h_small[0];
-    if (total) {
-      bool fit = false;
-      {
-        Reservation r;
-        rc = reserve(c, nullptr, total, c->bytevals ? vlen : 0, r);
-        if (rc) break;
-        uint32_t value = 1;
-        if (c->bytevals) {  // one copy of the value; ids r.off + 1 .. r.off + total - 1 get empty values
-          if (vlen && (e = cudaMemcpyAsync(c->arena + r.aoff, val, vlen, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess)
-            break;
-          launch_value_stamp(c->rb, nullptr, total, 0, c->voff + r.off, vlen, r.aoff, c->stream);
-          value = (uint32_t)r.off;
-        }
-        if ((e = cudaMemsetAsync(flagw, 0, 4, c->stream)) != cudaSuccess) break;
-        launch_tok_emit(c->rb, d_text, n, c->d_tok_off, (char*)c->pool + r.off * c->rb, value, flagw, c->stream);
-        if ((e = cudaMemcpyAsync(c->h_small + 1, flagw, 4, cudaMemcpyDeviceToHost, c->stream)) != cudaSuccess) break;
-        if ((e = cudaStreamSynchronize(c->stream)) != cudaSuccess) break;
-        fit = !(c->h_small[1] & ERRF_KEYLEN);
-        if (fit) r.add(m);
-      }
-      if (!fit) {
-        // a word of this piece does not fit the key slot (a URL in a corpus): the piece's records are dropped again and
-        // the piece is tokenised on the host -- words that fit are staged like emit_str / emit_str_value pairs, the
-        // long ones go to the host-side store of long keys.  Rare by assumption: 64 MB take a fraction of a second here.
-        uint64_t words_here = 0;
-        for (size_t a = p; a < pn && rc == 0;) {
-          while (a < pn && is_space(t[a])) a++;
-          size_t b = a;
-          while (b < pn && !is_space(t[b])) b++;
-          if (b > a) {
-            rc = c->bytevals ? mrhbm_emit_str_value(m, t + a, b - a, val, vlen) : mrhbm_emit_str(m, t + a, b - a, 1u);
-            words_here++;
-          }
-          a = b;
-        }
-        if (rc) break;
-        total_words += words_here;
-      } else {
-        total_words += total;
-      }
-    }
+    bool on_host = false;
+    uint64_t pairs = 0;
+    e = job.device(d_text, p, n, rc, on_host, pairs);
+    if (e != cudaSuccess || rc) break;
+    if (on_host && (rc = job.host(p, pn, pairs)) != 0) break;
+    total_pairs += pairs;
     p = pn;
     pe = pne;
     k++;
@@ -1204,17 +1177,188 @@ int map_words(mrhbm_map* m, const unsigned char* t, size_t len, const void* val,
     cudaStreamSynchronize(c->copy_stream);  // an upload may still be reading the caller's text
     cudaStreamSynchronize(c->stream);
     c->led.rewind(mark0);
-    m->long_pairs.resize(long0);  // (words of a piece that was tokenised on the host)
+    m->long_pairs.resize(long0);  // (pairs of a piece that was handled on the host)
     m->fill = 0;                  // the staging buffer was empty when the call began (stage_flush above)
     if (e != cudaSuccess) {
       cudaGetLastError();
-      return fail(c, MRHBM_E_CUDA, "%s: %s", what, cudaGetErrorString(e));
+      return fail(c, MRHBM_E_CUDA, "%s: %s", job.what, cudaGetErrorString(e));
     }
     return rc;
   }
-  if (words) *words = total_words;
+  if (count) *count = total_pairs;
   return MRHBM_OK;
 }
+
+// mrhbm_map_wordcount and mrhbm_map_words_value: every maximal run of non-space bytes of the text becomes the pair
+// (word, 1), or on a byte-values ctx (word, val[0 .. vlen)).  With byte values the value bytes go to the arena once per
+// device piece and every pair of the piece carries the value id of the piece's first pair (see PoolLedger).
+struct WordsJob {
+  static constexpr bool kLines = false;
+  mrhbm_map* m;
+  const unsigned char* t;
+  const void* val;
+  size_t vlen;
+  const char* what;
+
+  cudaError_t device(const unsigned char* d_text, size_t, size_t n, int& rc, bool& on_host, uint64_t& pairs) {
+    mrhbm_ctx* c = m->ctx;
+    cudaError_t e;
+    uint32_t* flagw = c->d_small + 1;
+    const uint64_t nb = tok_blocks(n);
+    launch_tok_count(d_text, n, c->d_tok_cnt, c->stream);
+    launch_exscan(c->d_tok_cnt, (uint32_t)nb, c->d_tok_off, nullptr, nullptr, 0xffffffffu, nullptr, nullptr, c->d_small, 0, c->stream,
+                  c->d_small + 64);
+    if ((e = cudaMemcpyAsync(c->h_small, c->d_small, 4, cudaMemcpyDeviceToHost, c->stream)) != cudaSuccess) return e;
+    if ((e = cudaStreamSynchronize(c->stream)) != cudaSuccess) return e;
+    const uint64_t total = c->h_small[0];
+    if (!total) return cudaSuccess;
+    Reservation r;
+    rc = reserve(c, nullptr, total, c->bytevals ? vlen : 0, r);
+    if (rc) return cudaSuccess;
+    uint32_t value = 1;
+    if (c->bytevals) {  // one copy of the value; ids r.off + 1 .. r.off + total - 1 get empty values
+      if (vlen && (e = cudaMemcpyAsync(c->arena + r.aoff, val, vlen, cudaMemcpyHostToDevice, c->stream)) != cudaSuccess)
+        return e;
+      launch_value_stamp(c->rb, nullptr, total, 0, c->voff + r.off, vlen, r.aoff, c->stream);
+      value = (uint32_t)r.off;
+    }
+    if ((e = cudaMemsetAsync(flagw, 0, 4, c->stream)) != cudaSuccess) return e;
+    launch_tok_emit(c->rb, d_text, n, c->d_tok_off, (char*)c->pool + r.off * c->rb, value, flagw, c->stream);
+    if ((e = cudaMemcpyAsync(c->h_small + 1, flagw, 4, cudaMemcpyDeviceToHost, c->stream)) != cudaSuccess) return e;
+    if ((e = cudaStreamSynchronize(c->stream)) != cudaSuccess) return e;
+    if (c->h_small[1] & ERRF_KEYLEN) {  // the piece's records are dropped again (r rewinds)
+      on_host = true;
+      return cudaSuccess;
+    }
+    r.add(m);
+    pairs = total;
+    return cudaSuccess;
+  }
+  // a word of this piece does not fit the key slot (a URL in a corpus): the piece is tokenised on the host -- words
+  // that fit are staged like emit_str / emit_str_value pairs, the long ones go to the host-side store of long keys.
+  // Rare by assumption: 64 MB take a fraction of a second here.
+  int host(size_t p, size_t pn, uint64_t& pairs) {
+    mrhbm_ctx* c = m->ctx;
+    int rc = 0;
+    uint64_t words_here = 0;
+    for (size_t a = p; a < pn && rc == 0;) {
+      while (a < pn && is_space(t[a])) a++;
+      size_t b = a;
+      while (b < pn && !is_space(t[b])) b++;
+      if (b > a) {
+        rc = c->bytevals ? mrhbm_emit_str_value(m, t + a, b - a, val, vlen) : mrhbm_emit_str(m, t + a, b - a, 1u);
+        words_here++;
+      }
+      a = b;
+    }
+    if (!rc) pairs = words_here;
+    return rc;
+  }
+};
+
+// mrhbm_map_key_numbers: every line "key number" becomes the pair (key, the number's 11 bytes), each pair with a value
+// of its own.  A device piece reserves one record and 11 value bytes per line; the kernel writes the records, voff and
+// the values, and lists the tokens the device does not round (mrhbm_decimal.cuh), which the host then rounds and
+// patches.  A key longer than the record class, or more such tokens than the list holds, leaves the piece to the host.
+constexpr uint32_t kKnFixCap = 1u << 16;
+struct KeyNumbersJob {
+  static constexpr bool kLines = true;
+  mrhbm_map* m;
+  const unsigned char* t;
+  const char* what = "key_numbers";
+
+  int bad_line(size_t at) {
+    return fail(m->ctx, MRHBM_E_INVAL, "key_numbers: the line at byte %zu is not \"key number\" (a decimal number)", at);
+  }
+  cudaError_t device(const unsigned char* d_text, size_t p, size_t n, int& rc, bool& on_host, uint64_t& pairs) {
+    mrhbm_ctx* c = m->ctx;
+    cudaError_t e;
+    uint32_t* flags = c->d_small + 1;  // [0] ERRF_*, [1] the first malformed line's offset, [2] fix-ups
+    const uint64_t nb = tok_blocks(n);
+    launch_kn_count(d_text, n, c->d_tok_cnt, c->stream);
+    launch_exscan(c->d_tok_cnt, (uint32_t)nb, c->d_tok_off, nullptr, nullptr, 0xffffffffu, nullptr, nullptr, c->d_small, 0, c->stream,
+                  c->d_small + 64);
+    if ((e = cudaMemcpyAsync(c->h_small, c->d_small, 4, cudaMemcpyDeviceToHost, c->stream)) != cudaSuccess) return e;
+    if ((e = cudaStreamSynchronize(c->stream)) != cudaSuccess) return e;
+    const uint64_t total = c->h_small[0];
+    if (!total) return cudaSuccess;
+    Reservation r;
+    rc = reserve(c, nullptr, total, total * kNumBytes, r);
+    if (rc) return cudaSuccess;
+    if ((e = cudaMemsetAsync(flags, 0, 12, c->stream)) != cudaSuccess) return e;
+    if ((e = cudaMemsetAsync(flags + 1, 0xff, 4, c->stream)) != cudaSuccess) return e;
+    const KnOut o{(uint4*)((char*)c->pool + r.off * c->rb), c->arena + r.aoff, c->voff + r.off, r.off, r.aoff,
+                  c->d_pow5, (uint4*)c->d_kn_fix, kKnFixCap, flags};
+    launch_kn_emit(c->rb, d_text, n, c->d_tok_off, o, c->stream);
+    if ((e = cudaMemcpyAsync(c->h_small + 1, flags, 12, cudaMemcpyDeviceToHost, c->stream)) != cudaSuccess) return e;
+    if ((e = cudaStreamSynchronize(c->stream)) != cudaSuccess) return e;
+    const uint32_t ef = c->h_small[1], nfix = c->h_small[3];
+    if (ef & ERRF_LINE) {
+      rc = bad_line(p + c->h_small[2]);
+      return cudaSuccess;
+    }
+    if ((ef & ERRF_KEYLEN) || nfix > kKnFixCap) {  // the piece's records are dropped again (r rewinds)
+      on_host = true;
+      return cudaSuccess;
+    }
+    if (nfix) {
+      std::vector<uint4> fx(nfix);
+      if ((e = cudaMemcpyAsync(fx.data(), c->d_kn_fix, nfix * sizeof(uint4), cudaMemcpyDeviceToHost, c->stream)) != cudaSuccess)
+        return e;
+      if ((e = cudaStreamSynchronize(c->stream)) != cudaSuccess) return e;
+      std::vector<ulonglong2> patch(nfix);
+      for (uint32_t i = 0; i < nfix; i++) {
+        uint64_t bits = 0;
+        dec_parse_host(t + p + fx[i].y, fx[i].z, &bits);  // (the kernel has checked the grammar)
+        patch[i] = make_ulonglong2(fx[i].x, bits);
+      }
+      // (pageable: staged before the call returns)
+      if ((e = cudaMemcpyAsync(c->d_kn_fix, patch.data(), nfix * sizeof(ulonglong2), cudaMemcpyHostToDevice, c->stream)) !=
+          cudaSuccess)
+        return e;
+      launch_kn_patch(c->d_kn_fix, nfix, c->arena + r.aoff, c->stream);
+    }
+    r.add(m);
+    pairs = total;
+    return cudaSuccess;
+  }
+  // the same lines on the host, the same grammar, values from std::from_chars, pairs through mrhbm_emit_str_value
+  // (long keys to the host-side store); flushed at the end so that the next device piece's records follow them
+  int host(size_t p, size_t pn, uint64_t& pairs) {
+    uint64_t here = 0;
+    for (size_t a = p; a < pn;) {
+      size_t eol = a;
+      while (eol < pn && t[eol] != '\n') eol++;
+      size_t f[4], nf = 0, i = a;  // the first two fields' bounds
+      bool extra = false;
+      while (i < eol) {
+        while (i < eol && is_space(t[i])) i++;
+        if (i == eol) break;
+        const size_t b = i;
+        while (i < eol && !is_space(t[i])) i++;
+        if (nf == 4) {
+          extra = true;
+          break;
+        }
+        f[nf++] = b;
+        f[nf++] = i;
+      }
+      if (nf) {
+        uint64_t bits = 0;
+        if (extra || nf != 4 || !dec_parse_host(t + f[2], f[3] - f[2], &bits)) return bad_line(a);
+        unsigned char enc[kNumBytes];
+        num_encode(bits, enc);
+        const int rc = mrhbm_emit_str_value(m, t + f[0], f[1] - f[0], enc, kNumBytes);
+        if (rc) return rc;
+        here++;
+      }
+      a = eol + 1;
+    }
+    const int rc = stage_flush(m);
+    if (!rc) pairs = here;
+    return rc;
+  }
+};
 
 }  // namespace
 
@@ -1227,7 +1371,8 @@ int mrhbm_map_wordcount(mrhbm_map* m, const void* text, size_t len, uint64_t* wo
   if (words) *words = 0;
   if (c->cfg.key_kind != MRHBM_KEY_STR) return fail(c, MRHBM_E_INVAL, "wordcount needs a string-key ctx");
   if (c->bytevals) return refuse_int_values(c);
-  return map_words(m, (const unsigned char*)text, len, nullptr, 0, words);
+  WordsJob job{m, (const unsigned char*)text, nullptr, 0, "wordcount"};
+  return map_pieces(m, (const unsigned char*)text, len, job, words);
 }
 
 int mrhbm_map_words_value(mrhbm_map* m, const void* text, size_t len, const void* val, size_t vlen, uint64_t* words) {
@@ -1239,7 +1384,38 @@ int mrhbm_map_words_value(mrhbm_map* m, const void* text, size_t len, const void
   if (c->cfg.key_kind != MRHBM_KEY_STR) return fail(c, MRHBM_E_INVAL, "words_value needs a string-key ctx");
   int rc = check_value(c, val, vlen);
   if (rc) return rc;
-  return map_words(m, (const unsigned char*)text, len, val, vlen, words);
+  WordsJob job{m, (const unsigned char*)text, val, vlen, "words_value"};
+  return map_pieces(m, (const unsigned char*)text, len, job, words);
+}
+
+int mrhbm_map_key_numbers(mrhbm_map* m, const void* text, size_t len, uint64_t* lines) {
+  if (!m || (!text && len)) return MRHBM_E_INVAL;
+  mrhbm_ctx* c = m->ctx;
+  Entry g(c);
+  if (lines) *lines = 0;
+  if (!c->bytevals) return refuse_byte_values(c);
+  if (c->cfg.key_kind != MRHBM_KEY_STR) return fail(c, MRHBM_E_INVAL, "key_numbers needs a string-key ctx");
+  if (!c->d_pow5) {
+    static const std::vector<uint64_t> pow5 = [] {  // (computed once per process)
+      std::vector<uint64_t> v(2 * kPow5Count);
+      dec_pow5_table(v.data());
+      return v;
+    }();
+    cudaError_t ea = cudaMalloc((void**)&c->d_pow5, pow5.size() * sizeof(uint64_t));
+    if (ea == cudaSuccess) ea = cudaMalloc(&c->d_kn_fix, kKnFixCap * sizeof(uint4));
+    if (ea == cudaSuccess)
+      ea = cudaMemcpy(c->d_pow5, pow5.data(), pow5.size() * sizeof(uint64_t), cudaMemcpyHostToDevice);
+    if (ea != cudaSuccess) {
+      cudaGetLastError();
+      if (c->d_pow5) cudaFree(c->d_pow5);
+      if (c->d_kn_fix) cudaFree(c->d_kn_fix);
+      c->d_pow5 = nullptr;
+      c->d_kn_fix = nullptr;
+      return fail(c, MRHBM_E_NOMEM, "key_numbers: %s", cudaGetErrorString(ea));
+    }
+  }
+  KeyNumbersJob job{m, (const unsigned char*)text};
+  return map_pieces(m, (const unsigned char*)text, len, job, lines);
 }
 
 // ---- synthetic word-count text (SURVEY App. B), host side: the input of the end-to-end word-count measurements

@@ -13,6 +13,7 @@
 #include <algorithm>
 #include <type_traits>
 
+#include "mrhbm_decimal.cuh"
 #include "mrhbm_dev.cuh"
 #include "mrhbm_sort.cuh"
 #include "mrhbm_split_plan.h"
@@ -143,6 +144,110 @@ __global__ void __launch_bounds__(256) k_tok_emit(const unsigned char* __restric
     uint4* d = recs + ((uint64_t)block_off[blk] + before) * (RB / 16);
 #pragma unroll
     for (int v = 0; v < RB / 16; v++) d[v] = rec.v[v];
+  }
+}
+
+// ============================================================================
+// device-side key-number mapfn (mrhbm_map_key_numbers): lines "key number" -> (key, 11-byte number)
+// ============================================================================
+// The start of a line's first field: a field start with only white space other than '\n' back to the line's start
+// (the piece starts at a line start).  *ls: the line's start.
+__device__ __forceinline__ bool kn_first(const unsigned char* t, uint64_t i, uint64_t* ls) {
+  if (!tok_start(t, i)) return false;
+  uint64_t j = i;
+  while (j > 0 && t[j - 1] != '\n' && tok_space(t[j - 1])) j--;
+  *ls = j;
+  return j == 0 || t[j - 1] == '\n';
+}
+// one thread per byte, one count of first fields per 256-byte block
+__global__ void __launch_bounds__(256) k_kn_count(const unsigned char* __restrict__ t, uint64_t len,
+                                                  uint32_t* __restrict__ block_counts) {
+  uint64_t nb = (len + 255) / 256, ls;
+  for (uint64_t blk = blockIdx.x; blk < nb; blk += gridDim.x) {
+    uint64_t i = blk * 256 + threadIdx.x;
+    int st = i < len && kn_first(t, i, &ls);
+    int c = __syncthreads_count(st);
+    if (threadIdx.x == 0) block_counts[blk] = (uint32_t)c;
+  }
+}
+// The thread at a first field walks its line: key, white space, number, white space up to '\n'.  Pair idx (its rank
+// among the piece's lines) gets record recs[idx] with value id first + idx, and its encoded number at vals + 11 idx.
+template <int RB>
+__global__ void __launch_bounds__(256) k_kn_emit(const unsigned char* __restrict__ t, uint64_t len,
+                                                 const uint32_t* __restrict__ block_off, KnOut o) {
+  constexpr int KB = Rec<RB>::kKeyBytes;
+  __shared__ uint32_t wcount[8];
+  uint64_t nb = (len + 255) / 256;
+  for (uint64_t blk = blockIdx.x; blk < nb; blk += gridDim.x) {
+    uint64_t i = blk * 256 + threadIdx.x, ls = 0;
+    bool st = i < len && kn_first(t, i, &ls);
+    uint32_t m = __ballot_sync(0xffffffffu, st);
+    uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (lane == 0) wcount[warp] = __popc(m);
+    __syncthreads();
+    uint32_t before = __popc(m & ((1u << lane) - 1u));
+    for (uint32_t w = 0; w < warp; w++) before += wcount[w];
+    __syncthreads();
+    if (!st) continue;
+    const uint64_t idx = (uint64_t)block_off[blk] + before;
+    union {
+      unsigned char b[RB];
+      uint4 v[RB / 16];
+    } rec;
+#pragma unroll
+    for (int v = 0; v < RB / 16; v++) rec.v[v] = make_uint4(0, 0, 0, 0);
+    int l = 0;
+    uint64_t p = i;
+    while (p < len && !tok_space(t[p]) && l < KB) {
+      const unsigned char ch = t[p++];
+      if (ch <= 1) {  // escaped, as mrhbm_emit_str does it
+        rec.b[l++] = 1;
+        if (l < KB) rec.b[l++] = (unsigned char)(ch + 1);
+        else l = KB + 1;
+      } else {
+        rec.b[l++] = ch;
+      }
+    }
+    if (l >= KB || (p < len && !tok_space(t[p]))) {  // does not fit (one zero byte must remain): a host piece
+      atomicOr(o.flags, (uint32_t)ERRF_KEYLEN);
+      rec.b[KB - 1] = 0;
+      while (p < len && !tok_space(t[p])) p++;
+    }
+    while (p < len && t[p] != '\n' && tok_space(t[p])) p++;
+    const uint64_t s = p;
+    while (p < len && !tok_space(t[p])) p++;
+    const uint64_t ns = p - s;
+    while (p < len && t[p] != '\n' && tok_space(t[p])) p++;
+    DecScan d;
+    uint64_t bits = 0;
+    if (ns == 0 || (p < len && t[p] != '\n') || !dec_scan(t + s, ns, &d)) {  // not "key number"
+      atomicOr(o.flags, (uint32_t)ERRF_LINE);
+      atomicMin(o.flags + 1, (uint32_t)ls);
+    } else if (dec_to_bits(d, o.pow5, &bits) != DEC_EXACT) {  // the host rounds it and patches the 11 bytes
+      const uint32_t slot = atomicAdd(o.flags + 2, 1u);
+      if (slot < o.fix_cap) o.fix[slot] = make_uint4((uint32_t)idx, (uint32_t)s, (uint32_t)ns, 0);
+    }
+    unsigned char enc[kNumBytes];
+    num_encode(bits, enc);
+#pragma unroll
+    for (int k = 0; k < kNumBytes; k++) o.vals[idx * kNumBytes + k] = enc[k];
+    o.voff[idx + 1] = o.aoff + (idx + 1) * kNumBytes;
+    if (idx == 0) o.voff[0] = o.aoff;
+    rec.v[RB / 16 - 1].w = (uint32_t)(o.first + idx);
+    uint4* dst = o.recs + idx * (RB / 16);
+#pragma unroll
+    for (int v = 0; v < RB / 16; v++) dst[v] = rec.v[v];
+  }
+}
+// the host's values of the fix-up list: {pair index, double bits}
+__global__ void __launch_bounds__(256) k_kn_patch(const ulonglong2* __restrict__ fix, uint32_t n,
+                                                  unsigned char* __restrict__ vals) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const ulonglong2 f = fix[i];
+    unsigned char enc[kNumBytes];
+    num_encode(f.y, enc);
+#pragma unroll
+    for (int k = 0; k < kNumBytes; k++) vals[f.x * kNumBytes + k] = enc[k];
   }
 }
 
@@ -1604,6 +1709,29 @@ int launch_tok_emit(int rb, const unsigned char* text, uint64_t len, const uint3
     case 64: k_tok_emit<64><<<grid, 256, 0, s>>>(text, len, block_off, (uint4*)recs, value, flags); break;
     default: k_tok_emit<128><<<grid, 256, 0, s>>>(text, len, block_off, (uint4*)recs, value, flags); break;
   }
+  return 1;
+}
+int launch_kn_count(const unsigned char* text, uint64_t len, uint32_t* block_counts, cudaStream_t s) {
+  if (!len) return 0;
+  uint64_t nb = (len + 255) / 256;
+  k_kn_count<<<(int)std::min<uint64_t>(nb, (uint64_t)g_sm_count * 16), 256, 0, s>>>(text, len, block_counts);
+  return 1;
+}
+int launch_kn_emit(int rb, const unsigned char* text, uint64_t len, const uint32_t* block_off, const KnOut& o,
+                   cudaStream_t s) {
+  if (!len || rb == 16) return 0;
+  uint64_t nb = (len + 255) / 256;
+  int grid = (int)std::min<uint64_t>(nb, (uint64_t)g_sm_count * 16);
+  switch (rb) {
+    case 32: k_kn_emit<32><<<grid, 256, 0, s>>>(text, len, block_off, o); break;
+    case 64: k_kn_emit<64><<<grid, 256, 0, s>>>(text, len, block_off, o); break;
+    default: k_kn_emit<128><<<grid, 256, 0, s>>>(text, len, block_off, o); break;
+  }
+  return 1;
+}
+int launch_kn_patch(const void* fix, uint32_t n, unsigned char* vals, cudaStream_t s) {
+  if (!n) return 0;
+  k_kn_patch<<<(int)std::min<uint32_t>((n + 255) / 256, (uint32_t)g_sm_count * 4), 256, 0, s>>>((const ulonglong2*)fix, n, vals);
   return 1;
 }
 int launch_combine(const void* recs, uint64_t n, uint32_t* gtab, const GtabLayout& tab, uint32_t* flags, bool checked,

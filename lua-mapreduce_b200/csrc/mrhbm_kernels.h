@@ -94,7 +94,8 @@ MRHBM_HD inline uint32_t bin_count(const ShuffleBuffers& b, uint32_t bin) {
 }
 enum { CNT_NBIG = 0, CNT_TICKET = 1, CNT_ERR = 2, CNT_TOTAL = 3, CNT_GBIG = 4 };
 // ERRF_NOTNUM / ERRF_NAN (MRHBM_RED_FSUM): a value that is not a number encoding, a key whose sum is NaN
-enum { ERRF_SKEW = 1, ERRF_OVERFLOW = 2, ERRF_CAPACITY = 4, ERRF_KEYLEN = 8, ERRF_NOTNUM = 16, ERRF_NAN = 32 };
+// ERRF_LINE (mrhbm_map_key_numbers): a line that is not "key number"
+enum { ERRF_SKEW = 1, ERRF_OVERFLOW = 2, ERRF_CAPACITY = 4, ERRF_KEYLEN = 8, ERRF_NOTNUM = 16, ERRF_NAN = 32, ERRF_LINE = 64 };
 
 // every launcher returns the number of kernels it launched
 int launch_gen_u64(void* dst, uint64_t seed, uint64_t start, uint64_t n, cudaStream_t s);
@@ -123,6 +124,25 @@ int launch_tok_count(const unsigned char* text, uint64_t len, uint32_t* block_co
 int launch_tok_emit(int rb, const unsigned char* text, uint64_t len, const uint32_t* block_off, void* recs,
                     uint32_t value, uint32_t* flags, cudaStream_t s);
 inline uint64_t tok_blocks(uint64_t len) { return (len + 255) / 256; }
+// device-side key-number mapfn: first fields of lines per 256-byte block, then (after the same exclusive scan) one
+// record (key, value id first + i) and one 11-byte number per line.  flags[0] |= ERRF_KEYLEN for a key that exceeds
+// the key slot, ERRF_LINE for a malformed line, flags[1] = min over malformed lines of their start, flags[2] = the
+// tokens the host must round (the first fix_cap of them in fix[]: {pair index, token offset, token length, 0})
+struct KnOut {
+  uint4* recs;           // the piece's records
+  unsigned char* vals;   // arena + aoff: the piece's values, 11 bytes each
+  uint64_t* voff;        // voff + first
+  uint64_t first, aoff;  // the piece's first pool index and arena offset
+  const uint64_t* pow5;  // dec_pow5_table
+  uint4* fix;
+  uint32_t fix_cap;
+  uint32_t* flags;
+};
+int launch_kn_count(const unsigned char* text, uint64_t len, uint32_t* block_counts, cudaStream_t s);
+int launch_kn_emit(int rb, const unsigned char* text, uint64_t len, const uint32_t* block_off, const KnOut& o,
+                   cudaStream_t s);
+// fix[i] = {pair index, double bits}: the number's 11 bytes at vals + 11 * pair index
+int launch_kn_patch(const void* fix, uint32_t n, unsigned char* vals, cudaStream_t s);
 // The map-side combiner's global table for records of rb bytes: `nbuckets` buckets of one 32-byte L2 sector each,
 // two 16-byte short entries per bucket, then, for string records only, 2^long_log long entries of one record each.
 // A short key probes buckets linearly from bucket(hash), wrapping at nbuckets (not a power of two: the table is

@@ -276,7 +276,14 @@ function hbm.map_job(map_key)
     assert(byte_values, "hbm_mapfn = 'words_file' needs value_kind = 'bytes'")
     return assert(m:words_value(text, hbm.encode_value(value)))
   end
-  return emit, finish, words
+  -- a mapfn module declaring hbm_mapfn = "key_numbers_file" (value_kind = "bytes", string keys): the device parses the
+  -- file's lines "key number" -- emit(key, tonumber(number)) per line, decimal numbers only
+  local key_numbers = function(text)
+    assert(byte_values, "hbm_mapfn = 'key_numbers_file' needs value_kind = 'bytes'")
+    assert(not tuple_keys, "hbm_mapfn = 'key_numbers_file' needs string keys")
+    return assert(m:key_numbers(text))
+  end
+  return emit, finish, words, key_numbers
 end
 
 -- server_prepare_reduce (server.lua:279-329)

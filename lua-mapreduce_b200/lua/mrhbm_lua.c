@@ -202,6 +202,17 @@ static int map_words_value(lua_State *L) {
   lua_pushnumber(L, (lua_Number)n);
   return 1;
 }
+/* map:key_numbers(text) -> number of pairs, with values = "bytes" and string keys: every line "key number" of the
+ * text becomes (key, the number's value encoding), parsed on the device (a number sum's mapfn) */
+static int map_key_numbers(lua_State *L) {
+  lmap *m = (lmap *)luaL_checkudata(L, 1, MAP_MT);
+  size_t len;
+  const char *t = luaL_checklstring(L, 2, &len);
+  uint64_t n = 0;
+  if (!m->h || mrhbm_map_key_numbers(m->h, t, len, &n) != MRHBM_OK) return fail(L, m->ctx);
+  lua_pushnumber(L, (lua_Number)n);
+  return 1;
+}
 static int map_commit(lua_State *L) { /* job.lua:217-221: remove_file + build */
   lmap *m = (lmap *)luaL_checkudata(L, 1, MAP_MT);
   mrhbm_map *h = m->h;
@@ -330,7 +341,7 @@ static const luaL_Reg ctx_methods[] = {{"map_begin", ctx_map_begin}, {"shuffle",
                                        {"reset", ctx_reset}, {"set_splitters", ctx_set_splitters},
                                        {"sample_splitters", ctx_sample_splitters}, {"__gc", ctx_gc}, {NULL, NULL}};
 static const luaL_Reg map_methods[] = {{"emit", map_emit}, {"wordcount", map_wordcount},
-                                       {"words_value", map_words_value}, {"commit", map_commit},
+                                       {"words_value", map_words_value}, {"key_numbers", map_key_numbers}, {"commit", map_commit},
                                        {"abort", map_abort}, {"__gc", map_abort}, {NULL, NULL}};
 static const luaL_Reg mod_funcs[] = {{"new", l_new}, {NULL, NULL}};
 

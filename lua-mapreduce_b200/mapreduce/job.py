@@ -70,6 +70,11 @@ class Job:
                 with open(self.doc["value"], "rb") as fh:
                     m.words_value(fh.read(), tuple_keys.encode_value(self.doc["value"]))
                 mapfn = None
+            elif hbm_mapfn == "key_numbers_file" and hasattr(m, "key_numbers"):
+                # the job value is a file of lines "key number": the device parses them, emit(key, float(number))
+                with open(self.doc["value"], "rb") as fh:
+                    m.key_numbers(fh.read())
+                mapfn = None
             kind = cfg["hbm"]["key_kind"]
             if kind == "u64":
                 enc_key = int

@@ -217,6 +217,13 @@ class server:
         if getattr(mods["mapfn"], "hbm_mapfn", None) == "words_file" and hbm["value_kind"] != "bytes":
             raise ValueError("hbm_mapfn = 'words_file' pairs every word with the file name, a string value: "
                              "configure hbm = {'value_kind': 'bytes'}")
+        if getattr(mods["mapfn"], "hbm_mapfn", None) == "key_numbers_file":
+            if hbm["value_kind"] != "bytes":
+                raise ValueError("hbm_mapfn = 'key_numbers_file' pairs every key with a number, a byte value: "
+                                 "configure hbm = {'value_kind': 'bytes'}")
+            if hbm["key_kind"] != "str":  # the host mapfn's u64 or tuple keys would be encoded differently
+                raise ValueError("hbm_mapfn = 'key_numbers_file' emits the key field's bytes as a string key: it needs "
+                                 "key_kind = 'str', not %r" % (hbm["key_kind"],))
         if distinct:
             distinct_combiner(mods["combinerfn"], hbm["value_kind"])
         hbm.update(partitioner=_BUILTIN_PART[pname], num_partitions=nparts,

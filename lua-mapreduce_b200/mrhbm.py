@@ -59,6 +59,7 @@ EXPORTS = [
     "mrhbm_checksum_result", "mrhbm_stats_get", "mrhbm_reset", "mrhbm_comm_unique_id", "mrhbm_comm_init",
     "mrhbm_set_splitters", "mrhbm_sample_splitters", "mrhbm_emit_str_value", "mrhbm_emit_u64_value",
     "mrhbm_emit_batch_values", "mrhbm_groups_next_values", "mrhbm_result_values", "mrhbm_map_words_value",
+    "mrhbm_map_key_numbers",
 ]
 
 _lib = None
@@ -126,6 +127,7 @@ def load(build_if_missing=True):
     sig("mrhbm_groups_next_values", i, vp, C.POINTER(vp), C.POINTER(sz), C.POINTER(vp), C.POINTER(vp), C.POINTER(sz))
     sig("mrhbm_result_values", i, vp, vp, sz, vp, C.POINTER(sz))
     sig("mrhbm_map_words_value", i, vp, vp, sz, C.c_char_p, sz, C.POINTER(u64))
+    sig("mrhbm_map_key_numbers", i, vp, vp, sz, C.POINTER(u64))
     _lib = L
     return L
 
@@ -252,6 +254,15 @@ class Map:
         n = C.c_uint64()
         ptr, nbytes, keep = self._text(text, nbytes)
         self.ctx._chk(self.ctx.L.mrhbm_map_words_value(self.h, ptr, nbytes, v, len(v), C.byref(n)))
+        return n.value
+
+    def key_numbers(self, text, nbytes=None):
+        """F_BYTE_VALUES, string keys: every line "key number" of the text (text as for wordcount) becomes the pair
+        (key, tuple.encode_value(float(number))), parsed on the device (see mrhbm_map_key_numbers); returns the number
+        of pairs emitted"""
+        n = C.c_uint64()
+        ptr, nbytes, keep = self._text(text, nbytes)
+        self.ctx._chk(self.ctx.L.mrhbm_map_key_numbers(self.h, ptr, nbytes, C.byref(n)))
         return n.value
 
     def commit(self):
