@@ -19,20 +19,6 @@ namespace mrhbm {
 namespace {
 constexpr unsigned long long kEmpty = ~0ull;  // an entry's fingerprint and index before the claim (memset to 0xff)
 
-// 64-bit fingerprint of the key slot words and the value bytes (never kEmpty)
-template <int RB>
-__device__ __forceinline__ uint64_t fingerprint(const uint32_t* r, const ValView& v) {
-  uint64_t h = fp_step(0x5851F42D4C957F2Dull, v.len);
-#pragma unroll
-  for (int i = 0; i < Rec<RB>::kKeyWords; i += 2)
-    h = fp_step(h, (uint64_t)r[i] | (i + 1 < Rec<RB>::kKeyWords ? (uint64_t)r[i + 1] << 32 : 0ull));
-  const uint64_t nw = (v.len + 3) / 4;
-  for (uint64_t i = 0; i < nw; i += 2)
-    h = fp_step(h, (uint64_t)val_word(v, i) | (i + 1 < nw ? (uint64_t)val_word(v, i + 1) << 32 : 0ull));
-  h = mix64(h);
-  return h == kEmpty ? 0 : h;
-}
-
 // the record r (value id id, bytes v) against the record at q: equal key slots and equal value bytes
 template <int RB>
 __device__ __forceinline__ bool same_pair(const uint32_t* r, uint64_t id, const ValView& v, const uint32_t* __restrict__ q,
@@ -66,7 +52,7 @@ __global__ void __launch_bounds__(kDistinctTile) k_distinct_mark(const unsigned 
   load_record<RB>(pool, p, r);
   const uint64_t id = rec_value<RB>(r);
   const ValView v = val_view(arena, voff, id);
-  const uint64_t fp = fingerprint<RB>(r, v);
+  const uint64_t fp = pair_fingerprint<RB>(r, v);
   for (uint64_t s = fp & mask;; s = (s + 1) & mask) {
     unsigned long long* e = (unsigned long long*)&tab[s];
     unsigned long long f = *(volatile unsigned long long*)e;

@@ -5,6 +5,7 @@
 #include <cstdint>
 
 #include "mrhbm_dev.cuh"
+#include "mrhbm_valbytes.cuh"
 
 namespace mrhbm {
 
@@ -43,6 +44,21 @@ __host__ __device__ __forceinline__ uint64_t key_fingerprint(const uint32_t* r) 
 #pragma unroll
   for (int i = 0; i < Rec<RB>::kKeyWords; i += 2)
     h = fp_step(h, (uint64_t)r[i] | (i + 1 < Rec<RB>::kKeyWords ? (uint64_t)r[i + 1] << 32 : 0ull));
+  h = mix64(h);
+  return h == ~0ull ? 0 : h;
+}
+
+// MRHBM_COMBINE_DISTINCT's (and the distinct reducer's) 64-bit fingerprint of the key slot words and the value bytes
+// (never ~0, the empty entry); host-callable for tests/native/distinct_fingerprint_check.cu
+template <int RB>
+__host__ __device__ __forceinline__ uint64_t pair_fingerprint(const uint32_t* r, const ValView& v) {
+  uint64_t h = fp_step(0x5851F42D4C957F2Dull, v.len);
+#pragma unroll
+  for (int i = 0; i < Rec<RB>::kKeyWords; i += 2)
+    h = fp_step(h, (uint64_t)r[i] | (i + 1 < Rec<RB>::kKeyWords ? (uint64_t)r[i + 1] << 32 : 0ull));
+  const uint64_t nw = (v.len + 3) / 4;
+  for (uint64_t i = 0; i < nw; i += 2)
+    h = fp_step(h, (uint64_t)val_word(v, i) | (i + 1 < nw ? (uint64_t)val_word(v, i + 1) << 32 : 0ull));
   h = mix64(h);
   return h == ~0ull ? 0 : h;
 }
