@@ -112,7 +112,30 @@ enum {
    * bin of more rows than one shared-memory sort takes, key slot + 8 bytes per result row of merge scratch and, for
    * the groups that span a chunk of such a bin, partial accumulators of 1096 bytes per slot, 2 ceil(rows / cap) + 2
    * slots (cap = 32 KB / record bytes). */
-  MRHBM_RED_FSUM = 3
+  MRHBM_RED_FSUM = 3,
+  /* MRHBM_F_BYTE_VALUES only, with combiner MRHBM_COMBINE_NONE or MRHBM_COMBINE_DISTINCT (any other combination fails
+   * mrhbm_init with MRHBM_E_INVAL; one GPU, as byte values are): the reducefn "the number of distinct values of the
+   * key", COUNT(DISTINCT) -- unique visitors per page, the document frequency of a word, distinct sources per
+   * destination -- computed on the device, no host reducefn runs.  After mrhbm_shuffle there is exactly one row per
+   * key; its value is the number of distinct values among the key's committed pairs over all map jobs, encoded as the
+   * 11-byte number of MRHBM_RED_FSUM (the bytes of tuple.encode_value(float(n))).  Values are equal when their bytes
+   * are, exactly as in MRHBM_RED_DISTINCT: two emits of the same bytes under different value ids count once, the empty
+   * value counts as a value, the numbers 1 and 1.0 have the same encoding and count once, while -0 and +0 have
+   * different bytes and count twice.  Keys longer than the record class get the same count on the host, at their
+   * place in the key order.  The result does not depend on emission order, map jobs, bins, runs, the distinct
+   * combiner or any MRHBM_F_* layout flag: it is bit-identical across all of them.  Reading the result, as for
+   * MRHBM_RED_FSUM: mrhbm_groups_next_values gives every group, long keys included, its one encoded count;
+   * mrhbm_result_values gives one value per mrhbm_result_copy row, and the row's value field is the row index
+   * (mrhbm_groups_next fails, mrhbm_result_copy needs sums = NULL).  mrhbm_result_info: pairs_in = committed pairs,
+   * pairs_recv = distinct pairs the shuffle carried, groups = keys.  mrhbm_checksum_result's out[3..5] keep their
+   * meaning; in[0..2] == out[0..2] does not hold (a row holds a count, not a value id).  The dedupe (the distinct set
+   * of MRHBM_RED_DISTINCT, each surviving pair carrying the value 1) is timed in mrhbm_stats.ms_combine; the integer
+   * sum of those 1s per key runs through the stages of MRHBM_RED_SUM and is timed where they are, all inside ms_total.
+   * Hot keys cost what they cost MRHBM_RED_SUM: no value ordering runs.  Limits: fewer than 2^31 committed pairs per
+   * shuffle (else MRHBM_E_INVAL), so every count is exact in a double.  Extra device memory: the distinct set of
+   * MRHBM_RED_DISTINCT (16 bytes x a power of two >= 2 x pairs, plus 4 + record bytes per pair), and 11 bytes of value
+   * and 8 of offset per result row. */
+  MRHBM_RED_COUNT_DISTINCT = 4
 };
 
 /* built-in combinerfn, run on the map side (job.lua:92-96,198-202: reducing the combined values must give what
@@ -186,7 +209,7 @@ typedef struct mrhbm_config {
 #define MRHBM_F_NO_OPTIMISTIC 4u /* always run the exact two-pass (histogram) partition layout */
 /* Byte-string values (lua-mapreduce's emit(key, value) takes any Lua string or number, utils.lua:100-120): a value is
  * opaque bytes, 0 to 1 GiB long, carried through group-only mode.  Needs reducer = MRHBM_RED_NONE (or a byte-values
- * reducer: MRHBM_RED_DISTINCT, MRHBM_RED_FSUM) and combiner
+ * reducer: MRHBM_RED_DISTINCT, MRHBM_RED_FSUM, MRHBM_RED_COUNT_DISTINCT) and combiner
  * MRHBM_COMBINE_NONE or MRHBM_COMBINE_DISTINCT (else mrhbm_init fails with MRHBM_E_INVAL) and one GPU (mrhbm_comm_init with world > 1 fails).  On such a ctx:
  *   - pairs are emitted with mrhbm_emit_str_value / mrhbm_emit_u64_value / mrhbm_emit_batch_values /
  *     mrhbm_map_words_value / mrhbm_map_key_numbers; the integer-valued emits (emit_str, emit_u64, emit_batch, emit_device, map_gen_*,
@@ -197,7 +220,8 @@ typedef struct mrhbm_config {
  *     except that the pairs of one device piece of mrhbm_map_words_value share the id of the piece's first pair;
  *     fewer than 2^32 pairs may be emitted between mrhbm_reset calls, those of aborted and replaced jobs included.
  * The order of a key's values is unspecified with MRHBM_RED_NONE; MRHBM_RED_DISTINCT gives each key's distinct values
- * in ascending byte order; MRHBM_RED_FSUM gives each key one value, the exact sum of its numbers.  The new calls fail with MRHBM_E_INVAL on a ctx
+ * in ascending byte order; MRHBM_RED_FSUM gives each key one value, the exact sum of its numbers; MRHBM_RED_COUNT_DISTINCT
+ * gives each key one value, the number of its distinct values.  The new calls fail with MRHBM_E_INVAL on a ctx
  * without the flag. */
 #define MRHBM_F_BYTE_VALUES 8u
 

@@ -67,7 +67,7 @@ struct mrhbm_ctx {
   uint64_t *row_off = nullptr, *val_tile = nullptr, *val_pieces = nullptr;
   uint64_t cvals_cap = 0, row_cap = 0, tile_cap = 0, pieces_cap = 0, cvals_bytes = 0;
   std::vector<const std::string*> long_vals;  // values of the long-key groups (LongGroup::values index them)
-  std::deque<std::string> long_sums;          // MRHBM_RED_FSUM: the long-key groups' encoded sums (long_vals point here)
+  std::deque<std::string> long_sums;          // MRHBM_RED_FSUM / _COUNT_DISTINCT: the long-key groups' encoded results (long_vals point here)
   // Keys that do not fit a record slot (rare: the reference takes any key length, utils.lua:104-110) never reach the
   // device: their pairs wait on the host, per committed map job, are partitioned and grouped at the barrier (on several
   // GPUs after an all-gather) and merged into the reduce-side iteration at their place in the key order.
@@ -151,6 +151,9 @@ struct mrhbm_ctx {
   int64_t* ns_acc = nullptr;
   uint32_t *ns_flags = nullptr, *ns_head = nullptr;
   uint64_t ns_cap = 0;
+  // MRHBM_RED_COUNT_DISTINCT: the distinct set's survivors carry the value 1 through the integer sum of MRHBM_RED_SUM;
+  // the first result access encodes each key's count as a number (k_num_encode)
+  bool red_count = false;
   uint64_t N = 0, groups = 0;
   bool shuffled = false;
   std::vector<uint32_t> h_bin_off, h_uoff;
@@ -526,13 +529,14 @@ int ensure_compact(mrhbm_ctx* c) {
   if (rc) return rc;
   launch_compact(c->rb, c->rv, c->B, c->ckeys, c->csums, c->stream);
   CU(c, cudaGetLastError());
-  if (c->red_fsum) {
-    // every row's sum (double bits) is in csums: its 11-byte number at cvals[11 r ..), and the row index as its id
+  if (c->red_fsum || c->red_count) {
+    // every row's sum (double bits; MRHBM_RED_COUNT_DISTINCT: its integer count) is in csums: its 11-byte number at
+    // cvals[11 r ..), and the row index as its id
     const uint64_t n = c->groups;
     rc = grow(c, &c->row_cap, n + 1, n + 1, {{(void**)&c->row_off, sizeof(uint64_t)}});
     if (!rc) rc = grow(c, &c->cvals_cap, kNumBytes * n + 1, kNumBytes * n + 1, {{(void**)&c->cvals, 1}});
     if (rc) return rc;
-    launch_num_encode(c->csums, n, c->cvals, c->row_off, c->stream);
+    launch_num_encode(c->csums, n, c->cvals, c->row_off, c->stream, c->red_count);
     CU(c, cudaGetLastError());
     c->cvals_bytes = kNumBytes * n;
   } else if (c->bytevals) {
@@ -565,8 +569,10 @@ int ensure_compact(mrhbm_ctx* c) {
 // each distinct (key slot, value bytes) pair, in pool order, to dd_out.  off[t] receives the survivors before tile t
 // (off.back(): all of them); rg the ranges as the kernels saw them (rg[k].tbase: the first tile of range k).
 // `what` names the caller in the error of a set larger than it takes; *launches (optional) += kernels launched.
+// ones (MRHBM_RED_COUNT_DISTINCT): the survivors always go to dd_out, repeats or not, with their value field set to 1.
 int distinct_set(mrhbm_ctx* c, const std::vector<std::pair<uint64_t, uint64_t>>& ranges, const char* what,
-                 std::vector<DistinctRange>& rg, std::vector<uint32_t>& off, uint32_t* launches = nullptr) {
+                 std::vector<DistinctRange>& rg, std::vector<uint32_t>& off, uint32_t* launches = nullptr,
+                 bool ones = false) {
   cudaStream_t s = c->stream;
   rg.clear();
   uint64_t n = 0, nt = 0;
@@ -598,8 +604,8 @@ int distinct_set(mrhbm_ctx* c, const std::vector<std::pair<uint64_t, uint64_t>>&
   CU(c, cudaGetLastError());
   CU(c, cudaMemcpyAsync(off.data(), tile_off, (nt + 1) * 4, cudaMemcpyDeviceToHost, s));
   CU(c, cudaStreamSynchronize(s));
-  if (off[nt] < n) {
-    k += launch_distinct_scatter(c->rb, c->pool, drg, nr, (uint32_t)nt, c->dd_tab, c->dd_slot, tile_off, c->dd_out, s);
+  if (off[nt] < n || ones) {
+    k += launch_distinct_scatter(c->rb, c->pool, drg, nr, (uint32_t)nt, c->dd_tab, c->dd_slot, tile_off, c->dd_out, ones, s);
     CU(c, cudaGetLastError());
   }
   if (launches) *launches += k;
@@ -825,7 +831,7 @@ int mrhbm_init(const mrhbm_config* cfg, mrhbm_ctx** out) {
       return fail(c, MRHBM_E_INVAL, "string keys need partitioner FNV_LUA, WORDHASH or RANGE");
   } else
     return fail(c, MRHBM_E_INVAL, "unknown key_kind %u", cfg->key_kind);
-  if (cfg->reducer > MRHBM_RED_FSUM) return fail(c, MRHBM_E_INVAL, "unknown reducer %u", cfg->reducer);
+  if (cfg->reducer > MRHBM_RED_COUNT_DISTINCT) return fail(c, MRHBM_E_INVAL, "unknown reducer %u", cfg->reducer);
   if (cfg->combiner > MRHBM_COMBINE_FSUM) return fail(c, MRHBM_E_INVAL, "unknown combiner %u", cfg->combiner);
   if (cfg->combiner == MRHBM_COMBINE_FSUM && (!(cfg->flags & MRHBM_F_BYTE_VALUES) || cfg->reducer != MRHBM_RED_FSUM))
     return fail(c, MRHBM_E_INVAL, "combiner MRHBM_COMBINE_FSUM needs byte values (MRHBM_F_BYTE_VALUES) and reducer MRHBM_RED_FSUM");
@@ -837,12 +843,17 @@ int mrhbm_init(const mrhbm_config* cfg, mrhbm_ctx** out) {
   if (cfg->reducer == MRHBM_RED_FSUM && (!(cfg->flags & MRHBM_F_BYTE_VALUES) ||
                                          (cfg->combiner != MRHBM_COMBINE_NONE && cfg->combiner != MRHBM_COMBINE_FSUM)))
     return fail(c, MRHBM_E_INVAL, "reducer MRHBM_RED_FSUM needs byte values (MRHBM_F_BYTE_VALUES) and combiner MRHBM_COMBINE_NONE or MRHBM_COMBINE_FSUM");
+  if (cfg->reducer == MRHBM_RED_COUNT_DISTINCT && (!(cfg->flags & MRHBM_F_BYTE_VALUES) ||
+                                                   (cfg->combiner != MRHBM_COMBINE_NONE && cfg->combiner != MRHBM_COMBINE_DISTINCT)))
+    return fail(c, MRHBM_E_INVAL, "reducer MRHBM_RED_COUNT_DISTINCT needs byte values (MRHBM_F_BYTE_VALUES) and combiner MRHBM_COMBINE_NONE or MRHBM_COMBINE_DISTINCT");
   if ((cfg->flags & MRHBM_F_BYTE_VALUES) && (cfg->reducer == MRHBM_RED_SUM || cfg->combiner == MRHBM_COMBINE_REDUCER))
-    return fail(c, MRHBM_E_INVAL, "byte values (MRHBM_F_BYTE_VALUES) need reducer MRHBM_RED_NONE, MRHBM_RED_DISTINCT or MRHBM_RED_FSUM and combiner 0 or MRHBM_COMBINE_DISTINCT");
+    return fail(c, MRHBM_E_INVAL, "byte values (MRHBM_F_BYTE_VALUES) need reducer MRHBM_RED_NONE, MRHBM_RED_DISTINCT, MRHBM_RED_FSUM or MRHBM_RED_COUNT_DISTINCT and combiner 0 or MRHBM_COMBINE_DISTINCT");
   c->bytevals = c->led.byte_values = (cfg->flags & MRHBM_F_BYTE_VALUES) != 0;
   c->red_distinct = cfg->reducer == MRHBM_RED_DISTINCT;
   c->red_fsum = cfg->reducer == MRHBM_RED_FSUM;
-  c->sb.no_reduce = cfg->reducer != MRHBM_RED_SUM;
+  c->red_count = cfg->reducer == MRHBM_RED_COUNT_DISTINCT;
+  // (MRHBM_RED_COUNT_DISTINCT sums a 1 per distinct pair: the sort reduces as for MRHBM_RED_SUM)
+  c->sb.no_reduce = cfg->reducer != MRHBM_RED_SUM && !c->red_count;
   CU(c, cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
   if (cfg->partitioner == MRHBM_PART_RANGE && cfg->num_partitions == 1) {  // one key range, no splitters: its table now
     int rc = install_splitters(c, {});
@@ -1714,7 +1725,8 @@ struct Src {
 // shuffle: when a string key's sum does not fit the u32 value of a combined record (or one value is too large
 // for the table's state word), this shuffle hands on the raw pairs instead.  MRHBM_RED_DISTINCT: the first copy of
 // each distinct (key slot, value bytes) pair over all committed pairs (distinct_set), in the set's scratch; the pool
-// and the ledger stay as they are.  EV_START .. EV_CSTART.
+// and the ledger stay as they are.  MRHBM_RED_COUNT_DISTINCT: the same pairs, always in the scratch and each with the
+// value 1 (pool values are value ids, never summed).  EV_START .. EV_CSTART.
 int collect_sources(mrhbm_ctx* c, std::vector<Src>& srcs, uint64_t* N, mrhbm_stats& st) {
   srcs.clear();
   uint64_t n = 0;
@@ -1725,11 +1737,12 @@ int collect_sources(mrhbm_ctx* c, std::vector<Src>& srcs, uint64_t* N, mrhbm_sta
     n += r.second;
   }
   *N = n;
-  if (c->red_distinct) {
+  if (c->red_distinct || c->red_count) {
     std::vector<DistinctRange> rg;
     std::vector<uint32_t> off;
-    int rc = distinct_set(c, live, "distinct reducer: a shuffle of", rg, off, &st.launches);
-    if (rc || off.back() == n) return rc;
+    int rc = distinct_set(c, live, c->red_count ? "count-distinct reducer: a shuffle of" : "distinct reducer: a shuffle of",
+                          rg, off, &st.launches, c->red_count);
+    if (rc || (off.back() == n && !c->red_count)) return rc;
     srcs.assign(1, Src{(const char*)c->dd_out, off.back()});
     *N = off.back();
     return 0;
@@ -2429,7 +2442,7 @@ int build_long_groups(mrhbm_ctx* c) {
   }
   // group the pairs of the partitions this rank owns (partition p lives on rank p % G, slot p / G)
   std::vector<std::map<std::string, std::vector<uint64_t>>> acc(c->Pl);
-  const bool sum = !c->sb.no_reduce;
+  const bool sum = !c->sb.no_reduce && !c->red_count;  // (count distinct: the value indices, counted below)
   for (size_t w = 0; w + 3 <= all_blobs.size();) {
     const uint32_t klen = all_blobs[w];
     uint64_t v;
@@ -2461,6 +2474,17 @@ int build_long_groups(mrhbm_ctx* c) {
         }
         uint64_t bits;
         if (!acc_round(sum, &bits)) return fail(c, MRHBM_E_INVAL, "reducer MRHBM_RED_FSUM: a long key's sum is NaN (+inf and -inf)");
+        std::string& e = c->long_sums.emplace_back(kNumBytes, '\0');
+        num_encode(bits, (unsigned char*)&e[0]);
+        kv.second.assign(1, c->long_vals.size());
+        c->long_vals.push_back(&e);
+      }
+      if (c->red_count) {  // the number of the key's distinct value bytes, encoded as the device encodes it
+        std::set<std::string> seen;
+        for (uint64_t i : kv.second) seen.insert(*c->long_vals[i]);
+        const double n = (double)seen.size();
+        uint64_t bits;
+        memcpy(&bits, &n, 8);
         std::string& e = c->long_sums.emplace_back(kNumBytes, '\0');
         num_encode(bits, (unsigned char*)&e[0]);
         kv.second.assign(1, c->long_vals.size());
@@ -2507,6 +2531,8 @@ int mrhbm_shuffle(mrhbm_ctx* c) {
   if (N_in >= 0xfffffff0ull) return fail(c, MRHBM_E_INVAL, "more than 2^32 pairs on one GPU (%llu)", (unsigned long long)N_in);
   if (c->red_fsum && N_in >= (1ull << 31))  // (each accumulator digit takes fewer than 2^31 addends)
     return fail(c, MRHBM_E_INVAL, "reducer MRHBM_RED_FSUM: a shuffle of %llu pairs (limit 2^31)", (unsigned long long)N_in);
+  if (c->red_count && N_in >= (1ull << 31))  // (the distinct set's limit; every count is then exact in a double)
+    return fail(c, MRHBM_E_INVAL, "reducer MRHBM_RED_COUNT_DISTINCT: a shuffle of %llu pairs (limit 2^31)", (unsigned long long)N_in);
   if (c->cfg.partitioner == MRHBM_PART_RANGE && c->world == 1 && !c->spl_set)  // (several GPUs: at the first all-gather)
     return fail(c, MRHBM_E_INVAL, "MRHBM_PART_RANGE needs splitters: call mrhbm_set_splitters or mrhbm_sample_splitters");
   mrhbm_stats st{};

@@ -5,7 +5,8 @@
 //                       index to its own with atomicMin; it remembers the entry
 //   k_distinct_count    a record survives when it is its entry's minimum; survivors per tile of kTile records
 //   (launch_exscan of the tile counts)
-//   k_distinct_scatter  the survivors, whole records in pool order, to a scratch buffer at their tile's offset
+//   k_distinct_scatter  the survivors, whole records in pool order, to a scratch buffer at their tile's offset (for
+//                       MRHBM_RED_COUNT_DISTINCT with their value field set to 1)
 // The caller copies each range's survivors back to the range's start.  Records move as they are: value ids, voff and
 // the arena are not touched.
 #include <cstdint>
@@ -85,7 +86,9 @@ __global__ void __launch_bounds__(kDistinctTile) k_distinct_count(const Distinct
   if (threadIdx.x == 0) tile_cnt[blockIdx.x] = (uint32_t)n;
 }
 
-template <int RB>
+// ONES (MRHBM_RED_COUNT_DISTINCT): every survivor's value field becomes 1, so the shuffle's integer sum of a key's
+// rows is its count of distinct values; the existing callers keep the value ids.
+template <int RB, bool ONES>
 __global__ void __launch_bounds__(kDistinctTile) k_distinct_scatter(const unsigned char* __restrict__ pool,
                                                                     const DistinctRange* __restrict__ rg, uint32_t nr,
                                                                     const ulonglong2* __restrict__ tab,
@@ -99,7 +102,13 @@ __global__ void __launch_bounds__(kDistinctTile) k_distinct_scatter(const unsign
   const uint4* src = (const uint4*)(pool + p * RB);
   uint4* dst = (uint4*)(out + ((uint64_t)tile_off[blockIdx.x] + rank) * RB);
 #pragma unroll
-  for (int i = 0; i < Rec<RB>::kVec; i++) dst[i] = __ldg(src + i);
+  for (int i = 0; i < Rec<RB>::kVec - (ONES ? 1 : 0); i++) dst[i] = __ldg(src + i);
+  if constexpr (ONES) {  // the value field ends the record: the last vector's .z/.w for u64 keys, its .w for strings
+    uint4 last = __ldg(src + Rec<RB>::kVec - 1);
+    if constexpr (Rec<RB>::kU64) last.z = 1u;
+    last.w = Rec<RB>::kU64 ? 0u : 1u;
+    dst[Rec<RB>::kVec - 1] = last;
+  }
 }
 
 int launch_distinct_mark(int rb, const void* pool, const DistinctRange* rg, uint32_t nr, uint32_t ntiles,
@@ -125,18 +134,22 @@ int launch_distinct_count(const DistinctRange* rg, uint32_t nr, uint32_t ntiles,
 }
 
 int launch_distinct_scatter(int rb, const void* pool, const DistinctRange* rg, uint32_t nr, uint32_t ntiles,
-                            const void* tab, const uint32_t* slot_of, const uint32_t* tile_off, void* out,
+                            const void* tab, const uint32_t* slot_of, const uint32_t* tile_off, void* out, bool ones,
                             cudaStream_t s) {
   if (!ntiles) return 0;
   const unsigned char* P = (const unsigned char*)pool;
   const ulonglong2* T = (const ulonglong2*)tab;
   unsigned char* O = (unsigned char*)out;
+#define SCATTER(RB)                                                                                                   \
+  (ones ? k_distinct_scatter<RB, true><<<ntiles, kDistinctTile, 0, s>>>(P, rg, nr, T, slot_of, tile_off, O)            \
+        : k_distinct_scatter<RB, false><<<ntiles, kDistinctTile, 0, s>>>(P, rg, nr, T, slot_of, tile_off, O))
   switch (rb) {
-    case 16: k_distinct_scatter<16><<<ntiles, kDistinctTile, 0, s>>>(P, rg, nr, T, slot_of, tile_off, O); break;
-    case 32: k_distinct_scatter<32><<<ntiles, kDistinctTile, 0, s>>>(P, rg, nr, T, slot_of, tile_off, O); break;
-    case 64: k_distinct_scatter<64><<<ntiles, kDistinctTile, 0, s>>>(P, rg, nr, T, slot_of, tile_off, O); break;
-    default: k_distinct_scatter<128><<<ntiles, kDistinctTile, 0, s>>>(P, rg, nr, T, slot_of, tile_off, O); break;
+    case 16: SCATTER(16); break;
+    case 32: SCATTER(32); break;
+    case 64: SCATTER(64); break;
+    default: SCATTER(128); break;
   }
+#undef SCATTER
   return 1;
 }
 

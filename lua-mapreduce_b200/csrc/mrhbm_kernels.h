@@ -286,9 +286,10 @@ int launch_distinct_mark(int rb, const void* pool, const DistinctRange* rg, uint
 // tile_cnt[t] = the records of tile t that are the first copy of their pair
 int launch_distinct_count(const DistinctRange* rg, uint32_t nr, uint32_t ntiles, const void* tab, const uint32_t* slot_of,
                           uint32_t* tile_cnt, cudaStream_t s);
-// those records, in pool order, to out: tile t's at out[tile_off[t] ..) (tile_off: the exclusive scan of tile_cnt)
+// those records, in pool order, to out: tile t's at out[tile_off[t] ..) (tile_off: the exclusive scan of tile_cnt);
+// ones: with their value field set to 1 (MRHBM_RED_COUNT_DISTINCT), else as they are
 int launch_distinct_scatter(int rb, const void* pool, const DistinctRange* rg, uint32_t nr, uint32_t ntiles,
-                            const void* tab, const uint32_t* slot_of, const uint32_t* tile_off, void* out,
+                            const void* tab, const uint32_t* slot_of, const uint32_t* tile_off, void* out, bool ones,
                             cudaStream_t s);
 
 // ---- MRHBM_RED_DISTINCT (mrhbm_value_order.cu) ----
@@ -328,7 +329,9 @@ int launch_num_sum(int rb, const ShuffleBuffers& b, uint32_t nb, uint32_t nbig, 
                    const uint64_t* voff, const NumScratch& sc, cudaStream_t s);
 // compacted rows whose ids hold double bits -> row r's encoded number at vals[11 r ..), row_off[r] = 11 r (n + 1
 // entries), ids[r] = r
-int launch_num_encode(uint64_t* ids, uint64_t n, unsigned char* vals, uint64_t* row_off, cudaStream_t s);
+// counts: the ids hold integer counts instead (MRHBM_RED_COUNT_DISTINCT), each encoded as the number (double) it is
+int launch_num_encode(uint64_t* ids, uint64_t n, unsigned char* vals, uint64_t* row_off, cudaStream_t s,
+                      bool counts = false);
 
 // ---- MRHBM_COMBINE_FSUM (mrhbm_num_combine.cu) ----
 // One map job's records (DistinctRange, as the distinct combiner takes them) grouped by key slot and each key's numbers

@@ -304,13 +304,15 @@ __global__ void __launch_bounds__(kMergeThreads) k_num_key_merge(ShuffleBuffers 
   }
 }
 
-// Compacted rows (ids[r]: the sum's double bits) -> their encoded values: row r's 11 bytes at vals + 11 r, row_off[r] =
-// 11 r (n + 1 entries), and ids[r] = r, the row's value id.
+// Compacted rows (ids[r]: the sum's double bits; COUNTS: an integer count below 2^53, so exact as a double) -> their
+// encoded values: row r's 11 bytes at vals + 11 r, row_off[r] = 11 r (n + 1 entries), and ids[r] = r, the row's value id.
+template <bool COUNTS>
 __global__ void k_num_encode(uint64_t* ids, uint64_t n, unsigned char* vals, uint64_t* row_off) {
   for (uint64_t r = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; r <= n; r += (uint64_t)gridDim.x * blockDim.x) {
     row_off[r] = kNumBytes * r;
     if (r < n) {
-      num_encode(ids[r], vals + kNumBytes * r);
+      const uint64_t x = ids[r];
+      num_encode(COUNTS ? (uint64_t)__double_as_longlong((double)x) : x, vals + kNumBytes * r);
       ids[r] = r;
     }
   }
@@ -379,9 +381,12 @@ int launch_num_key_merge(int rb, const ShuffleBuffers& b, uint32_t nbig, uint32_
   return n;
 }
 
-int launch_num_encode(uint64_t* ids, uint64_t n, unsigned char* vals, uint64_t* row_off, cudaStream_t s) {
+int launch_num_encode(uint64_t* ids, uint64_t n, unsigned char* vals, uint64_t* row_off, cudaStream_t s, bool counts) {
   const uint64_t blocks = (n + 256) / 256 < 4096 ? (n + 256) / 256 : 4096;
-  k_num_encode<<<(unsigned)blocks, 256, 0, s>>>(ids, n, vals, row_off);
+  if (counts)
+    k_num_encode<true><<<(unsigned)blocks, 256, 0, s>>>(ids, n, vals, row_off);
+  else
+    k_num_encode<false><<<(unsigned)blocks, 256, 0, s>>>(ids, n, vals, row_off);
   return 1;
 }
 

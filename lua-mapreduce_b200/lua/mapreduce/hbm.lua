@@ -23,7 +23,9 @@ local hbm = { _VERSION = "0.1", _NAME = "mapreduce.hbm" }
 --     value_kind = "bytes" job: hbm_reducefn = "fsum" (its reducefn emits the sum of its number values; the device
 --     sums them exactly, rounds once, and hbm.groups hands out that one number), or hbm_reducefn = "distinct" (its
 --     reducefn emits the distinct values ascending by their
---     encoded bytes; the device computes them and hbm.groups hands them out as the reducefn's result)
+--     encoded bytes; the device computes them and hbm.groups hands them out as the reducefn's result), or
+--     hbm_reducefn = "count_distinct" (its reducefn emits the number of distinct values, a table used as a set then
+--     emit(n); the device counts them by their encoded bytes and hbm.groups hands out that one number)
 local ctx -- one context per worker process (job.lua keeps `funcs`/`initialized` per process too)
 local sample_splitters = false -- hbm_splitters = "sample": hbm.prepare_reduce samples them before the shuffle
 local tuple_keys = false -- hbm.configure(..., { key_kind = "tuple" }); an upvalue of configure, map_job and groups
@@ -48,13 +50,15 @@ function hbm.configure(partition_mod, reduce_mod, combiner_mod, opts)
   local builtin = reduce_mod.hbm_reducefn == "sum"
   local distinct_red = reduce_mod.hbm_reducefn == "distinct"
   local fsum_red = reduce_mod.hbm_reducefn == "fsum"
+  local count_red = reduce_mod.hbm_reducefn == "count_distinct"
   opts = opts or {}
   tuple_keys = opts.key_kind == "tuple" -- composite keys travel as encoded byte strings
   byte_values = opts.value_kind == "bytes" -- values travel as encoded byte strings (hbm.encode_value)
-  assert(not (byte_values and reduce_mod.hbm_reducefn ~= nil and not distinct_red and not fsum_red),
-         "value_kind = 'bytes' hands string and number values to a general reducefn: the reducefn must not declare an hbm_reducefn other than 'distinct' or 'fsum'")
+  assert(not (byte_values and reduce_mod.hbm_reducefn ~= nil and not distinct_red and not fsum_red and not count_red),
+         "value_kind = 'bytes' hands string and number values to a general reducefn: the reducefn must not declare an hbm_reducefn other than 'distinct', 'fsum' or 'count_distinct'")
   assert(not distinct_red or byte_values, "hbm_reducefn = 'distinct' needs value_kind = 'bytes'")
   assert(not fsum_red or byte_values, "hbm_reducefn = 'fsum' needs value_kind = 'bytes'")
+  assert(not count_red or byte_values, "hbm_reducefn = 'count_distinct' needs value_kind = 'bytes'")
   -- hbm_combinerfn = "fsum" (hbm_reducefn = "fsum"): each map job's numbers per key become the exact expansion of
   -- their sum at its commit (include/mrhbm.h, MRHBM_COMBINE_FSUM)
   local fsum_comb = combiner_mod ~= nil and combiner_mod.hbm_combinerfn == "fsum"
@@ -72,7 +76,8 @@ function hbm.configure(partition_mod, reduce_mod, combiner_mod, opts)
     num_partitions = assert(partition_mod.NUM_REDUCERS, "partitionfn module must expose NUM_REDUCERS"),
     partitioner = assert(partition_mod.hbm_partitionfn, "partitionfn module must declare hbm_partitionfn"),
     combiner = distinct and "distinct" or (fsum_comb and "fsum" or combiner_mod ~= nil),
-    reducer = builtin and "sum" or (distinct_red and "distinct" or (fsum_red and "fsum" or "none")),
+    reducer = builtin and "sum" or (distinct_red and "distinct" or (fsum_red and "fsum" or
+              (count_red and "count_distinct" or "none"))),
     device = opts.device,
     values = byte_values and "bytes" or "int",
   }

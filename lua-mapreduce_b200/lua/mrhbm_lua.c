@@ -37,11 +37,12 @@ static int fail(lua_State *L, mrhbm_ctx *c) { /* luamongo style: nil, msg */
 }
 
 /* mrhbm.new{ key_kind="str"|"u64", max_key_bytes=, num_partitions=, partitioner="fnv_lua"|"mulhash"|
- *            "wordhash"|"range", combiner=bool|"distinct"|"fsum", reducer="sum"|"none"|"distinct"|"fsum", device=,
- *            values="int"|"bytes" }
- * values = "bytes" (MRHBM_F_BYTE_VALUES, needs reducer = "none", "distinct" or "fsum"): m:emit takes string
- * values and ctx:groups yields tables of strings (reducer = "distinct": each key's distinct values, ascending;
- * reducer = "fsum": one value, the exact sum of the key's numbers) */
+ *            "wordhash"|"range", combiner=bool|"distinct"|"fsum", reducer="sum"|"none"|"distinct"|"fsum"|
+ *            "count_distinct", device=, values="int"|"bytes" }
+ * values = "bytes" (MRHBM_F_BYTE_VALUES, needs reducer = "none", "distinct", "fsum" or "count_distinct"): m:emit takes
+ * string values and ctx:groups yields tables of strings (reducer = "distinct": each key's distinct values, ascending;
+ * reducer = "fsum": one value, the exact sum of the key's numbers; reducer = "count_distinct": one value, the number
+ * of the key's distinct values) */
 static int l_new(lua_State *L) {
   mrhbm_config cfg;
   const char *s;
@@ -66,12 +67,14 @@ static int l_new(lua_State *L) {
                : lua_toboolean(L, -1) ? MRHBM_COMBINE_REDUCER : MRHBM_COMBINE_NONE;
   lua_getfield(L, 1, "device");
   cfg.device = (int32_t)luaL_optinteger(L, -1, -1);
-  lua_getfield(L, 1, "reducer"); /* "sum" (built-in) | "none" (general reducefn on the host) | "distinct" | "fsum" */
+  lua_getfield(L, 1, "reducer"); /* "sum" (built-in) | "none" (general reducefn on the host) | "distinct" | "fsum" |
+                                    "count_distinct" */
   s = luaL_optstring(L, -1, "sum");
-  cfg.reducer = strcmp(s, "none") == 0       ? MRHBM_RED_NONE
-                : strcmp(s, "distinct") == 0 ? MRHBM_RED_DISTINCT
-                : strcmp(s, "fsum") == 0     ? MRHBM_RED_FSUM
-                                             : MRHBM_RED_SUM;
+  cfg.reducer = strcmp(s, "none") == 0             ? MRHBM_RED_NONE
+                : strcmp(s, "distinct") == 0       ? MRHBM_RED_DISTINCT
+                : strcmp(s, "fsum") == 0           ? MRHBM_RED_FSUM
+                : strcmp(s, "count_distinct") == 0 ? MRHBM_RED_COUNT_DISTINCT
+                                                   : MRHBM_RED_SUM;
   lua_getfield(L, 1, "values");
   s = luaL_optstring(L, -1, "int");
   if (strcmp(s, "bytes") == 0) cfg.flags |= MRHBM_F_BYTE_VALUES;

@@ -131,16 +131,17 @@ class Job:
                 ks = [x.replace(b"\x01\x01", b"\x00").replace(b"\x01\x02", b"\x01") if b"\x01" in x else x for x in ks]
         return [(kk, [vv]) for kk, vv in zip(ks, v.tolist())]
 
-    def _bulk_fsum(self, part):
-        """hbm_reducefn = "fsum": [(key, [sum])] of one partition in ascending key order from one bulk copy of the
-        shuffle's keys and values (mrhbm_result_copy + mrhbm_result_values, cached on the board per shuffle), the
-        device's single value per key handed out as the reducefn's result.  None when the ctx offers no bulk access
-        (keys longer than a result slot, test stand-ins): the iterator gives the same values."""
+    def _bulk_numbers(self, part):
+        """hbm_reducefn = "fsum" or "count_distinct": [(key, [number])] of one partition in ascending key order from
+        one bulk copy of the shuffle's keys and values (mrhbm_result_copy + mrhbm_result_values, cached on the board
+        per shuffle), the device's single number per key (a sum, or a count of distinct values) handed out as the
+        reducefn's result.  None when the ctx offers no bulk access (keys longer than a result slot, test stand-ins):
+        the iterator gives the same values."""
         import numpy as np
         b, ctx = self.board, self.board.ctx
         if not hasattr(ctx, "result_values"):
             return None
-        cache = getattr(b, "_bulk_fsum", None)
+        cache = getattr(b, "_bulk_numbers", None)
         if cache is None or cache[0] is not ctx or cache[1] != b.iteration:
             try:
                 keys, _, po = ctx.result_copy()
@@ -148,9 +149,9 @@ class Job:
             except Exception as e:
                 if getattr(e, "code", None) != -4:  # MRHBM_E_KEY
                     raise
-                b._bulk_fsum = (ctx, b.iteration, None, None, None, False)
+                b._bulk_numbers = (ctx, b.iteration, None, None, None, False)
                 return None
-            cache = b._bulk_fsum = (ctx, b.iteration, keys, blob, po, bool(ctx.result_info().sorted))
+            cache = b._bulk_numbers = (ctx, b.iteration, keys, blob, po, bool(ctx.result_info().sorted))
         _, _, keys, blob, po, is_sorted = cache
         if keys is None:
             return None
@@ -192,14 +193,16 @@ class Job:
         decode = tuple_keys.decode if cfg["hbm"]["key_kind"] == "tuple" else None
         byte_values = cfg["hbm"].get("value_kind") == "bytes"
         device_distinct = cfg["hbm"].get("reducer") == 2  # hbm_reducefn = "distinct": the values are its output
-        if cfg["hbm"].get("reducer") == 3 and decode is None:  # hbm_reducefn = "fsum": one number per key, in bulk
-            fsum = self._bulk_fsum(part)
-            if fsum is not None:
-                self.doc["value"]["pairs"] = fsum
+        # hbm_reducefn = "fsum" or "count_distinct": one number per key, in bulk
+        one_number = cfg["hbm"].get("reducer") in (3, 4)
+        if one_number and decode is None:
+            numbers = self._bulk_numbers(part)
+            if numbers is not None:
+                self.doc["value"]["pairs"] = numbers
                 self.written = True
                 self.board.mark(self.doc, STATUS.WRITTEN, written_time=time.time(), real_time=time.time() - self.t)
                 return
-        device_distinct |= cfg["hbm"].get("reducer") == 3  # (tuple keys, long keys: the iterator's one value per key)
+        device_distinct |= one_number  # (tuple keys, long keys: the iterator's one value per key)
         bulk = self._bulk_groups(part) if (aci and cfg["hbm"].get("reducer", 0) == 0 and decode is None) else None
         if bulk is not None:
             # built-in reducer + ACI flags: every value list is the singleton the device produced and the reference

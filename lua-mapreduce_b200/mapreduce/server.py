@@ -130,6 +130,28 @@ def distinct_reducer(red, value_kind):
                              "computes" % (values, out))
 
 
+def count_distinct_reducer(red, value_kind):
+    """Checks a reducefn module that declares hbm_reducefn = "count_distinct": the device then hands every key the
+    number of its distinct values (compared by their encoded bytes), and the reducefn is not called, so it must emit
+    exactly that one number."""
+    from .tuple import encode_value
+    if value_kind != "bytes":
+        raise ValueError("hbm_reducefn = 'count_distinct' compares string and number values by their bytes: "
+                         "configure hbm = {'value_kind': 'bytes'}")
+    for values in _DISTINCT_PROBES:
+        out = []
+        try:
+            red.reducefn(b"probe", list(values), out.append)
+        except Exception as e:
+            raise ValueError("hbm_reducefn = 'count_distinct': reducefn failed on the values %r: %r" % (values, e))
+        want = len({encode_value(v) for v in values})
+        ok = len(out) == 1 and isinstance(out[0], (int, float)) and not isinstance(out[0], bool) and out[0] == want
+        if not ok:
+            raise ValueError("hbm_reducefn = 'count_distinct', but reducefn turns the values %r into %r instead of "
+                             "the number of their distinct values, %d: the declaration must describe what the reducefn "
+                             "computes" % (values, out, want))
+
+
 class server:
     def __init__(self, connection_string, dbname, auth_table=None):
         self.cnn_string, self.dbname = connection_string, dbname
@@ -169,8 +191,9 @@ class server:
         # associative/commutative/idempotent flags, examples/WordCount/reducefn.lua:10-14)
         red, part = mods["reducefn"], mods["partitionfn"]
         builtin_red = getattr(red, "hbm_reducefn", None)
-        if builtin_red not in (None, "sum", "distinct", "fsum"):
-            raise NotImplementedError("unknown hbm_reducefn %r (built-ins: 'sum', 'distinct', 'fsum')" % (builtin_red,))
+        if builtin_red not in (None, "sum", "distinct", "fsum", "count_distinct"):
+            raise NotImplementedError("unknown hbm_reducefn %r (built-ins: 'sum', 'distinct', 'fsum', 'count_distinct')"
+                                      % (builtin_red,))
         # no declaration = general reducer: the device partitions, sorts and groups, reducefn runs
         # on the host per group (job.lua:264-284); values are unsigned integers < 2^32
         # A combinerfn only ever runs on the device, as the declared built-in (it must equal the reducefn there).
@@ -203,10 +226,10 @@ class server:
             raise ValueError("hbm value_kind must be 'int' or 'bytes', got %r" % (hbm["value_kind"],))
         if fsum_comb:
             fsum_combiner(mods["combinerfn"], builtin_red, hbm["value_kind"])
-        if hbm["value_kind"] == "bytes" and builtin_red not in (None, "distinct", "fsum"):
+        if hbm["value_kind"] == "bytes" and builtin_red not in (None, "distinct", "fsum", "count_distinct"):
             raise ValueError("hbm value_kind = 'bytes' hands string and number values to a general reducefn: "
-                             "the reducefn module must not declare an hbm_reducefn other than 'distinct' or 'fsum' (it "
-                             "declares %r)" % (builtin_red,))
+                             "the reducefn module must not declare an hbm_reducefn other than 'distinct', 'fsum' or "
+                             "'count_distinct' (it declares %r)" % (builtin_red,))
         if builtin_red == "distinct":  # every key's distinct values, ascending, on the device: reducefn is not called
             distinct_reducer(red, hbm["value_kind"])
         if builtin_red == "fsum":  # every key's numbers summed exactly on the device: reducefn is not called
@@ -214,6 +237,8 @@ class server:
             if distinct:  # a device combiner would drop repeated values before they are summed
                 raise ValueError("hbm_reducefn = 'fsum' takes no device combiner: the combinerfn module declares "
                                  "hbm_combinerfn = %r" % (mods["combinerfn"].hbm_combinerfn,))
+        if builtin_red == "count_distinct":  # every key's number of distinct values, on the device: reducefn is not called
+            count_distinct_reducer(red, hbm["value_kind"])
         if getattr(mods["mapfn"], "hbm_mapfn", None) == "words_file" and hbm["value_kind"] != "bytes":
             raise ValueError("hbm_mapfn = 'words_file' pairs every word with the file name, a string value: "
                              "configure hbm = {'value_kind': 'bytes'}")
@@ -228,7 +253,7 @@ class server:
             distinct_combiner(mods["combinerfn"], hbm["value_kind"])
         hbm.update(partitioner=_BUILTIN_PART[pname], num_partitions=nparts,
                    combiner="distinct" if distinct else "fsum" if fsum_comb else device_combiner,
-                   reducer={"sum": 0, "distinct": 2, "fsum": 3}.get(builtin_red, 1),
+                   reducer={"sum": 0, "distinct": 2, "fsum": 3, "count_distinct": 4}.get(builtin_red, 1),
                    splitters=range_splitters(part, nparts, hbm["key_kind"]) if pname == "range" else None)
         self.config = dict(mapfn=params["mapfn"], reducefn=params["reducefn"], partitionfn=params["partitionfn"],
                            combinerfn=params.get("combinerfn"), init_args=self.init_args,

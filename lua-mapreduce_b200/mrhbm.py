@@ -12,7 +12,7 @@ from . import build as _build
 
 KEY_U64, KEY_STR = 0, 1
 PART_FNV_LUA, PART_MULHASH, PART_WORDHASH, PART_RANGE = 0, 1, 2, 3
-RED_SUM, RED_NONE, RED_DISTINCT, RED_FSUM = 0, 1, 2, 3
+RED_SUM, RED_NONE, RED_DISTINCT, RED_FSUM, RED_COUNT_DISTINCT = 0, 1, 2, 3, 4
 COMBINE_NONE, COMBINE_REDUCER, COMBINE_DISTINCT, COMBINE_FSUM = 0, 1, 2, 3
 F_FORCE_RUNS, F_SMALL_BINS, F_NO_OPTIMISTIC, F_BYTE_VALUES = 1, 2, 4, 8
 E_NODEVICE = -8
